@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""bench.py — images/sec of the FasterViT hot path on B200 (see the contract in the task statement).
+"""bench.py — images/sec of the FasterViT hot path on an H100 (sm_90a).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload fv0_fwd] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload fv0_fwd] [--impl reference] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one synthetic batch. Default workload = BASELINE.json
 configs[1]: faster_vit_0_224 forward-only, batch 256 per GPU (random-init weights, synthetic N(0,1)
@@ -45,7 +45,7 @@ WORKLOADS = {
     # inside the captured step + the row-scale epilogues, same FLOPs
     "fv4_train_droppath": ("faster_vit_4_224", {}, 128, (224, 224), "train"),
     "fv0_fwd_b8": ("faster_vit_0_224", {}, 8, (224, 224), "fwd"),
-    "fv4_21k_384_train": ("faster_vit_4_21k_384", dict(drop_path_rate=0.0), 32, (384, 384), "train"),
+    "fv4_21k_384_train": ("faster_vit_4_21k_384", dict(drop_path_rate=0.0), 16, (384, 384), "train"),  # fits 80 GB
 }
 ORACLE_CASE = {"fv0_fwd": "fv0", "fv4_fwd": "fv4", "ar0_fwd": "ar0", "fv0_train": "fv0", "fv4_train": "fv4"}
 # algorithmic forward GFLOP per image (BASELINE.md §2, measured on the reference with FlopCounterMode)
@@ -63,11 +63,12 @@ def peaks() -> dict:
     if p.exists():
         d = json.loads(p.read_text())
         return dict(tensor=float(d["bf16_tflops_sustained"]), hbm=float(d["hbm_gbs"]), src="measured")
-    return dict(tensor=1400.0, hbm=6650.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 989 TFLOP/s dense FP16 / BF16, 3.35 TB/s HBM3 -- not reached figures
+    return dict(tensor=989.0, hbm=3350.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi sampler (B200_PROFILING.md 'clocks line'). It is started before the warm-up steps (nvidia-smi needs
+    """nvidia-smi sampler of the SM clock during the timed steps. It is started before the warm-up steps (nvidia-smi needs
     ~1 s before its first sample) and every line is time-stamped on arrival; `stop()` reports the samples that fall
     inside the timed region [mark_begin, mark_end]. If the timed region is too short to hold two samples, the
     samples of the warm-up + timed period (the GPU is under the same load) are used and `window` says so."""
@@ -188,8 +189,11 @@ def quick_measure(workload: str, dev, pk: dict, steps: int = 8, warmup: int = 3)
     """One more BASELINE config measured in the same process (device-resident rotating inputs, CUDA events over
     `steps` steps after `warmup`), with the GEMM kernel's share and roofline fraction from the per-launch table.
     Used for the `also_measured` block so that the driver-run record covers every single-GPU config."""
+    import gc
     import fastervit_b200 as F
     entry, kwargs, batch, hw, mode = WORKLOADS[workload]
+    gc.collect()   # the previous workload's plans (CUDA graphs and their memory pools) sit in reference cycles
+    torch.cuda.empty_cache()
     torch.manual_seed(0)
     model = F.create_model(entry, **kwargs).to(dev)
     model = model.train() if mode == "train" else model.eval()
@@ -250,6 +254,7 @@ def quick_measure(workload: str, dev, pk: dict, steps: int = 8, warmup: int = 3)
         out["latency_ms"] = {"median": round(lat[len(lat) // 2], 4), "p10": round(lat[3], 4), "p90": round(lat[26], 4),
                              "what": "wall clock of one synchronous model(x) call, 30 calls"}
     del plan, model, xs
+    gc.collect()
     torch.cuda.empty_cache()
     return out
 
@@ -304,6 +309,24 @@ def optimizer_leg(model, x, targets, pk) -> dict:
             "params": n_params, "bound": "hbm", "peak_gbs": pk["hbm"], **out}
 
 
+def dump_outputs(out_dir: Path, model, last: dict, mode: str, n_grad: int = 1 << 21) -> None:
+    """What the last timed step handed its caller: the logits, and for a training step the loss and the parameter
+    gradients. The gradients are sampled: n_grad positions of the concatenated gradients (model.parameters() order)
+    drawn with a fixed seed, stored with their positions, so two builds can be compared element for element."""
+    import numpy as np
+    out_dir.mkdir(parents=True, exist_ok=True)
+    np.save(out_dir / "logits.npy", last["logits"].float().cpu().numpy())
+    if mode == "train":
+        np.save(out_dir / "loss.npy", last["loss"].double().cpu().numpy().reshape(1))
+        grads = [p.grad.detach().reshape(-1).float() if p.grad is not None else torch.zeros(p.numel(), device=p.device)
+                 for p in model.parameters()]
+        flat = torch.cat(grads)
+        n = min(n_grad, flat.numel())
+        idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(1234))[:n].sort().values
+        np.save(out_dir / "grad_sample.npy", flat[idx.to(flat.device)].cpu().numpy())
+        np.save(out_dir / "grad_sample_index.npy", idx.double().numpy())
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -316,6 +339,10 @@ def main() -> None:
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-also", action="store_true", help="skip the also_measured block (other BASELINE configs)")
     ap.add_argument("--profile-out", default="", help="write the per-launch timing table (JSON) here")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32 / "
+                         "float64): logits, and for training the loss and a fixed, seeded sample of the parameter "
+                         "gradients")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -341,10 +368,10 @@ def main() -> None:
         # the config this arm really ran: the same model / mode / input shape / metric (img/s is batch-normalised), but
         # each step is a bounded sample of the workload -- a small batch on the host cores -- and it says so
         config = {"workload": f"{entry} {what}, 3x{hw[0]}x{hw[1]} synthetic N(0,1), random-init weights; CPU sample: "
-                              f"batch {r['batch']} per step on {r['cores']} host threads (the B200 arm runs batch "
+                              f"batch {r['batch']} per step on {r['cores']} host threads (the GPU arm runs batch "
                               f"{batch}/GPU; a full batch is ~1 min per step on these cores)",
                   "global_batch": r["batch"], "parallelism": f"{r['cores']} CPU threads, 1 process",
-                  "sample_of": f"batch {batch}/GPU workload of the B200 arm", "l2": "n/a (CPU)"}
+                  "sample_of": f"batch {batch}/GPU workload of the GPU arm", "l2": "n/a (CPU)"}
         line = {"impl": "reference", "metric": "images/sec", "value": r["value"], "unit": "img/s",
                 "n_gpus": args.gpus, "steps": r["steps_done"], "warmup": args.warmup,
                 "ms_per_step": r["ms_per_step"], "higher_is_better": True, "scaling": "weak",
@@ -355,9 +382,9 @@ def main() -> None:
         print(json.dumps(line))
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback; use --impl reference)")
+        raise SystemExit("bench.py: no CUDA device (the CUDA path has no CPU fallback; use --impl reference)")
     import fastervit_b200 as F
     from fastervit_b200 import lib as L
     torch.cuda.set_device(local_rank)
@@ -368,7 +395,7 @@ def main() -> None:
         if os.environ.get("NCCL_DEBUG", "").upper() == "VERSION":
             os.environ["NCCL_DEBUG"] = "WARN"   # keep NCCL's version banner off stdout (one JSON line contract)
         # NCCL's CTAs cannot share an SM with a GEMM CTA: keep their number small and known, the backward launches in
-        # the shadow of an all-reduce are capped to 148 - FVIT_NCCL_CTAS SMs (engine_train._allreduce_shadow)
+        # the shadow of an all-reduce are capped to (SM count) - FVIT_NCCL_CTAS SMs (engine_train._allreduce_shadow)
         os.environ.setdefault("NCCL_MAX_CTAS", os.environ.get("FVIT_NCCL_CTAS", "16"))
         dist.init_process_group("nccl", device_id=dev)
 
@@ -389,13 +416,22 @@ def main() -> None:
 
     targets = torch.randint(0, 1000, (batch,), device=dev, generator=g)
 
-    def step(xb):
+    last = {}
+
+    def step(xb, keep=False):
         if mode == "train":
-            loss = torch.nn.functional.cross_entropy(model(xb), targets)
+            logits = model(xb)
+            loss = torch.nn.functional.cross_entropy(logits, targets)
             loss.backward()
-            model.zero_grad(set_to_none=True)
+            if keep:   # the last timed step: its gradients stay in place for --dump-outputs
+                last.update(logits=logits.detach(), loss=loss.detach())
+            else:
+                model.zero_grad(set_to_none=True)
             return loss
-        return model(xb)
+        out = model(xb)
+        if keep:
+            last["logits"] = out
+        return out
 
     sampler = ClockSampler(local_rank)
     sampler.start()   # before the warm-up: nvidia-smi takes about a second to deliver its first sample
@@ -408,13 +444,17 @@ def main() -> None:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for i in range(args.steps):
-            out = step(xs[i % nbuf])
+            out = step(xs[i % nbuf], keep=bool(args.dump_outputs) and i == args.steps - 1)
         e1.record()
         sync_all()
         sampler.mark_end()
         launches = L.launch_count()
         ms = e0.elapsed_time(e1)
         clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(Path(args.dump_outputs), model, last, mode)
+    if mode == "train":
+        model.zero_grad(set_to_none=True)
     t = torch.tensor([ms], device=dev)
     if dist is not None:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -501,25 +541,14 @@ def main() -> None:
         gm = by.get("fvit_gemm")
         prof_table = {k: dict(ms=round(v["ms"], 4), launches=v["n"], share=round(v["ms"] / tot, 4),
                               gflop=round(v["flops"] / 1e9, 3)) for k, v in sorted(by.items(), key=lambda kv: -kv[1]["ms"])}
-        traffic, traffic_src = None, None   # DRAM bytes per GEMM launch from the newest committed ncu launch list
-        for tf in sorted((ROOT / "profiles").glob("r*_traffic.json"), reverse=True):
-            try:
-                traffic = json.loads(tf.read_text()).get(args.workload, {}).get("gemm_dram_bytes_per_launch")
-            except (OSError, ValueError):
-                traffic = None
-            if traffic is not None:
-                traffic_src = f"profiles/{tf.name}"
-                break
         if gm:
             ach = gm["flops"] / (gm["ms"] / 1e3) / 1e12
-            roofline = {"kernel": "gemm_tcgen05_kernel (fvit_gemm: conv taps + linear layers; fwd, dgrad and wgrad launches)",
+            roofline = {"kernel": "gemm_wgmma_kernel (fvit_gemm: conv taps + linear layers; fwd, dgrad and wgrad launches)",
                         "bound": "tensor",
                         "achieved": round(ach, 2), "peak": pk["tensor"], "unit": "TFLOP/s",
                         "frac": round(ach / pk["tensor"], 4),
-                        "traffic": None if traffic is None else round(traffic),
-                        "traffic_unit": (f"DRAM bytes per launch (ncu dram__bytes_read+write, {traffic_src})" if traffic_src
-                                         else "no ncu launch list with DRAM bytes committed for this workload"),
-                        "peak_source": f"{pk['src']} bf16 dense sustained (MEASURED_PEAKS.json)",
+                        "traffic": None, "traffic_unit": "DRAM bytes per launch: not measured",
+                        "peak_source": f"{pk['src']} (bf16 dense)",
                         "launches_per_step": gm["n"], "avg_launch_ms": round(gm["ms"] / gm["n"], 5),
                         "alg_gflop_per_launch": round(gm["flops"] / gm["n"] / 1e9, 3),
                         "share_of_step": round(gm["ms"] / tot, 4)}

@@ -1,4 +1,4 @@
-"""fastervit_b200 — B200-native (sm_100a) FasterViT forward/backward behind the reference's API.
+"""fastervit_b200 — H100-native (sm_90a) FasterViT forward/backward behind the reference's API.
 
     from fastervit_b200 import create_model
     model = create_model('faster_vit_0_224').cuda().eval()

@@ -4,7 +4,7 @@ level's Downsample (`xo`, fastervit.py:705-709), one BatchNorm2d `norm{i}` per r
 `forward_raw(x) -> tuple of [B, C_i, H_i, W_i]`, `forward(tensors, mask) -> {idx: (features, mask)}` with the padding
 mask resized to every level (fastervit.py:829-846), frozen stages (fastervit.py:803-815).
 
-The hot path is the same sm_100a launch list as classification: the wrapped model's eval plan is run up to the points
+The hot path is the same sm_90a launch list as classification: the wrapped model's eval plan is run up to the points
 where the level outputs are live and `fvit_feature_map_fwd` applies the level's folded BatchNorm while converting the
 token-major activation to NCHW. Variable input sizes go through the any-res entrypoints (one cached plan per shape; the
 level geometry is padded to window multiples exactly as faster_vit_any_res.py:851-867 does).

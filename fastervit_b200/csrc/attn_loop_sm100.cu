@@ -3,18 +3,18 @@
 // sequences longer than one 128-row tile.
 //
 // Work item = (window, head, tile of 128 query rows). Keys are visited in tiles of 128, twice:
-//   pass 1: S_j = Q K_j^T (tcgen05, 128 x 128 fp32 in TMEM)  -> running row maximum of S_j*scale + bias
+//   pass 1: S_j = Q K_j^T (wgmma, 128 x 128 fp32 in a shared-memory tile) -> running row maximum of S_j*scale + bias
 //   pass 2: S_j again, P_j = exp2(S_j*scale*log2e + bias*log2e - max) as fp16 into the swizzled operand tile,
-//           O += P_j V_j (TMEM accumulator over the key tiles), row sums of the rounded probabilities
+//           O += P_j V_j (fp32 shared-memory accumulator over the key tiles), row sums of the rounded probabilities
 // so no accumulator is ever rescaled; the score recomputation is 2*S*S*hd FLOPs of a contraction that is < 3 % of
 // the model. Scores / probabilities never touch HBM.
 //
-//   warp 0     : TMA producer  — Q tile, K / V tiles through a 4-stage ring, relative-position-bias tiles
-//                (fp32 [128 rows x 64 keys] units, two 128B-swizzled boxes each) through a 3-stage ring
-//   warp 1     : MMA issuer    — score MMAs double-buffered in TMEM so S_{j+1} is in flight while the softmax
-//                warps work on S_j; O accumulates in a third TMEM region
-//   warps 2..5 : softmax       — one thread per query row (tcgen05.ld, bias from shared memory, exp2, P store),
-//                then the O epilogue (1 / rowsum, fp16, 16-byte stores) and the optional log-sum-exp row vector
+//   warp 4     : TMA producer  — Q tile, K / V tiles through a 2-stage ring, relative-position-bias tiles
+//                (fp32 [128 rows x 32 keys] units, one 128B-swizzled box each) through a 2-stage ring, all in the
+//                order the compute warpgroup consumes them
+//   warps 0..3 : one warpgroup — the score and P V MMAs (wgmma, two m64 halves), softmax with one thread per query
+//                row (bias from shared memory, exp2, P store), then the O epilogue (1 / rowsum, fp16, 16-byte
+//                stores) and the optional log-sum-exp row vector
 #include <cuda_fp16.h>
 
 #include "../../include/fvit.h"
@@ -23,11 +23,13 @@
 
 namespace fvit {
 
-constexpr int AL_THREADS = 192;
+constexpr int AL_THREADS = 160;
 constexpr int AL_ROWS = 128;
-constexpr int AL_NKV = 4;    // K / V tile ring depth
-constexpr int AL_NB = 3;     // bias unit ring depth
-constexpr int AL_BUNIT = 64; // key columns per bias unit
+constexpr int AL_PRODUCER = 4;  // the TMA warp; warps 0..3 are the compute warpgroup
+constexpr int AL_NKV = 2;       // K / V tile ring depth
+constexpr int AL_NB = 2;        // bias unit ring depth
+constexpr int AL_BUNIT = 32;    // key columns per bias unit
+constexpr int AL_ACC_LD = 132;  // floats per row of the fp32 score tile
 
 
 struct AttnLoopParams {
@@ -39,81 +41,47 @@ struct AttnLoopParams {
   float* lse;  // optional [groups * S, heads]: log2-domain log-sum-exp of the scaled, biased scores
 };
 
-// Order in which pass 2 consumes K / V tiles: K_0, then for every j: K_{j+1} (if any), V_j — the score MMA of the
-// next key tile is issued before the P V MMA of the current one. Producer and MMA issuer walk the same sequence.
-__device__ __forceinline__ void pass2_tile(int t, int nkt, bool& is_v, int& j) {
-  if (t == 0) {
-    is_v = false, j = 0;
-    return;
-  }
-  // t >= 1: pairs (K_{j+1}, V_j) for j < nkt - 1, then the lone V_{nkt-1}
-  const int pair = (t - 1) >> 1;
-  if (pair < nkt - 1) {
-    is_v = ((t - 1) & 1) != 0;
-    j = is_v ? pair : pair + 1;
-  } else {
-    is_v = true, j = nkt - 1;
-  }
-}
-
-// DUAL = two CTAs per SM (32-wide heads: 104 KB of shared memory, 256 TMEM columns each): a 2-stage K / V ring, bias
-// units of 32 key columns and ONE score stage -- the other CTA's MMAs and TMA loads fill this CTA's softmax phases,
-// which one warp per scheduler cannot hide on its own. !DUAL = one CTA per SM with the deeper rings (64-wide heads).
-template <int HDP, bool DUAL>
-__global__ void __launch_bounds__(AL_THREADS, DUAL ? 2 : 1)
+template <int HDP>
+__global__ void __launch_bounds__(AL_THREADS, 1)
     attn_loop_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_bias,
                      const __grid_constant__ AttnLoopParams p) {
   constexpr uint32_t SWZ = HDP == 64 ? SWZ_128B : SWZ_64B;
   constexpr uint32_t ROW_BYTES = HDP * 2;
   constexpr uint32_t SBO_QKV = 8 * ROW_BYTES;
   constexpr int TILE_BYTES = AL_ROWS * HDP * 2;
-  constexpr int NKV = DUAL ? 2 : AL_NKV;          // K / V tile ring depth
-  constexpr int NB = AL_NB;                       // bias unit ring depth
-  constexpr int BUNIT = DUAL ? 32 : AL_BUNIT;     // key columns per bias unit
+  constexpr int NKV = AL_NKV, NB = AL_NB, BUNIT = AL_BUNIT;
   constexpr int BUNIT_BYTES = AL_ROWS * BUNIT * 4;
   constexpr int UNITS = 128 / BUNIT;              // bias units per key tile
-  constexpr int NS = DUAL ? 1 : 2;                // score stages in TMEM
-  constexpr uint32_t TMEM_COLS = DUAL ? 256 : 512;
+  constexpr int O_LD = HDP + 4;
   constexpr int Q_OFF = 0;
   constexpr int KV_OFF = TILE_BYTES;
   constexpr int P_OFF = KV_OFF + NKV * TILE_BYTES;
   constexpr int BIAS_OFF = P_OFF + AL_ROWS * 128 * 2;
-  constexpr int CTRL_OFF = BIAS_OFF + NB * BUNIT_BYTES;
+  constexpr int SACC_OFF = BIAS_OFF + NB * BUNIT_BYTES;
+  constexpr int OACC_OFF = SACC_OFF + AL_ROWS * AL_ACC_LD * 4;
+  constexpr int CTRL_OFF = OACC_OFF + AL_ROWS * O_LD * 4;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = p.S, nkt = p.nkt;
+  float* sacc = reinterpret_cast<float*>(smem + SACC_OFF);
+  float* oacc = reinterpret_cast<float*>(smem + OACC_OFF);
   uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + CTRL_OFF);
   uint64_t* q_empty = q_full + 1;
   uint64_t* kv_full = q_empty + 1;         // [NKV]
-  uint64_t* kv_empty = kv_full + AL_NKV;   // [NKV] (sized for the deeper ring)
-  uint64_t* b_full = kv_empty + AL_NKV;    // [NB]
-  uint64_t* b_empty = b_full + AL_NB;      // [NB]
-  uint64_t* s_full = b_empty + AL_NB;      // [NS]
-  uint64_t* s_empty = s_full + 2;          // [2]
-  uint64_t* p_full = s_empty + 2;
-  uint64_t* p_empty = p_full + 1;
-  uint64_t* o_full = p_empty + 1;
-  uint64_t* o_empty = o_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_empty + 1);
+  uint64_t* kv_empty = kv_full + NKV;      // [NKV]
+  uint64_t* b_full = kv_empty + NKV;       // [NB]
+  uint64_t* b_empty = b_full + NB;         // [NB]
 
-  if (warp == 0 && lane == 0) {
+  if (warp == AL_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmap_qkv);
     if (p.has_bias) tma_prefetch_desc(&tmap_bias);
     mbar_init(q_full, 1), mbar_init(q_empty, 1);
     for (int i = 0; i < NKV; ++i) mbar_init(&kv_full[i], 1), mbar_init(&kv_empty[i], 1);
     for (int i = 0; i < NB; ++i) mbar_init(&b_full[i], 1), mbar_init(&b_empty[i], 4);
-    for (int i = 0; i < 2; ++i) mbar_init(&s_full[i], 1), mbar_init(&s_empty[i], 4);
-    mbar_init(p_full, 4), mbar_init(p_empty, 1), mbar_init(o_full, 1), mbar_init(o_empty, 4);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S[2] = {tmem_base, tmem_base + (NS == 2 ? 128u : 0u)};
-  const uint32_t tmem_O = tmem_base + 128u * NS;
 
   const int items = p.groups * p.heads * p.nqt;
   // item -> (head, q tile) outer, window inner: CTAs running side by side share the bias tiles in L2
@@ -125,9 +93,16 @@ __global__ void __launch_bounds__(AL_THREADS, DUAL ? 2 : 1)
   };
   auto units_of = [&](int j) { return min(UNITS, (min(128, S - j * 128) + BUNIT - 1) / BUNIT); };  // live bias units of key tile j
 
-  if (warp == 0) {
+  if (warp == AL_PRODUCER) {
     if (lane == 0) {
       uint32_t kv_cnt = 0, b_cnt = 0, it = 0;
+      auto load_kv = [&](int which, int j, int row0, int head) {
+        const int st = kv_cnt % NKV;
+        mbar_wait(&kv_empty[st], ((kv_cnt / NKV) & 1) ^ 1);
+        mbar_expect_tx(&kv_full[st], TILE_BYTES);
+        tma_load_2d(smem + KV_OFF + st * TILE_BYTES, &tmap_qkv, &kv_full[st], (which * p.heads + head) * HDP, row0 + j * 128);
+        ++kv_cnt;
+      };
       for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
         int grp, head, qi;
         decode(w, grp, head, qi);
@@ -135,112 +110,63 @@ __global__ void __launch_bounds__(AL_THREADS, DUAL ? 2 : 1)
         mbar_wait(q_empty, (it & 1) ^ 1);
         mbar_expect_tx(q_full, TILE_BYTES);
         tma_load_2d(smem + Q_OFF, &tmap_qkv, q_full, head * HDP, row0 + qi * 128);
-        // K / V tiles and bias units are produced in the order their consumers need them. The bias units of key tile j
-        // go out only after everything the softmax warps need to CONSUME them has been issued -- K_j (for S_j) and, in
-        // pass 2, V_{j-1} (the softmax of tile j first waits for the P V MMA of tile j-1 to release the P buffer):
-        // pass 1: K_0 b_0 K_1 b_1 ...; pass 2: K_0 b_0 K_1 V_0 b_1 K_2 V_1 b_2 ... A producer blocked on a full bias
-        // ring therefore never holds back a tile the ring's consumers are waiting for.
+        // consumption order: pass 1 K_0 b_0 K_1 b_1 ...; pass 2 K_0 b_0 V_0 K_1 b_1 V_1 ...
         for (int pass = 0; pass < 2; ++pass) {
-          const int ntiles = pass == 0 ? nkt : 2 * nkt;
-          for (int t = 0; t < ntiles; ++t) {
-            bool is_v = false;
-            int j = t;
-            if (pass == 1) pass2_tile(t, nkt, is_v, j);
-            const int st = kv_cnt % NKV;
-            mbar_wait(&kv_empty[st], ((kv_cnt / NKV) & 1) ^ 1);
-            mbar_expect_tx(&kv_full[st], TILE_BYTES);
-            tma_load_2d(smem + KV_OFF + st * TILE_BYTES, &tmap_qkv, &kv_full[st],
-                        ((is_v ? 2 : 1) * p.heads + head) * HDP, row0 + j * 128);
-            ++kv_cnt;
-            // which tile's bias follows this box: pass 1 -> the K tile itself; pass 2 -> K_0 itself, V_{j} -> tile j+1
-            const int bias_j = pass == 0 ? j : (is_v ? j + 1 : (j == 0 ? 0 : -1));
-            if (p.has_bias && bias_j >= 0 && bias_j < nkt) {
-              {
-                for (int u = 0; u < units_of(bias_j); ++u) {
-                  const int bs = b_cnt % NB;
-                  mbar_wait(&b_empty[bs], ((b_cnt / NB) & 1) ^ 1);
-                  mbar_expect_tx(&b_full[bs], BUNIT_BYTES);
-                  uint8_t* dst = smem + BIAS_OFF + bs * BUNIT_BYTES;
-                  const int c0 = bias_j * 128 + u * BUNIT;
-                  tma_load_2d(dst, &tmap_bias, &b_full[bs], c0, head * S + qi * 128);
-                  if (BUNIT == 64) tma_load_2d(dst + AL_ROWS * 128, &tmap_bias, &b_full[bs], c0 + 32, head * S + qi * 128);
-                  ++b_cnt;
-                }
+          for (int j = 0; j < nkt; ++j) {
+            load_kv(1, j, row0, head);
+            if (p.has_bias) {
+              for (int u = 0; u < units_of(j); ++u) {
+                const int bs = b_cnt % NB;
+                mbar_wait(&b_empty[bs], ((b_cnt / NB) & 1) ^ 1);
+                mbar_expect_tx(&b_full[bs], BUNIT_BYTES);
+                tma_load_2d(smem + BIAS_OFF + bs * BUNIT_BYTES, &tmap_bias, &b_full[bs], j * 128 + u * BUNIT,
+                            head * S + qi * 128);
+                ++b_cnt;
               }
             }
+            if (pass == 1) load_kv(2, j, row0, head);
           }
         }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_f16(128, 128, 0, 0);
-      const uint32_t idesc_o = make_idesc_f16(128, HDP, 0, 1);  // B = V, MN-major
-      const uint32_t sQ = smem_u32(smem + Q_OFF);
-      const uint32_t sP = smem_u32(smem + P_OFF);
-      uint32_t kv_cnt = 0, s_cnt = 0, p_cnt = 0, it = 0;
-      auto issue_s = [&]() {  // S = Q K^T from the next ring stage into the next score stage
-        const int st = kv_cnt % NKV;
-        mbar_wait(&kv_full[st], (kv_cnt / NKV) & 1);
-        const int ss = s_cnt % NS;
-        mbar_wait(&s_empty[ss], ((s_cnt / NS) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t sK = smem_u32(smem + KV_OFF + st * TILE_BYTES);
-#pragma unroll
-        for (int k = 0; k < HDP / 16; ++k)
-          umma_f16_ss(tmem_S[ss], make_smem_desc(sQ + k * 32, 16, SBO_QKV, SWZ), make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ),
-                      idesc_s, k > 0 ? 1u : 0u);
-        umma_commit(&s_full[ss]);
-        umma_commit(&kv_empty[st]);
-        ++kv_cnt, ++s_cnt;
-      };
-      auto issue_pv = [&](bool first) {  // O (+)= P V from the next ring stage
-        const int st = kv_cnt % NKV;
-        mbar_wait(&kv_full[st], (kv_cnt / NKV) & 1);
-        mbar_wait(p_full, p_cnt & 1);
-        tc_fence_after();
-        const uint32_t sV = smem_u32(smem + KV_OFF + st * TILE_BYTES);
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks)
-          umma_f16_ss(tmem_O, make_smem_desc(sP + (ks >> 2) * (AL_ROWS * 128) + (ks & 3) * 32, 16, 1024, SWZ_128B),
-                      make_smem_desc(sV + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ), idesc_o, (!first || ks > 0) ? 1u : 0u);
-        umma_commit(p_empty);
-        umma_commit(&kv_empty[st]);
-        ++kv_cnt, ++p_cnt;
-      };
-      for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
-        mbar_wait(q_full, it & 1);
-        for (int j = 0; j < nkt; ++j) issue_s();  // pass 1: maxima only
-        mbar_wait(o_empty, (it & 1) ^ 1);         // previous item's O has been read out
-        issue_s();                                // pass 2: K_0
-        for (int j = 0; j < nkt; ++j) {
-          if (j + 1 < nkt) issue_s();
-          else umma_commit(q_empty);              // last score MMA of the item issued: Q may be overwritten once it retires
-          issue_pv(j == 0);
-        }
-        umma_commit(o_full);
       }
     }
   } else {
     const int quad = warp & 3;
     const int r = quad * 32 + lane;  // query row inside the tile
+    const int tid = threadIdx.x;
     uint8_t* sP = smem + P_OFF;
-    uint32_t s_cnt = 0, b_cnt = 0, p_cnt = 0, it = 0;
+    const uint32_t sQ = smem_u32(smem + Q_OFF);
+    const uint32_t sPu = smem_u32(sP);
+    const float* arow = sacc + r * AL_ACC_LD;
+    uint32_t kv_cnt = 0, b_cnt = 0, it = 0;
     const bool use_bias = p.has_bias != 0;
+    // S_j = Q K_j^T from the next ring stage into the score tile (the stage is released once the MMAs are done)
+    auto score_mma = [&](bool last_of_item) {
+      const int st = kv_cnt % NKV;
+      mbar_wait(&kv_full[st], (kv_cnt / NKV) & 1);
+      const uint32_t sK = smem_u32(smem + KV_OFF + st * TILE_BYTES);
+      named_bar_sync(1, 128);  // every read of the previous score tile is done
+      wg_mma_128<128, 0, 0, HDP / 16>(
+          sacc, AL_ACC_LD,
+          [&](int h, int k) { return make_smem_desc(sQ + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
+          [&](int k) { return make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ); }, false);
+      named_bar_sync(1, 128);
+      if (tid == 0) {
+        mbar_arrive(&kv_empty[st]);
+        if (last_of_item) mbar_arrive(q_empty);
+      }
+      ++kv_cnt;
+    };
     for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
       int grp, head, qi;
       decode(w, grp, head, qi);
       const int qrow = qi * 128 + r;
       const bool row_ok = qrow < S;
       float mx = -INFINITY, sum = 0.f;
+      mbar_wait(q_full, it & 1);
       for (int pass = 0; pass < 2; ++pass) {
         for (int j = 0; j < nkt; ++j) {
-          const int ss = s_cnt % NS;
-          mbar_wait(&s_full[ss], (s_cnt / NS) & 1);
-          tc_fence_after();
-          const uint32_t ts = tmem_S[ss] + ((uint32_t)(quad * 32) << 16);
+          score_mma(pass == 1 && j == nkt - 1);
           const int ncols = min(128, S - j * 128);  // valid keys of this tile
-          if (pass == 1) mbar_wait(p_empty, (p_cnt & 1) ^ 1);  // the previous P V MMA has consumed the P tile
           for (int u = 0; u < UNITS; ++u) {
             const bool unit_live = u * BUNIT < ncols;
             const uint8_t* bunit = nullptr;
@@ -249,16 +175,13 @@ __global__ void __launch_bounds__(AL_THREADS, DUAL ? 2 : 1)
               mbar_wait(&b_full[bs], (b_cnt / NB) & 1);
               bunit = smem + BIAS_OFF + bs * BUNIT_BYTES;
             }
-#pragma unroll
-            for (int h = 0; h < BUNIT / 32; ++h) {
-              const int c0 = u * BUNIT + h * 32;  // first key column of this 32-wide chunk
-              if (pass == 0 && c0 >= ncols) continue;
+            const int c0 = u * BUNIT;  // first key column of this 32-wide chunk
+            if (pass == 1 || c0 < ncols) {
               uint32_t raw[32];
               float sc[32];
               if (c0 < ncols) {
-                tmem_ld32(ts + c0, raw);
-                tmem_ld_wait();
-                const uint8_t* brow = bunit ? bunit + h * (AL_ROWS * 128) + r * 128 : nullptr;
+                ld_row32(arow + c0, raw);
+                const uint8_t* brow = bunit ? bunit + r * 128 : nullptr;
 #pragma unroll
                 for (int q4 = 0; q4 < 8; ++q4) {
                   float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -304,31 +227,33 @@ __global__ void __launch_bounds__(AL_THREADS, DUAL ? 2 : 1)
           }
           if (pass == 0 && !row_ok) mx = 0.f;
           if (pass == 1) {
+            // O (+)= P_j V_j: P is complete once every thread has written its row
             fence_proxy_async_smem();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(p_full);
-            ++p_cnt;
-          } else {
-            tc_fence_before();
-            __syncwarp();
+            named_bar_sync(1, 128);
+            const int st = kv_cnt % NKV;
+            mbar_wait(&kv_full[st], (kv_cnt / NKV) & 1);
+            const uint32_t sV = smem_u32(smem + KV_OFF + st * TILE_BYTES);
+            wg_mma_128<HDP, 0, 1, 8>(
+          oacc, O_LD,
+                [&](int h, int ks) {
+                  return make_smem_desc(sPu + (ks >> 2) * (AL_ROWS * 128) + h * 64 * 128 + (ks & 3) * 32, 16, 1024, SWZ_128B);
+                },
+                [&](int ks) { return make_smem_desc(sV + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, j > 0);
+            named_bar_sync(1, 128);  // P V complete: V stage and P tile are free, O rows are readable
+            if (tid == 0) mbar_arrive(&kv_empty[st]);
+            ++kv_cnt;
           }
-          if (lane == 0) mbar_arrive(&s_empty[ss]);
-          ++s_cnt;
         }
         if (pass == 0 && !row_ok) mx = 0.f;
       }
       // O epilogue
-      mbar_wait(o_full, it & 1);
-      tc_fence_after();
       const float inv = row_ok ? 1.f / sum : 0.f;
       const long long grow = (long long)grp * S + qrow;
-      const uint32_t to = tmem_O + ((uint32_t)(quad * 32) << 16);
+      const float* orow_acc = oacc + r * O_LD;
 #pragma unroll
       for (int c0 = 0; c0 < HDP; c0 += 32) {
         uint32_t raw[32];
-        tmem_ld32(to + c0, raw);
-        tmem_ld_wait();
+        ld_row32(orow_acc + c0, raw);
         if (row_ok) {
           __half* orow = p.out + grow * p.ldo + head * HDP;
 #pragma unroll
@@ -345,33 +270,23 @@ __global__ void __launch_bounds__(AL_THREADS, DUAL ? 2 : 1)
         }
       }
       if (p.lse && row_ok) p.lse[grow * p.heads + head] = mx + log2f(sum);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(o_empty);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
-template <int HDP, bool DUAL>
+template <int HDP>
 static int launch_attn_loop(const CUtensorMap& tq, const CUtensorMap& tb, const AttnLoopParams& p, cudaStream_t st) {
-  constexpr int NKV = DUAL ? 2 : AL_NKV;
-  constexpr int BUNIT_BYTES = AL_ROWS * (DUAL ? 32 : AL_BUNIT) * 4;
-  constexpr size_t smem = 1024 + (size_t)(1 + NKV) * AL_ROWS * HDP * 2 + AL_ROWS * 128 * 2 + AL_NB * BUNIT_BYTES + 256;
-  static_assert(!DUAL || smem <= 113 * 1024, "two CTAs per SM need <= 113 KB each");
+  constexpr size_t smem = 1024 + (size_t)(1 + AL_NKV) * AL_ROWS * HDP * 2 + AL_ROWS * 128 * 2 +
+                          AL_NB * AL_ROWS * AL_BUNIT * 4 + AL_ROWS * AL_ACC_LD * 4 + AL_ROWS * (HDP + 4) * 4 + 256;
+  static_assert(smem <= 227 * 1024, "attn_loop_kernel: shared memory");
   static bool configured = false;
   if (!configured) {
-    FVIT_CUDA(cudaFuncSetAttribute(attn_loop_kernel<HDP, DUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    FVIT_CUDA(cudaFuncSetAttribute(attn_loop_kernel<HDP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
   const long long items = (long long)p.groups * p.heads * p.nqt;
-  const int slots = num_sms() * (DUAL ? 2 : 1);
-  attn_loop_kernel<HDP, DUAL><<<(unsigned)(items < slots ? items : slots), AL_THREADS, smem, st>>>(tq, tb, p);
+  const int slots = num_sms();
+  attn_loop_kernel<HDP><<<(unsigned)(items < slots ? items : slots), AL_THREADS, smem, st>>>(tq, tb, p);
   return post_launch("attn_loop_kernel");
 }
 
@@ -414,27 +329,26 @@ extern "C" int fvit_attn_loop_fwd(const void* qkv, int64_t ldq, int32_t groups, 
   } else {
     tb = tq;
   }
-  if (hdp == 64) return launch_attn_loop<64, false>(tq, tb, p, (cudaStream_t)stream);
-  static int dual = -1;  // FVIT_ATTN_LOOP_DUAL=0: one CTA per SM for 32-wide heads too (A/B)
-  if (dual < 0) {
-    const char* e = getenv("FVIT_ATTN_LOOP_DUAL");
-    dual = e ? atoi(e) : 1;
-  }
-  if (dual) return launch_attn_loop<32, true>(tq, tb, p, (cudaStream_t)stream);
-  return launch_attn_loop<32, false>(tq, tb, p, (cudaStream_t)stream);
+  if (hdp == 64) return launch_attn_loop<64>(tq, tb, p, (cudaStream_t)stream);
+  return launch_attn_loop<32>(tq, tb, p, (cudaStream_t)stream);
 }
 
 // =====================================================================================================
-// fvit_attn_loop_bwd: tensor-core backward of the attention core for 128 < S <= 256 (two query / key tiles).
-// Work item = (window, head). With lse (forward) and delta = rowsum(dO * O) per query row:
-//   for key tile j:  for query tile i:
-//       S = Q_i K_j^T, dP = dO_i V_j^T                        (tcgen05, TMEM columns [0,128) / [128,256))
-//       P = exp2(S*scale*log2e + bias*log2e - lse), dS = P*(dP - delta)   (one thread per query row; fp16 tiles in
-//           shared memory; dS accumulated into dbias with 16-byte reductions)
-//       dV_j += P^T dO_i, dK_j += dS^T Q_i, dQ_i += dS K_j    (TMEM accumulators: dV, dK per key tile, dQ_0 / dQ_1
-//           across the key loop — all 512 columns are in use)
-//   dV_j, dK_j are written after the query loop, dQ_i after the key loop. Nothing but q, k, v, dO, O, lse is read
-// from HBM and nothing but dq, dk, dv (+ the dbias reductions) is written.
+// fvit_attn_loop_bwd_long: tensor-core backward of the attention core for windows longer than one tile (S > 128: any-res
+// S = 148, the 21k models' 14 x 14 ... 48 x 48 windows, fv.py:1253-1418). Work item = (window, head); with lse (forward)
+// and delta = rowsum(dO * O) per query row, key tiles j outside, query tiles i inside:
+//   S = Q_i K_j^T, dP = dO_i V_j^T     (wgmma, in two 64-key halves through fp32 shared-memory tiles)
+//   P = exp2(S*scale*log2e + bias*log2e - lse), dS = P*(dP - delta)   (one thread per query row; fp16 tiles in shared
+//       memory; dS accumulated into dbias with 16-byte reductions)
+//   dV_j += P^T dO_i, dK_j += dS^T Q_i (register accumulators of the warpgroup over the query loop)
+//   and the PARTIAL dQ_i = dS K_j of this pair (not accumulated: nt tiles of dQ do not fit on chip).
+// The thread that owns query row r of every tile adds the partial to its row of an fp32 scratch matrix
+// dq_scratch[groups * S, heads * HDP] (plain 16-byte stores for j = 0, 16-byte reductions afterwards) and converts
+// the row to fp16 once the key loop is over. Only one CTA ever touches a (window, head) slice and only one thread a
+// row of it, so the reductions need no initialisation and no ordering beyond program order. Q_i / dO_i stream through
+// the operand ring (L2 hits after the first key tile); delta and the log-sum-exp rows sit in shared memory.
+//   warp 4     : TMA producer (K_j / V_j, then Q_i / dO_i for every i, in consumption order)
+//   warps 0..3 : one warpgroup: every MMA, the softmax gradient and the epilogues
 namespace fvit {
 
 struct AttnLoopBwdParams {
@@ -451,155 +365,109 @@ struct AttnLoopBwdParams {
   long long lddq;
 };
 
+struct AttnLoopBwdLongParams {
+  AttnLoopBwdParams b;
+  float* dq32;
+  long long lddq32;
+};
+
+constexpr int ALL_THREADS = AL_THREADS;
+constexpr int ALL_HALF_LD = 68;  // floats per row of the 64-column fp32 score / dP tiles
+
 template <int HDP>
-__global__ void __launch_bounds__(AL_THREADS, 1)
-    attn_loop_bwd_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
-                         const __grid_constant__ AttnLoopBwdParams p) {
+struct AttnBwdLongSmem {
+  static constexpr int TILE_BYTES = AL_ROWS * HDP * 2;
+  static constexpr int NQ = HDP == 32 ? 2 : 1;              // (Q_i, dO_i) ring depth
+  static constexpr int QDO_OFF = 0;
+  static constexpr int KV_OFF = NQ * 2 * TILE_BYTES;        // one (K_j, V_j) stage
+  static constexpr int P_OFF = KV_OFF + 2 * TILE_BYTES;
+  static constexpr int DS_OFF = P_OFF + AL_ROWS * 128 * 2;
+  static constexpr int WORK_OFF = DS_OFF + AL_ROWS * 128 * 2;  // S / dP halves, dQ partial, dK / dV staging
+  static constexpr int WORK_BYTES = 2 * AL_ROWS * ALL_HALF_LD * 4;
+  static constexpr int CTRL_OFF = WORK_OFF + WORK_BYTES;
+  static constexpr int ROWV_OFF = CTRL_OFF + 256;           // delta[nt * 128], lse[nt * 128]
+  static_assert(2 * AL_ROWS * (HDP + 4) * 4 <= WORK_BYTES, "dK / dV staging fits the work area");
+};
+
+template <int HDP>
+__global__ void __launch_bounds__(ALL_THREADS, 1)
+    attn_loop_bwd_long_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
+                              const __grid_constant__ AttnLoopBwdLongParams pl) {
+  using SM = AttnBwdLongSmem<HDP>;
+  const AttnLoopBwdParams& p = pl.b;
   constexpr uint32_t SWZ = HDP == 64 ? SWZ_128B : SWZ_64B;
   constexpr uint32_t ROW_BYTES = HDP * 2;
   constexpr uint32_t SBO_QKV = 8 * ROW_BYTES;
-  constexpr int TILE_BYTES = AL_ROWS * HDP * 2;
-  constexpr int QDO_OFF = 0;                      // Q_0, dO_0, Q_1, dO_1
-  constexpr int KV_OFF = 4 * TILE_BYTES;          // 2 stages of (K_j, V_j)
-  constexpr int P_OFF = KV_OFF + 4 * TILE_BYTES;
-  constexpr int DS_OFF = P_OFF + AL_ROWS * 128 * 2;
-  constexpr int CTRL_OFF = DS_OFF + AL_ROWS * 128 * 2;
+  constexpr int TILE_BYTES = SM::TILE_BYTES;
+  constexpr int NQ = SM::NQ;
+  constexpr int G_LD = HDP + 4;  // row stride of the dQ / dK / dV fp32 tiles
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = p.S, nt = p.nt;
-  uint64_t* qdo_full = reinterpret_cast<uint64_t*>(smem + CTRL_OFF);
-  uint64_t* qdo_empty = qdo_full + 1;
-  uint64_t* kv_full = qdo_empty + 1;   // [2]
-  uint64_t* kv_empty = kv_full + 2;    // [2]
-  uint64_t* sdp_full = kv_empty + 2;
-  uint64_t* sdp_empty = sdp_full + 1;
-  uint64_t* pds_full = sdp_empty + 1;
-  uint64_t* pds_empty = pds_full + 1;
-  uint64_t* dkv_full = pds_empty + 1;
-  uint64_t* dkv_empty = dkv_full + 1;
-  uint64_t* dq_full = dkv_empty + 1;
-  uint64_t* dq_empty = dq_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(dq_empty + 1);
+  uint64_t* qdo_full = reinterpret_cast<uint64_t*>(smem + SM::CTRL_OFF);  // [2]
+  uint64_t* qdo_empty = qdo_full + 2;  // [2]
+  uint64_t* kv_full = qdo_empty + 2;
+  uint64_t* kv_empty = kv_full + 1;
+  float* s_delta = reinterpret_cast<float*>(smem + SM::ROWV_OFF);
+  float* s_lse = s_delta + nt * 128;
+  float* work = reinterpret_cast<float*>(smem + SM::WORK_OFF);
+  float* s_half = work;                                // S[:, 64c .. 64c + 64)
+  float* dp_half = work + AL_ROWS * ALL_HALF_LD;       // dP[:, 64c .. 64c + 64)
 
-  if (warp == 0 && lane == 0) {
+  if (warp == AL_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmap_qkv);
     tma_prefetch_desc(&tmap_do);
-    mbar_init(qdo_full, 1), mbar_init(qdo_empty, 1);
-    for (int i = 0; i < 2; ++i) mbar_init(&kv_full[i], 1), mbar_init(&kv_empty[i], 1);
-    mbar_init(sdp_full, 1), mbar_init(sdp_empty, 4);
-    mbar_init(pds_full, 4), mbar_init(pds_empty, 1);
-    mbar_init(dkv_full, 1), mbar_init(dkv_empty, 4);
-    mbar_init(dq_full, 1), mbar_init(dq_empty, 4);
+    for (int i = 0; i < 2; ++i) mbar_init(&qdo_full[i], 1), mbar_init(&qdo_empty[i], 1);
+    mbar_init(kv_full, 1), mbar_init(kv_empty, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base, tDP = tmem_base + 128, tDV = tmem_base + 256, tDK = tmem_base + 320;
-  const uint32_t tDQ[2] = {tmem_base + 384, tmem_base + 448};
 
   const int items = p.groups * p.heads;
-  // head-major item order: the CTAs running side by side reduce into the same dbias[head] lines of L2
 
-  if (warp == 0) {
+  if (warp == AL_PRODUCER) {
     if (lane == 0) {
-      uint32_t it = 0, kv_cnt = 0;
-      for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
+      uint32_t kv_cnt = 0, pair = 0;
+      for (int w = blockIdx.x; w < items; w += gridDim.x) {
         const int grp = w % p.groups, head = w / p.groups;
         const int row0 = grp * S;
-        mbar_wait(qdo_empty, (it & 1) ^ 1);
-        mbar_expect_tx(qdo_full, (uint32_t)(2 * nt * TILE_BYTES));
-        for (int i = 0; i < nt; ++i) {
-          tma_load_2d(smem + QDO_OFF + (2 * i) * TILE_BYTES, &tmap_qkv, qdo_full, head * HDP, row0 + i * 128);
-          tma_load_2d(smem + QDO_OFF + (2 * i + 1) * TILE_BYTES, &tmap_do, qdo_full, head * HDP, row0 + i * 128);
-        }
         for (int j = 0; j < nt; ++j, ++kv_cnt) {
-          const int st = kv_cnt & 1;
-          mbar_wait(&kv_empty[st], ((kv_cnt >> 1) & 1) ^ 1);
-          mbar_expect_tx(&kv_full[st], 2 * TILE_BYTES);
-          tma_load_2d(smem + KV_OFF + (2 * st) * TILE_BYTES, &tmap_qkv, &kv_full[st], (p.heads + head) * HDP, row0 + j * 128);
-          tma_load_2d(smem + KV_OFF + (2 * st + 1) * TILE_BYTES, &tmap_qkv, &kv_full[st], (2 * p.heads + head) * HDP,
-                      row0 + j * 128);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t id_ss = make_idesc_f16(128, 128, 0, 0);
-      const uint32_t id_tn = make_idesc_f16(128, HDP, 1, 1);  // A = P / dS read MN-major (M = keys), B MN-major
-      const uint32_t id_dq = make_idesc_f16(128, HDP, 0, 1);
-      const uint32_t sP = smem_u32(smem + P_OFF), sDS = smem_u32(smem + DS_OFF);
-      uint32_t it = 0, kv_cnt = 0, pair = 0, jcnt = 0;
-      for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
-        mbar_wait(qdo_full, it & 1);
-        mbar_wait(dq_empty, (it & 1) ^ 1);  // previous item's dQ accumulators have been read out
-        for (int j = 0; j < nt; ++j, ++kv_cnt, ++jcnt) {
-          const int st = kv_cnt & 1;
-          mbar_wait(&kv_full[st], (kv_cnt >> 1) & 1);
-          const uint32_t sK = smem_u32(smem + KV_OFF + (2 * st) * TILE_BYTES), sV = sK + TILE_BYTES;
+          mbar_wait(kv_empty, (kv_cnt & 1) ^ 1);
+          mbar_expect_tx(kv_full, 2 * TILE_BYTES);
+          tma_load_2d(smem + SM::KV_OFF, &tmap_qkv, kv_full, (p.heads + head) * HDP, row0 + j * 128);
+          tma_load_2d(smem + SM::KV_OFF + TILE_BYTES, &tmap_qkv, kv_full, (2 * p.heads + head) * HDP, row0 + j * 128);
           for (int i = 0; i < nt; ++i, ++pair) {
-            const uint32_t sQ = smem_u32(smem + QDO_OFF + (2 * i) * TILE_BYTES), sDO = sQ + TILE_BYTES;
-            mbar_wait(sdp_empty, (pair & 1) ^ 1);  // the softmax warps have read the previous pair's S / dP
-            tc_fence_after();
-#pragma unroll
-            for (int k = 0; k < HDP / 16; ++k)
-              umma_f16_ss(tS, make_smem_desc(sQ + k * 32, 16, SBO_QKV, SWZ), make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ), id_ss,
-                          k > 0 ? 1u : 0u);
-#pragma unroll
-            for (int k = 0; k < HDP / 16; ++k)
-              umma_f16_ss(tDP, make_smem_desc(sDO + k * 32, 16, SBO_QKV, SWZ), make_smem_desc(sV + k * 32, 16, SBO_QKV, SWZ), id_ss,
-                          k > 0 ? 1u : 0u);
-            umma_commit(sdp_full);
-            mbar_wait(pds_full, pair & 1);
-            if (i == 0) mbar_wait(dkv_empty, (jcnt & 1) ^ 1);  // previous key tile's dV / dK have been read out
-            tc_fence_after();
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks) {  // K = 128 query rows in steps of 16
-              const uint64_t aP = make_smem_desc(sP + ks * 2048, AL_ROWS * 128, 1024, SWZ_128B);
-              const uint64_t aDS = make_smem_desc(sDS + ks * 2048, AL_ROWS * 128, 1024, SWZ_128B);
-              const uint64_t bDO = make_smem_desc(sDO + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ);
-              const uint64_t bQ = make_smem_desc(sQ + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ);
-              umma_f16_ss(tDV, aP, bDO, id_tn, (i > 0 || ks > 0) ? 1u : 0u);
-              umma_f16_ss(tDK, aDS, bQ, id_tn, (i > 0 || ks > 0) ? 1u : 0u);
-            }
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks) {  // K = 128 keys
-              const uint64_t aDS = make_smem_desc(sDS + (ks >> 2) * (AL_ROWS * 128) + (ks & 3) * 32, 16, 1024, SWZ_128B);
-              const uint64_t bK = make_smem_desc(sK + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ);
-              umma_f16_ss(tDQ[i], aDS, bK, id_dq, (j > 0 || ks > 0) ? 1u : 0u);
-            }
-            umma_commit(pds_empty);
+            const int qs = pair % NQ;
+            mbar_wait(&qdo_empty[qs], ((pair / NQ) & 1) ^ 1);
+            mbar_expect_tx(&qdo_full[qs], 2 * TILE_BYTES);
+            tma_load_2d(smem + SM::QDO_OFF + (2 * qs) * TILE_BYTES, &tmap_qkv, &qdo_full[qs], head * HDP, row0 + i * 128);
+            tma_load_2d(smem + SM::QDO_OFF + (2 * qs + 1) * TILE_BYTES, &tmap_do, &qdo_full[qs], head * HDP, row0 + i * 128);
           }
-          umma_commit(dkv_full);
-          umma_commit(&kv_empty[st]);
         }
-        umma_commit(dq_full);
-        umma_commit(qdo_empty);
       }
     }
   } else {
     const int quad = warp & 3;
     const int r = quad * 32 + lane;
-    uint8_t* sP = smem + P_OFF;
-    uint8_t* sDS = smem + DS_OFF;
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-    uint32_t it = 0, pair = 0, jcnt = 0;
+    const int tid = threadIdx.x;
+    uint8_t* sP = smem + SM::P_OFF;
+    uint8_t* sDS = smem + SM::DS_OFF;
+    const uint32_t sPu = smem_u32(sP), sDSu = smem_u32(sDS);
+    const uint32_t sK = smem_u32(smem + SM::KV_OFF), sV = sK + TILE_BYTES;
+    uint32_t kv_cnt = 0, pair = 0;
     const int Cp = p.heads * HDP;
-    for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
+    for (int w = blockIdx.x; w < items; w += gridDim.x) {
       const int grp = w % p.groups, head = w / p.groups;
       const long long row0 = (long long)grp * S;
-      // per query row of both tiles: delta = sum_c dO * O and the forward's log-sum-exp
-      float delta[2] = {0.f, 0.f}, lse[2] = {0.f, 0.f};
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
+      // per query row: delta = sum_c dO * O and the forward's log-sum-exp
+      named_bar_sync(1, 128);  // the previous item's readers of the row vectors are done
+      for (int i = 0; i < nt; ++i) {
         const int q = i * 128 + r;
-        if (i < nt && q < S) {
+        float acc = 0.f, l = 0.f;
+        if (q < S) {
           const uint4* a = reinterpret_cast<const uint4*>(p.dout + (row0 + q) * p.lddo + head * HDP);
           const uint4* b = reinterpret_cast<const uint4*>(p.out + (row0 + q) * p.ldo + head * HDP);
-          float acc = 0.f;
 #pragma unroll
           for (int v = 0; v < HDP / 8; ++v) {
             const uint4 x = __ldg(a + v), y = __ldg(b + v);
@@ -611,468 +479,148 @@ __global__ void __launch_bounds__(AL_THREADS, 1)
               acc = fmaf(fx.x, fy.x, fmaf(fx.y, fy.y, acc));
             }
           }
-          delta[i] = acc;
-          lse[i] = p.lse[(row0 + q) * p.heads + head];
+          l = p.lse[(row0 + q) * p.heads + head];
         }
+        s_delta[q] = acc, s_lse[q] = l;
       }
-      for (int j = 0; j < nt; ++j, ++jcnt) {
+      for (int j = 0; j < nt; ++j, ++kv_cnt) {
         const int ncols = min(128, S - j * 128);
+        mbar_wait(kv_full, kv_cnt & 1);
+        // dV_j / dK_j accumulators (rows 64h .. 64h + 63 = keys of this tile), summed over the query tiles
+        float dv[2][HDP / 2], dk[2][HDP / 2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int u = 0; u < HDP / 2; ++u) dv[h][u] = 0.f, dk[h][u] = 0.f;
         for (int i = 0; i < nt; ++i, ++pair) {
-          const int q = i * 128 + r;
-          const bool row_ok = q < S;
-          const float my_lse = i == 0 ? lse[0] : lse[1], my_delta = i == 0 ? delta[0] : delta[1];
-          mbar_wait(sdp_full, pair & 1);
-          mbar_wait(pds_empty, (pair & 1) ^ 1);  // the previous pair's gradient MMAs have consumed P / dS
-          tc_fence_after();
-          const float* brow = (p.bias && row_ok) ? p.bias + ((long long)head * S + q) * S + j * 128 : nullptr;
-          float* dbrow = (p.dbias && row_ok) ? p.dbias + ((long long)head * S + q) * S + j * 128 : nullptr;
-#pragma unroll 1
-          for (int c0 = 0; c0 < 128; c0 += 32) {
-            uint32_t pkp[16], pkd[16];
-            if (c0 < ncols) {
-              uint32_t rs[32], rd[32];
-              tmem_ld32(tS + lane_off + c0, rs);
-              tmem_ld32(tDP + lane_off + c0, rd);
-              tmem_ld_wait();
-#pragma unroll
-              for (int q4 = 0; q4 < 8; ++q4) {
-                const int c = c0 + q4 * 4;
-                float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (brow && c < ncols) b4 = __ldg(reinterpret_cast<const float4*>(brow + c));
-                const float bb[4] = {b4.x, b4.y, b4.z, b4.w};
-                float pv[4], ds[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const bool in = row_ok && (c + e < ncols);
-                  const float sc = fmaf(__uint_as_float(rs[q4 * 4 + e]), p.scale_log2e, fmaf(bb[e], 1.4426950408889634f, -my_lse));
-                  pv[e] = in ? exp2f(sc) : 0.f;
-                  ds[e] = in ? pv[e] * (__uint_as_float(rd[q4 * 4 + e]) - my_delta) : 0.f;
-                }
-                if (dbrow && c < ncols)  // (S % 4 == 0: a 4-column group is entirely inside or outside the window)
-                  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dbrow + c), "f"(ds[0]), "f"(ds[1]),
-                               "f"(ds[2]), "f"(ds[3])
-                               : "memory");
-                const __half2 p0 = __floats2half2_rn(pv[0], pv[1]), p1 = __floats2half2_rn(pv[2], pv[3]);
-                const __half2 d0 = __floats2half2_rn(ds[0], ds[1]), d1 = __floats2half2_rn(ds[2], ds[3]);
-                pkp[q4 * 2] = *reinterpret_cast<const uint32_t*>(&p0), pkp[q4 * 2 + 1] = *reinterpret_cast<const uint32_t*>(&p1);
-                pkd[q4 * 2] = *reinterpret_cast<const uint32_t*>(&d0), pkd[q4 * 2 + 1] = *reinterpret_cast<const uint32_t*>(&d1);
-              }
-            } else {
-#pragma unroll
-              for (int e = 0; e < 16; ++e) pkp[e] = 0u, pkd[e] = 0u;
-            }
-#pragma unroll
-            for (int qq = 0; qq < 4; ++qq) {
-              const int c = c0 + qq * 8;
-              const uint32_t off = (c >> 6) * (AL_ROWS * 128) + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4);
-              *reinterpret_cast<uint4*>(sP + off) = make_uint4(pkp[4 * qq], pkp[4 * qq + 1], pkp[4 * qq + 2], pkp[4 * qq + 3]);
-              *reinterpret_cast<uint4*>(sDS + off) = make_uint4(pkd[4 * qq], pkd[4 * qq + 1], pkd[4 * qq + 2], pkd[4 * qq + 3]);
-            }
-          }
-          fence_proxy_async_smem();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(sdp_empty);
-            mbar_arrive(pds_full);
-          }
-        }
-        // dV_j / dK_j: row r of the accumulators is key j*128 + r
-        mbar_wait(dkv_full, jcnt & 1);
-        tc_fence_after();
-        {
-          const int key = j * 128 + r;
-          const bool ok = key < S;
-          __half* orow = p.dqkv + (row0 + key) * p.lddq + head * HDP;
-#pragma unroll
-          for (int which = 1; which < 3; ++which) {
-            const uint32_t tsrc = (which == 1 ? tDK : tDV) + lane_off;
-            const float mul = which == 1 ? p.scale : 1.f;
-#pragma unroll
-            for (int c0 = 0; c0 < HDP; c0 += 32) {
-              uint32_t raw[32];
-              tmem_ld32(tsrc + c0, raw);
-              tmem_ld_wait();
-              if (ok) {
-#pragma unroll
-                for (int qq = 0; qq < 4; ++qq) {
-                  uint32_t o4[4];
-#pragma unroll
-                  for (int u = 0; u < 4; ++u) {
-                    const __half2 hh = __floats2half2_rn(__uint_as_float(raw[qq * 8 + 2 * u]) * mul,
-                                                         __uint_as_float(raw[qq * 8 + 2 * u + 1]) * mul);
-                    o4[u] = *reinterpret_cast<const uint32_t*>(&hh);
-                  }
-                  *reinterpret_cast<uint4*>(orow + which * Cp + c0 + qq * 8) = make_uint4(o4[0], o4[1], o4[2], o4[3]);
-                }
-              }
-            }
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(dkv_empty);
-      }
-      // dQ_i: row r is query i*128 + r
-      mbar_wait(dq_full, it & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        if (i < nt) {
-          const int q = i * 128 + r;
-          const bool ok = q < S;
-          __half* orow = p.dqkv + (row0 + q) * p.lddq + head * HDP;
-#pragma unroll
-          for (int c0 = 0; c0 < HDP; c0 += 32) {
-            uint32_t raw[32];
-            tmem_ld32(tDQ[i] + lane_off + c0, raw);
-            tmem_ld_wait();
-            if (ok) {
-#pragma unroll
-              for (int qq = 0; qq < 4; ++qq) {
-                uint32_t o4[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                  const __half2 hh = __floats2half2_rn(__uint_as_float(raw[qq * 8 + 2 * u]) * p.scale,
-                                                       __uint_as_float(raw[qq * 8 + 2 * u + 1]) * p.scale);
-                  o4[u] = *reinterpret_cast<const uint32_t*>(&hh);
-                }
-                *reinterpret_cast<uint4*>(orow + c0 + qq * 8) = make_uint4(o4[0], o4[1], o4[2], o4[3]);
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(dq_empty);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-template <int HDP>
-static int launch_attn_loop_bwd(const CUtensorMap& tq, const CUtensorMap& td, const AttnLoopBwdParams& p, cudaStream_t st) {
-  constexpr size_t smem = 1024 + (size_t)8 * AL_ROWS * HDP * 2 + 2 * AL_ROWS * 128 * 2 + 256;
-  static bool configured = false;
-  if (!configured) {
-    FVIT_CUDA(cudaFuncSetAttribute(attn_loop_bwd_kernel<HDP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = true;
-  }
-  const int items = p.groups * p.heads;
-  const int sms = num_sms();
-  attn_loop_bwd_kernel<HDP><<<items < sms ? items : sms, AL_THREADS, smem, st>>>(tq, td, p);
-  return post_launch("attn_loop_bwd_kernel");
-}
-
-
-// =====================================================================================================
-// fvit_attn_loop_bwd_long: the same backward for windows of more than two tiles (S > 256: the 21k models' 24 x 24,
-// 32 x 32 and 48 x 48 windows, fv.py:1253-1418). Work item = (window, head); key tiles j outside, query tiles i inside:
-//   S = Q_i K_j^T, dP = dO_i V_j^T -> P, dS (as above) -> dV_j += P^T dO_i, dK_j += dS^T Q_i (TMEM, over the query loop)
-//   and the PARTIAL dQ_i = dS K_j of this pair in its own TMEM region (not accumulated: nt tiles of dQ do not fit).
-// The thread that owns query row r of every tile adds the partial to its row of an fp32 scratch matrix
-// dq_scratch[groups * S, heads * HDP] (plain 16-byte stores for j = 0, 16-byte reductions afterwards) and converts
-// the row to fp16 once the key loop is over. Only one CTA ever touches a (window, head) slice and only one thread a
-// row of it, so the reductions need no initialisation and no ordering beyond program order. Q_i / dO_i stream through
-// a two-stage ring (L2 hits after the first key tile); delta and the log-sum-exp rows sit in shared memory.
-struct AttnLoopBwdLongParams {
-  AttnLoopBwdParams b;
-  float* dq32;
-  long long lddq32;
-};
-
-constexpr int ALL_SOFTMAX_WARPS = 8;                      // two per TMEM lane quarter (64 score columns each)
-constexpr int ALL_THREADS = (2 + ALL_SOFTMAX_WARPS) * 32;  // + TMA producer, MMA issuer
-
-template <int HDP>
-__global__ void __launch_bounds__(ALL_THREADS, 1)
-    attn_loop_bwd_long_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
-                              const __grid_constant__ AttnLoopBwdLongParams pl) {
-  const AttnLoopBwdParams& p = pl.b;
-  constexpr uint32_t SWZ = HDP == 64 ? SWZ_128B : SWZ_64B;
-  constexpr uint32_t ROW_BYTES = HDP * 2;
-  constexpr uint32_t SBO_QKV = 8 * ROW_BYTES;
-  constexpr int TILE_BYTES = AL_ROWS * HDP * 2;
-  constexpr int QDO_OFF = 0;                      // 2 stages of (Q_i, dO_i)
-  constexpr int KV_OFF = 4 * TILE_BYTES;          // 2 stages of (K_j, V_j)
-  constexpr int P_OFF = KV_OFF + 4 * TILE_BYTES;
-  constexpr int DS_OFF = P_OFF + AL_ROWS * 128 * 2;
-  constexpr int CTRL_OFF = DS_OFF + AL_ROWS * 128 * 2;
-  constexpr int ROWV_OFF = CTRL_OFF + 256;        // delta[nt * 128], lse[nt * 128]
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int S = p.S, nt = p.nt;
-  uint64_t* qdo_full = reinterpret_cast<uint64_t*>(smem + CTRL_OFF);  // [2]
-  uint64_t* qdo_empty = qdo_full + 2;  // [2]
-  uint64_t* kv_full = qdo_empty + 2;   // [2]
-  uint64_t* kv_empty = kv_full + 2;    // [2]
-  uint64_t* sdp_full = kv_empty + 2;
-  uint64_t* sdp_empty = sdp_full + 1;
-  uint64_t* pds_full = sdp_empty + 1;
-  uint64_t* pds_empty = pds_full + 1;
-  uint64_t* dkv_full = pds_empty + 1;
-  uint64_t* dkv_empty = dkv_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(dkv_empty + 1);
-  float* s_delta = reinterpret_cast<float*>(smem + ROWV_OFF);
-  float* s_lse = s_delta + nt * 128;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_qkv);
-    tma_prefetch_desc(&tmap_do);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&qdo_full[i], 1), mbar_init(&qdo_empty[i], 1);
-      mbar_init(&kv_full[i], 1), mbar_init(&kv_empty[i], 1);
-    }
-    mbar_init(sdp_full, 1), mbar_init(sdp_empty, ALL_SOFTMAX_WARPS);
-    mbar_init(pds_full, ALL_SOFTMAX_WARPS), mbar_init(pds_empty, 1);
-    mbar_init(dkv_full, 1), mbar_init(dkv_empty, ALL_SOFTMAX_WARPS);
-    fence_mbar_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base, tDP = tmem_base + 128, tDV = tmem_base + 256, tDK = tmem_base + 320, tDQ = tmem_base + 384;
-
-  const int items = p.groups * p.heads;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t kv_cnt = 0, pair = 0;
-      for (int w = blockIdx.x; w < items; w += gridDim.x) {
-        const int grp = w % p.groups, head = w / p.groups;
-        const int row0 = grp * S;
-        for (int j = 0; j < nt; ++j, ++kv_cnt) {
-          const int st = kv_cnt & 1;
-          mbar_wait(&kv_empty[st], ((kv_cnt >> 1) & 1) ^ 1);
-          mbar_expect_tx(&kv_full[st], 2 * TILE_BYTES);
-          tma_load_2d(smem + KV_OFF + (2 * st) * TILE_BYTES, &tmap_qkv, &kv_full[st], (p.heads + head) * HDP, row0 + j * 128);
-          tma_load_2d(smem + KV_OFF + (2 * st + 1) * TILE_BYTES, &tmap_qkv, &kv_full[st], (2 * p.heads + head) * HDP,
-                      row0 + j * 128);
-          for (int i = 0; i < nt; ++i, ++pair) {
-            const int qs = pair & 1;
-            mbar_wait(&qdo_empty[qs], ((pair >> 1) & 1) ^ 1);
-            mbar_expect_tx(&qdo_full[qs], 2 * TILE_BYTES);
-            tma_load_2d(smem + QDO_OFF + (2 * qs) * TILE_BYTES, &tmap_qkv, &qdo_full[qs], head * HDP, row0 + i * 128);
-            tma_load_2d(smem + QDO_OFF + (2 * qs + 1) * TILE_BYTES, &tmap_do, &qdo_full[qs], head * HDP, row0 + i * 128);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t id_ss = make_idesc_f16(128, 128, 0, 0);
-      const uint32_t id_tn = make_idesc_f16(128, HDP, 1, 1);  // A = P / dS read MN-major (M = keys), B MN-major
-      const uint32_t id_dq = make_idesc_f16(128, HDP, 0, 1);
-      const uint32_t sP = smem_u32(smem + P_OFF), sDS = smem_u32(smem + DS_OFF);
-      uint32_t kv_cnt = 0, pair = 0, jcnt = 0;
-      for (int w = blockIdx.x; w < items; w += gridDim.x) {
-        for (int j = 0; j < nt; ++j, ++kv_cnt, ++jcnt) {
-          const int st = kv_cnt & 1;
-          mbar_wait(&kv_full[st], (kv_cnt >> 1) & 1);
-          const uint32_t sK = smem_u32(smem + KV_OFF + (2 * st) * TILE_BYTES), sV = sK + TILE_BYTES;
-          for (int i = 0; i < nt; ++i, ++pair) {
-            const int qs = pair & 1;
-            const uint32_t sQ = smem_u32(smem + QDO_OFF + (2 * qs) * TILE_BYTES), sDO = sQ + TILE_BYTES;
-            mbar_wait(&qdo_full[qs], (pair >> 1) & 1);
-            mbar_wait(sdp_empty, (pair & 1) ^ 1);  // the softmax warps have read the previous pair's S / dP
-            tc_fence_after();
-#pragma unroll
-            for (int k = 0; k < HDP / 16; ++k)
-              umma_f16_ss(tS, make_smem_desc(sQ + k * 32, 16, SBO_QKV, SWZ), make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ), id_ss,
-                          k > 0 ? 1u : 0u);
-#pragma unroll
-            for (int k = 0; k < HDP / 16; ++k)
-              umma_f16_ss(tDP, make_smem_desc(sDO + k * 32, 16, SBO_QKV, SWZ), make_smem_desc(sV + k * 32, 16, SBO_QKV, SWZ), id_ss,
-                          k > 0 ? 1u : 0u);
-            umma_commit(sdp_full);
-            // pds_full also says: the previous pair's dQ partial has been read out of tDQ
-            mbar_wait(pds_full, pair & 1);
-            if (i == 0) mbar_wait(dkv_empty, (jcnt & 1) ^ 1);  // previous key tile's dV / dK have been read out
-            tc_fence_after();
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks) {  // K = 128 query rows in steps of 16
-              const uint64_t aP = make_smem_desc(sP + ks * 2048, AL_ROWS * 128, 1024, SWZ_128B);
-              const uint64_t aDS = make_smem_desc(sDS + ks * 2048, AL_ROWS * 128, 1024, SWZ_128B);
-              const uint64_t bDO = make_smem_desc(sDO + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ);
-              const uint64_t bQ = make_smem_desc(sQ + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ);
-              umma_f16_ss(tDV, aP, bDO, id_tn, (i > 0 || ks > 0) ? 1u : 0u);
-              umma_f16_ss(tDK, aDS, bQ, id_tn, (i > 0 || ks > 0) ? 1u : 0u);
-            }
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks) {  // K = 128 keys
-              const uint64_t aDS = make_smem_desc(sDS + (ks >> 2) * (AL_ROWS * 128) + (ks & 3) * 32, 16, 1024, SWZ_128B);
-              const uint64_t bK = make_smem_desc(sK + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ);
-              umma_f16_ss(tDQ, aDS, bK, id_dq, ks > 0 ? 1u : 0u);
-            }
-            umma_commit(pds_empty);
-            umma_commit(&qdo_empty[qs]);
-          }
-          umma_commit(dkv_full);
-          umma_commit(&kv_empty[st]);
-        }
-      }
-    }
-  } else {
-    // eight softmax warps: TMEM lane quarter (warp & 3) = query rows 32 * quad .. + 31 of the tile, `half` = which 64 of
-    // the 128 key columns of a pair (and which half of the head columns in the epilogues). Two warps per scheduler
-    // hide each other's tcgen05.ld / bias latencies; the bias values of a pair are requested before the wait for its
-    // score MMAs (the addresses do not depend on them).
-    const int quad = warp & 3, half = (warp - 2) >> 2;
-    const int r = quad * 32 + lane;
-    uint8_t* sP = smem + P_OFF;
-    uint8_t* sDS = smem + DS_OFF;
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-    uint32_t pair = 0, jcnt = 0;
-    const int Cp = p.heads * HDP;
-    const int cbeg = half * 64;              // score columns [cbeg, cbeg + 64) of every pair
-    for (int w = blockIdx.x; w < items; w += gridDim.x) {
-      const int grp = w % p.groups, head = w / p.groups;
-      const long long row0 = (long long)grp * S;
-      // per query row: delta = sum_c dO * O and the forward's log-sum-exp (half 0 computes, both halves read)
-      if (half == 0) {
-        for (int i = 0; i < nt; ++i) {
-          const int q = i * 128 + r;
-          float acc = 0.f, l = 0.f;
-          if (q < S) {
-            const uint4* a = reinterpret_cast<const uint4*>(p.dout + (row0 + q) * p.lddo + head * HDP);
-            const uint4* b = reinterpret_cast<const uint4*>(p.out + (row0 + q) * p.ldo + head * HDP);
-#pragma unroll
-            for (int v = 0; v < HDP / 8; ++v) {
-              const uint4 x = __ldg(a + v), y = __ldg(b + v);
-              const __half2* hx = reinterpret_cast<const __half2*>(&x);
-              const __half2* hy = reinterpret_cast<const __half2*>(&y);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float2 fx = __half22float2(hx[e]), fy = __half22float2(hy[e]);
-                acc = fmaf(fx.x, fy.x, fmaf(fx.y, fy.y, acc));
-              }
-            }
-            l = p.lse[(row0 + q) * p.heads + head];
-          }
-          s_delta[q] = acc, s_lse[q] = l;
-        }
-      }
-      asm volatile("bar.sync 1, %0;" ::"n"(ALL_SOFTMAX_WARPS * 32) : "memory");   // (the softmax warps only)
-      // partial dQ of the pair (j, i): TMEM -> * scale -> this thread's share of the fp32 scratch row
-      auto flush_dq = [&](int j, int i) {
-        const int q = i * 128 + r;
-        float* drow = pl.dq32 + (row0 + q) * pl.lddq32 + head * HDP;
-#pragma unroll
-        for (int c0 = half * 32; c0 < HDP; c0 += 64) {
-          uint32_t raw[32];
-          tmem_ld32(tDQ + lane_off + c0, raw);
-          tmem_ld_wait();
-          if (q < S) {
-#pragma unroll
-            for (int q4 = 0; q4 < 8; ++q4) {
-              const float v0 = __uint_as_float(raw[q4 * 4]) * p.scale, v1 = __uint_as_float(raw[q4 * 4 + 1]) * p.scale;
-              const float v2 = __uint_as_float(raw[q4 * 4 + 2]) * p.scale, v3 = __uint_as_float(raw[q4 * 4 + 3]) * p.scale;
-              if (j == 0)
-                *reinterpret_cast<float4*>(drow + c0 + q4 * 4) = make_float4(v0, v1, v2, v3);
-              else
-                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(drow + c0 + q4 * 4), "f"(v0), "f"(v1),
-                             "f"(v2), "f"(v3)
-                             : "memory");
-            }
-          }
-        }
-      };
-      for (int j = 0; j < nt; ++j, ++jcnt) {
-        const int ncols = min(128, S - j * 128);
-        for (int i = 0; i < nt; ++i, ++pair) {
+          const int qs = pair % NQ;
+          mbar_wait(&qdo_full[qs], (pair / NQ) & 1);
+          const uint32_t sQ = smem_u32(smem + SM::QDO_OFF + (2 * qs) * TILE_BYTES), sDO = sQ + TILE_BYTES;
           const int q = i * 128 + r;
           const bool row_ok = q < S;
           const float my_lse = s_lse[q], my_delta = s_delta[q];
           const float* brow = (p.bias && row_ok) ? p.bias + ((long long)head * S + q) * S + j * 128 : nullptr;
           float* dbrow = (p.dbias && row_ok) ? p.dbias + ((long long)head * S + q) * S + j * 128 : nullptr;
-          // this pair's 64 bias values, in flight while the score MMAs run
-          float4 bq[16];
+#pragma unroll 1
+          for (int ch = 0; ch < 2; ++ch) {  // key columns [64ch, 64ch + 64) of the pair
+            named_bar_sync(1, 128);         // the work area is free
+            wg_mma_128<64, 0, 0, HDP / 16>(
+          s_half, ALL_HALF_LD,
+                [&](int h, int k) { return make_smem_desc(sQ + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
+                [&](int k) { return make_smem_desc(sK + ch * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); }, false);
+            wg_mma_128<64, 0, 0, HDP / 16>(
+          dp_half, ALL_HALF_LD,
+                [&](int h, int k) { return make_smem_desc(sDO + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
+                [&](int k) { return make_smem_desc(sV + ch * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); }, false);
+            named_bar_sync(1, 128);
+#pragma unroll 1
+            for (int cc = 0; cc < 64; cc += 16) {
+              const int c0 = ch * 64 + cc;
+              uint32_t pkp[8], pkd[8];
+              if (c0 < ncols) {
+                uint32_t rs[16], rd[16];
+                ld_row16(s_half + r * ALL_HALF_LD + cc, rs);
+                ld_row16(dp_half + r * ALL_HALF_LD + cc, rd);
 #pragma unroll
-          for (int u = 0; u < 16; ++u) {
-            const int c = cbeg + u * 4;
-            bq[u] = (brow && c < ncols) ? __ldg(reinterpret_cast<const float4*>(brow + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-          mbar_wait(sdp_full, pair & 1);
-          mbar_wait(pds_empty, (pair & 1) ^ 1);  // the previous pair's gradient MMAs are complete: P / dS free, dQ final
-          tc_fence_after();
-          if (i > 0) flush_dq(j, i - 1);
+                for (int q4 = 0; q4 < 4; ++q4) {
+                  const int c = c0 + q4 * 4;
+                  const float4 b4 =
+                      (brow && c < ncols) ? __ldg(reinterpret_cast<const float4*>(brow + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                  const float bb[4] = {b4.x, b4.y, b4.z, b4.w};
+                  float pv[4], ds[4];
 #pragma unroll
-          for (int cc = 0; cc < 64; cc += 16) {
-            const int c0 = cbeg + cc;
-            uint32_t pkp[8], pkd[8];
-            if (c0 < ncols) {
-              uint32_t rs[16], rd[16];
-              tmem_ld16(tS + lane_off + c0, rs);
-              tmem_ld16(tDP + lane_off + c0, rd);
-              tmem_ld_wait();
-#pragma unroll
-              for (int q4 = 0; q4 < 4; ++q4) {
-                const int c = c0 + q4 * 4;
-                const float4 b4 = bq[cc / 4 + q4];
-                const float bb[4] = {b4.x, b4.y, b4.z, b4.w};
-                float pv[4], ds[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const bool in = row_ok && (c + e < ncols);
-                  const float sc = fmaf(__uint_as_float(rs[q4 * 4 + e]), p.scale_log2e, fmaf(bb[e], 1.4426950408889634f, -my_lse));
-                  pv[e] = in ? exp2f(sc) : 0.f;
-                  ds[e] = in ? pv[e] * (__uint_as_float(rd[q4 * 4 + e]) - my_delta) : 0.f;
+                  for (int e = 0; e < 4; ++e) {
+                    const bool in = row_ok && (c + e < ncols);
+                    const float sc = fmaf(__uint_as_float(rs[q4 * 4 + e]), p.scale_log2e, fmaf(bb[e], 1.4426950408889634f, -my_lse));
+                    pv[e] = in ? exp2f(sc) : 0.f;
+                    ds[e] = in ? pv[e] * (__uint_as_float(rd[q4 * 4 + e]) - my_delta) : 0.f;
+                  }
+                  if (dbrow && c < ncols)  // (S % 4 == 0: a 4-column group is entirely inside or outside the window)
+                    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dbrow + c), "f"(ds[0]), "f"(ds[1]),
+                                 "f"(ds[2]), "f"(ds[3])
+                                 : "memory");
+                  const __half2 p0 = __floats2half2_rn(pv[0], pv[1]), p1 = __floats2half2_rn(pv[2], pv[3]);
+                  const __half2 d0 = __floats2half2_rn(ds[0], ds[1]), d1 = __floats2half2_rn(ds[2], ds[3]);
+                  pkp[q4 * 2] = *reinterpret_cast<const uint32_t*>(&p0), pkp[q4 * 2 + 1] = *reinterpret_cast<const uint32_t*>(&p1);
+                  pkd[q4 * 2] = *reinterpret_cast<const uint32_t*>(&d0), pkd[q4 * 2 + 1] = *reinterpret_cast<const uint32_t*>(&d1);
                 }
-                if (dbrow && c < ncols)  // (S % 4 == 0: a 4-column group is entirely inside or outside the window)
-                  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dbrow + c), "f"(ds[0]), "f"(ds[1]),
-                               "f"(ds[2]), "f"(ds[3])
-                               : "memory");
-                const __half2 p0 = __floats2half2_rn(pv[0], pv[1]), p1 = __floats2half2_rn(pv[2], pv[3]);
-                const __half2 d0 = __floats2half2_rn(ds[0], ds[1]), d1 = __floats2half2_rn(ds[2], ds[3]);
-                pkp[q4 * 2] = *reinterpret_cast<const uint32_t*>(&p0), pkp[q4 * 2 + 1] = *reinterpret_cast<const uint32_t*>(&p1);
-                pkd[q4 * 2] = *reinterpret_cast<const uint32_t*>(&d0), pkd[q4 * 2 + 1] = *reinterpret_cast<const uint32_t*>(&d1);
+              } else {
+#pragma unroll
+                for (int e = 0; e < 8; ++e) pkp[e] = 0u, pkd[e] = 0u;
               }
-            } else {
 #pragma unroll
-              for (int e = 0; e < 8; ++e) pkp[e] = 0u, pkd[e] = 0u;
-            }
-#pragma unroll
-            for (int qq = 0; qq < 2; ++qq) {
-              const int c = c0 + qq * 8;
-              const uint32_t off = (c >> 6) * (AL_ROWS * 128) + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4);
-              *reinterpret_cast<uint4*>(sP + off) = make_uint4(pkp[4 * qq], pkp[4 * qq + 1], pkp[4 * qq + 2], pkp[4 * qq + 3]);
-              *reinterpret_cast<uint4*>(sDS + off) = make_uint4(pkd[4 * qq], pkd[4 * qq + 1], pkd[4 * qq + 2], pkd[4 * qq + 3]);
+              for (int qq = 0; qq < 2; ++qq) {
+                const int c = c0 + qq * 8;
+                const uint32_t off = (c >> 6) * (AL_ROWS * 128) + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4);
+                *reinterpret_cast<uint4*>(sP + off) = make_uint4(pkp[4 * qq], pkp[4 * qq + 1], pkp[4 * qq + 2], pkp[4 * qq + 3]);
+                *reinterpret_cast<uint4*>(sDS + off) = make_uint4(pkd[4 * qq], pkd[4 * qq + 1], pkd[4 * qq + 2], pkd[4 * qq + 3]);
+              }
             }
           }
           fence_proxy_async_smem();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(sdp_empty);
-            mbar_arrive(pds_full);
+          named_bar_sync(1, 128);  // P / dS complete, S / dP reads done
+          // dV_j += P^T dO_i, dK_j += dS^T Q_i: A read MN-major (M = keys, K = 128 query rows)
+          wgmma_fence();
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks) {
+              Wgmma<HDP, 1, 1, 0>::mma(dv[h], make_smem_desc(sPu + h * (AL_ROWS * 128) + ks * 2048, AL_ROWS * 128, 1024, SWZ_128B),
+                                       make_smem_desc(sDO + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ), 1u);
+              Wgmma<HDP, 1, 1, 0>::mma(dk[h], make_smem_desc(sDSu + h * (AL_ROWS * 128) + ks * 2048, AL_ROWS * 128, 1024, SWZ_128B),
+                                       make_smem_desc(sQ + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ), 1u);
+            }
+          }
+          wgmma_commit();
+          wgmma_wait0();
+          // partial dQ_i = dS K_j into the work area, then this thread's row into the fp32 scratch
+          wg_mma_128<HDP, 0, 1, 8>(
+          work, G_LD,
+              [&](int h, int ks) {
+                return make_smem_desc(sDSu + (ks >> 2) * (AL_ROWS * 128) + h * 64 * 128 + (ks & 3) * 32, 16, 1024, SWZ_128B);
+              },
+              [&](int ks) { return make_smem_desc(sK + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, false);
+          named_bar_sync(1, 128);
+          if (tid == 0) mbar_arrive(&qdo_empty[qs]);  // Q_i / dO_i consumed
+          if (row_ok) {
+            float* drow = pl.dq32 + (row0 + q) * pl.lddq32 + head * HDP;
+            const float* arow = work + r * G_LD;
+#pragma unroll
+            for (int c0 = 0; c0 < HDP; c0 += 4) {
+              const float4 a = *reinterpret_cast<const float4*>(arow + c0);
+              const float v0 = a.x * p.scale, v1 = a.y * p.scale, v2 = a.z * p.scale, v3 = a.w * p.scale;
+              if (j == 0)
+                *reinterpret_cast<float4*>(drow + c0) = make_float4(v0, v1, v2, v3);
+              else
+                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(drow + c0), "f"(v0), "f"(v1), "f"(v2),
+                             "f"(v3)
+                             : "memory");
+            }
           }
         }
-        // every MMA of this key tile is complete: the last pair's dQ partial, then dV_j / dK_j (row r = key j*128 + r)
-        mbar_wait(dkv_full, jcnt & 1);
-        tc_fence_after();
-        flush_dq(j, nt - 1);
+        // every MMA of this key tile is complete: K_j / V_j are free; dK_j / dV_j (row r = key j*128 + r) through the
+        // work area
+        named_bar_sync(1, 128);
+        if (tid == 0) mbar_arrive(kv_empty);
+        float* gk = work;
+        float* gv = work + AL_ROWS * G_LD;
+        acc_store<HDP>(gk, G_LD, dk[0]);
+        acc_store<HDP>(gk + 64 * G_LD, G_LD, dk[1]);
+        acc_store<HDP>(gv, G_LD, dv[0]);
+        acc_store<HDP>(gv + 64 * G_LD, G_LD, dv[1]);
+        named_bar_sync(1, 128);
         {
           const int key = j * 128 + r;
           const bool ok = key < S;
           __half* orow = p.dqkv + (row0 + key) * p.lddq + head * HDP;
 #pragma unroll
           for (int which = 1; which < 3; ++which) {
-            const uint32_t tsrc = (which == 1 ? tDK : tDV) + lane_off;
+            const float* src = (which == 1 ? gk : gv) + r * G_LD;
             const float mul = which == 1 ? p.scale : 1.f;
 #pragma unroll
-            for (int c0 = half * 32; c0 < HDP; c0 += 64) {
+            for (int c0 = 0; c0 < HDP; c0 += 32) {
               uint32_t raw[32];
-              tmem_ld32(tsrc + c0, raw);
-              tmem_ld_wait();
+              ld_row32(src + c0, raw);
               if (ok) {
 #pragma unroll
                 for (int qq = 0; qq < 4; ++qq) {
@@ -1089,11 +637,8 @@ __global__ void __launch_bounds__(ALL_THREADS, 1)
             }
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(dkv_empty);
       }
-      // dQ rows of this (window, head): fp32 scratch (each column range written by this thread only) -> fp16
+      // dQ rows of this (window, head): fp32 scratch (each row written by this thread only) -> fp16
       __threadfence();
       for (int i = 0; i < nt; ++i) {
         const int q = i * 128 + r;
@@ -1101,34 +646,25 @@ __global__ void __launch_bounds__(ALL_THREADS, 1)
           const float* drow = pl.dq32 + (row0 + q) * pl.lddq32 + head * HDP;
           __half* orow = p.dqkv + (row0 + q) * p.lddq + head * HDP;
 #pragma unroll
-          for (int c0 = half * 32; c0 < HDP; c0 += 64) {
-#pragma unroll
-            for (int c = c0; c < c0 + 32; c += 8) {
-              const float4 a = __ldcg(reinterpret_cast<const float4*>(drow + c));
-              const float4 b = __ldcg(reinterpret_cast<const float4*>(drow + c + 4));
-              const __half2 h0 = __floats2half2_rn(a.x, a.y), h1 = __floats2half2_rn(a.z, a.w);
-              const __half2 h2 = __floats2half2_rn(b.x, b.y), h3 = __floats2half2_rn(b.z, b.w);
-              *reinterpret_cast<uint4*>(orow + c) =
-                  make_uint4(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1),
-                             *reinterpret_cast<const uint32_t*>(&h2), *reinterpret_cast<const uint32_t*>(&h3));
-            }
+          for (int c = 0; c < HDP; c += 8) {
+            const float4 a = __ldcg(reinterpret_cast<const float4*>(drow + c));
+            const float4 b = __ldcg(reinterpret_cast<const float4*>(drow + c + 4));
+            const __half2 h0 = __floats2half2_rn(a.x, a.y), h1 = __floats2half2_rn(a.z, a.w);
+            const __half2 h2 = __floats2half2_rn(b.x, b.y), h3 = __floats2half2_rn(b.z, b.w);
+            *reinterpret_cast<uint4*>(orow + c) =
+                make_uint4(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1),
+                           *reinterpret_cast<const uint32_t*>(&h2), *reinterpret_cast<const uint32_t*>(&h3));
           }
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
 template <int HDP>
 static int launch_attn_loop_bwd_long(const CUtensorMap& tq, const CUtensorMap& td, const AttnLoopBwdLongParams& p,
                                      cudaStream_t st) {
-  const size_t smem = 1024 + (size_t)8 * AL_ROWS * HDP * 2 + 2 * AL_ROWS * 128 * 2 + 256 + (size_t)p.b.nt * 128 * 8;
+  const size_t smem = 1024 + (size_t)AttnBwdLongSmem<HDP>::ROWV_OFF + (size_t)p.b.nt * 128 * 8;
   FVIT_CHECK(smem <= 227 * 1024, "fvit_attn_loop_bwd_long: S=%d needs %zu bytes of shared memory", p.b.S, smem);
   static size_t configured = 0;
   if (smem > configured) {
@@ -1142,38 +678,6 @@ static int launch_attn_loop_bwd_long(const CUtensorMap& tq, const CUtensorMap& t
 }
 
 }  // namespace fvit
-
-extern "C" int fvit_attn_loop_bwd(const void* qkv, int64_t ldq, const void* dout, int64_t lddo, const void* out, int64_t ldo,
-                                  const float* lse, int32_t groups, int32_t S, int32_t heads, int32_t hdp, const float* bias,
-                                  float scale, void* dqkv, int64_t lddq, float* dbias, void* stream) {
-  using namespace fvit;
-  FVIT_CHECK(qkv && dout && out && lse && dqkv && groups > 0 && heads > 0, "fvit_attn_loop_bwd: bad arguments");
-  FVIT_CHECK(S > 128 && S <= 256, "fvit_attn_loop_bwd: S=%d unsupported (129..256: two tiles of TMEM accumulators)", S);
-  FVIT_CHECK(S % 4 == 0, "fvit_attn_loop_bwd: S=%d must be a multiple of 4 (16-byte bias / dbias accesses)", S);
-  FVIT_CHECK(hdp == 32 || hdp == 64, "fvit_attn_loop_bwd: padded head dim %d unsupported", hdp);
-  FVIT_CHECK(ldq % 8 == 0 && lddo % 8 == 0 && ldo % 8 == 0 && lddq % 8 == 0, "fvit_attn_loop_bwd: bad leading dimensions");
-  AttnLoopBwdParams p;
-  p.groups = groups, p.S = S, p.heads = heads, p.nt = (S + 127) / 128;
-  p.scale = scale, p.scale_log2e = scale * 1.4426950408889634f;
-  p.bias = bias, p.dbias = dbias, p.lse = lse;
-  p.dout = (const __half*)dout, p.lddo = lddo, p.out = (const __half*)out, p.ldo = ldo;
-  p.dqkv = (__half*)dqkv, p.lddq = lddq;
-  CUtensorMap tq, td;
-  const CUtensorMapSwizzle swz = hdp == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  uint32_t box[2] = {(uint32_t)hdp, (uint32_t)AL_ROWS};
-  {
-    uint64_t dims[2] = {(uint64_t)(3 * heads * hdp), (uint64_t)groups * S};
-    uint64_t strides[1] = {(uint64_t)ldq * 2};
-    int rc = cached_tmap_16bit(&tq, qkv, 2, dims, strides, box, swz);
-    if (rc) return rc;
-    uint64_t dims2[2] = {(uint64_t)(heads * hdp), (uint64_t)groups * S};
-    uint64_t strides2[1] = {(uint64_t)lddo * 2};
-    rc = cached_tmap_16bit(&td, dout, 2, dims2, strides2, box, swz);
-    if (rc) return rc;
-  }
-  if (hdp == 64) return launch_attn_loop_bwd<64>(tq, td, p, (cudaStream_t)stream);
-  return launch_attn_loop_bwd<32>(tq, td, p, (cudaStream_t)stream);
-}
 
 extern "C" int fvit_attn_loop_bwd_long(const void* qkv, int64_t ldq, const void* dout, int64_t lddo, const void* out,
                                        int64_t ldo, const float* lse, int32_t groups, int32_t S, int32_t heads, int32_t hdp,

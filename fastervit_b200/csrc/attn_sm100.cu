@@ -1,17 +1,16 @@
-// fvit_attn_tc_fwd: tensor-core attention core of WindowAttention.forward (fv.py:559-565) for sm_100a.
+// fvit_attn_tc_fwd: tensor-core attention core of WindowAttention.forward (fv.py:559-565) for sm_90a.
 //
 // Work item = (tile of 128 consecutive token rows, head). A tile holds gpt = floor(128 / S) whole
 // windows (groups of S tokens: ct_size^2 carrier tokens + ws^2 window tokens, or the carrier grid of
 // one image); rows of the box beyond gpt*S belong to the next tile and are masked.
 //
-//   warp 0     : TMA producer — Q, K, V head slices (128 x hdp, 16-bit) of the packed qkv matrix into
-//                a 2-stage ring of swizzled shared-memory tiles
-//   warp 1     : MMA issuer — S = Q K^T  (tcgen05.mma, M=128, N=128, K=hdp, fp32 in TMEM, 2 stages)
-//                and O = P V (A = P from shared memory, B = V as an MN-major operand, N = hdp)
-//   warps 2..5 : softmax — one thread per query row: tcgen05.ld of its 128 scores, block-diagonal
-//                window mask, relative-position bias from shared memory, fp32 max / exp2 / sum,
-//                P written as fp16 straight into the UMMA (128B-swizzled) operand layout; then the
-//                O epilogue (1/rowsum, fp16, 16-byte stores).
+//   warp 4     : TMA producer — Q, K, V head slices (128 x hdp, 16-bit) of the packed qkv matrix into
+//                a ring of swizzled shared-memory tiles
+//   warps 0..3 : one warpgroup — S = Q K^T (wgmma, M=128 as two m64 halves, N=128, K=hdp) into an fp32
+//                score tile in shared memory; softmax with one thread per query row: block-diagonal
+//                window mask, relative-position bias from shared memory, fp32 max / exp2 / sum, P written
+//                as fp16 straight into the 128B-swizzled operand layout; O = P V (B = V as an MN-major
+//                operand, N = hdp) into the same tile; then the O epilogue (1/rowsum, fp16, 16-byte stores).
 // Scores and probabilities never touch HBM; per row the kernel reads 3*hdp*2 B and writes hdp*2 B.
 #include <cuda_fp16.h>
 
@@ -24,8 +23,11 @@
 
 namespace fvit {
 
-constexpr int AT_THREADS = 192;
+constexpr int AT_THREADS = 160;
 constexpr int AT_ROWS = 128;
+constexpr int AT_PRODUCER = 4;           // the TMA warp; warps 0..3 are the compute warpgroup
+constexpr int AT_ACC_LD = 132;           // floats per row of the fp32 accumulator tile (conflict-free float4 rows)
+constexpr int AT_ACC_BYTES = AT_ROWS * AT_ACC_LD * 4;
 
 struct AttnParams {
   int groups, S, heads, gpt, tiles;
@@ -39,24 +41,21 @@ struct AttnParams {
 
 template <int HDP>
 struct AttnSmem {
-  static constexpr int NST = HDP == 32 ? 2 : 1;              // Q/K/V ring depth (2 CTAs per SM either way)
+  static constexpr int NST = HDP == 32 ? 2 : 1;              // Q/K/V ring depth
   static constexpr int TILE_BYTES = AT_ROWS * HDP * 2;       // one of Q / K / V
   static constexpr int STAGE_BYTES = 3 * TILE_BYTES;
   static constexpr int P_BYTES = AT_ROWS * 128 * 2;          // 128 x 128 fp16, two 64-wide K atoms
   static constexpr int P_OFF = NST * STAGE_BYTES;
-  static constexpr int BIAS_OFF = P_OFF + P_BYTES;
+  static constexpr int ACC_OFF = P_OFF + P_BYTES;
+  static constexpr int BIAS_OFF = ACC_OFF + AT_ACC_BYTES;
 };
-
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
 
 // Window w of a tile lives in rows [w*slot, w*slot + S) of the 128-row operand tiles (slot = 16/32/64/
 // 128), so a query row only ever meets the keys of its own slot: the S x S diagonal blocks of the
 // 128 x 128 score matrix. Rows >= S of a slot hold the first rows of the next window (harmless:
 // masked as keys, not written as queries).
 template <int HDP>
-__global__ void __launch_bounds__(AT_THREADS, 2)
+__global__ void __launch_bounds__(AT_THREADS, 1)
     attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ AttnParams p) {
   using SM = AttnSmem<HDP>;
   constexpr int NST = SM::NST;
@@ -68,39 +67,25 @@ __global__ void __launch_bounds__(AT_THREADS, 2)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = p.S;
   float* bias_s = reinterpret_cast<float*>(smem + SM::BIAS_OFF);
+  float* acc = reinterpret_cast<float*>(smem + SM::ACC_OFF);
   uint8_t* ctrl = smem + SM::BIAS_OFF + ((S * S * 4 + 15) & ~15);
   uint64_t* qkv_full = reinterpret_cast<uint64_t*>(ctrl);  // [2]
   uint64_t* qkv_empty = qkv_full + 2;                      // [2]
-  uint64_t* s_full = qkv_empty + 2;                        // [2]
-  uint64_t* s_empty = s_full + 2;                          // [2]
-  uint64_t* p_full = s_empty + 2;                          // [1]
-  uint64_t* o_full = p_full + 1;                           // [1]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 1);
 
-  if (warp == 0 && lane == 0) {
+  if (warp == AT_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmap_qkv);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&qkv_full[i], 1);
       mbar_init(&qkv_empty[i], 1);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_empty[i], 4);
     }
-    mbar_init(p_full, 4);
-    mbar_init(o_full, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // two score stages of 128 fp32 columns; O (HDP columns) overwrites the stage it was computed from
-  const uint32_t tmem_S[2] = {tmem_base, tmem_base + 128};
 
   const int items = p.tiles * p.heads;
   const int nslots = AT_ROWS / p.slot;
 
-  if (warp == 0) {
+  if (warp == AT_PRODUCER) {
     if (lane == 0) {
       int it = 0;
       for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
@@ -121,56 +106,11 @@ __global__ void __launch_bounds__(AT_THREADS, 2)
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc1 = make_idesc_f16(128, 128, 0, 0);
-      const uint32_t idesc2 = make_idesc_f16(128, HDP, 0, 1);  // B = V, MN-major
-      const uint32_t sP = smem_u32(smem + SM::P_OFF);
-      auto issue_pv = [&](int j) {
-        // O = P V for item j (local index): waits for the softmax warps' P; O lands on S stage j&1
-        mbar_wait(p_full, j & 1);
-        tc_fence_after();
-        const uint32_t sV = smem_u32(smem + (j % NST) * SM::STAGE_BYTES + 2 * SM::TILE_BYTES);
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {  // 128 keys in steps of 16
-          const uint64_t ad = make_smem_desc(sP + (ks >> 2) * (AT_ROWS * 128) + (ks & 3) * 32, 16, 1024, SWZ_128B);
-          const uint64_t bd = make_smem_desc(sV + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ);
-          umma_f16_ss(tmem_S[j & 1], ad, bd, idesc2, ks > 0 ? 1u : 0u);
-        }
-        umma_commit(o_full);
-        umma_commit(&qkv_empty[j % NST]);
-      };
-      int it = 0;
-      for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
-        const int st = it % NST;
-        const uint32_t ph = (it / NST) & 1;
-        const int ss = it & 1;
-        mbar_wait(&qkv_full[st], ph);
-        mbar_wait(&s_empty[ss], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t sQ = smem_u32(smem + st * SM::STAGE_BYTES);
-        const uint32_t sK = sQ + SM::TILE_BYTES;
-#pragma unroll
-        for (int k = 0; k < HDP / 16; ++k) {
-          const uint64_t ad = make_smem_desc(sQ + k * 32, 16, SBO_QKV, SWZ);
-          const uint64_t bd = make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ);
-          umma_f16_ss(tmem_S[ss], ad, bd, idesc1, k > 0 ? 1u : 0u);
-        }
-        umma_commit(&s_full[ss]);
-        if (NST == 1) {
-          // single operand stage: the next item's loads need this item's P V to retire first
-          issue_pv(it);
-        } else if (it > 0) {
-          issue_pv(it - 1);
-        }
-      }
-      if (NST == 2 && it > 0) issue_pv(it - 1);
-    }
   } else {
-    // ------------------------------------------------------------------ softmax + epilogue warps
+    // ------------------------------------------------------------------ MMA + softmax + epilogue warpgroup
     const int quad = warp & 3;
     const int r = quad * 32 + lane;    // row in tile
-    const int tid = threadIdx.x - 64;  // 0..127 among the softmax threads
+    const int tid = threadIdx.x;       // 0..127
     const int slot = p.slot;
     const int sl = r / slot;           // window slot of this row
     const int j = r - sl * slot;       // token index inside the window
@@ -180,6 +120,8 @@ __global__ void __launch_bounds__(AT_THREADS, 2)
     const int wn = slot >= 32 ? S : 32;            // columns to visit starting at wlo
     const int nch = (wn + 31) / 32;
     uint8_t* sP = smem + SM::P_OFF;
+    const uint32_t sP_u = smem_u32(sP);
+    const float* arow = acc + r * AT_ACC_LD;
     // columns outside [wlo, wlo + 32*nch) are never written by this warp's rows: zero them once
     for (int c = 0; c < 128; c += 8) {
       if (c + 8 <= wlo || c >= wlo + 32 * nch)
@@ -189,8 +131,8 @@ __global__ void __launch_bounds__(AT_THREADS, 2)
     int it = 0;
     int staged_head = -1;
     for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
-      const int ss = it & 1;
-      const uint32_t sph = (it >> 1) & 1;
+      const int st = it % NST;
+      const uint32_t ph = (it / NST) & 1;
       const int head = w / p.tiles, tile = w % p.tiles;
       const int grp = tile * p.gpt + sl;
       const bool row_ok = j < S && sl < p.gpt && grp < p.groups;
@@ -217,9 +159,16 @@ __global__ void __launch_bounds__(AT_THREADS, 2)
         staged_head = head;
       }
 
-      mbar_wait(&s_full[ss], sph);
-      tc_fence_after();
-      const uint32_t ts = tmem_S[ss] + ((uint32_t)(quad * 32) << 16);
+      mbar_wait(&qkv_full[st], ph);
+      const uint32_t sQ = smem_u32(smem + st * SM::STAGE_BYTES);
+      const uint32_t sK = sQ + SM::TILE_BYTES;
+      const uint32_t sV = sQ + 2 * SM::TILE_BYTES;
+      named_bar_sync(1, 128);  // the previous item's O reads of the accumulator tile are done
+      wg_mma_128<128, 0, 0, HDP / 16>(
+          acc, AT_ACC_LD,
+          [&](int h, int k) { return make_smem_desc(sQ + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
+          [&](int k) { return make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ); }, false);
+      named_bar_sync(1, 128);
       // brow[c - lo] = bias of (this row, key c); rows that are not real queries read row 0 (unused)
       const float* brow = bias_s + (row_ok ? j : 0) * S;
       const bool use_bias = p.bias != nullptr;
@@ -228,8 +177,7 @@ __global__ void __launch_bounds__(AT_THREADS, 2)
       for (int ch = 0; ch < nch; ++ch) {
         const int c0 = wlo + 32 * ch;
         uint32_t raw[32];
-        tmem_ld32(ts + c0, raw);
-        tmem_ld_wait();
+        ld_row32(arow + c0, raw);
 #pragma unroll
         for (int u = 0; u < 32; ++u) {
           const int kk = c0 + u - lo;               // key index inside the window
@@ -245,8 +193,7 @@ __global__ void __launch_bounds__(AT_THREADS, 2)
       for (int ch = 0; ch < nch; ++ch) {
         const int c0 = wlo + 32 * ch;
         uint32_t raw[32];
-        tmem_ld32(ts + c0, raw);
-        tmem_ld_wait();
+        ld_row32(arow + c0, raw);
         uint32_t pk[16];
 #pragma unroll
         for (int u = 0; u < 32; u += 2) {
@@ -273,22 +220,24 @@ __global__ void __launch_bounds__(AT_THREADS, 2)
                 make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
         }
       }
-      // P is complete for this warp's rows: publish to the async proxy and signal the MMA warp
+      // P is complete: publish it to the async proxy; every score read is done before O overwrites the tile
       fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      // O epilogue (O overwrote the score stage)
-      mbar_wait(o_full, it & 1);
-      tc_fence_after();
+      named_bar_sync(1, 128);
+      wg_mma_128<HDP, 0, 1, 8>(
+          acc, AT_ACC_LD,  // 128 keys in steps of 16
+          [&](int h, int ks) {
+            return make_smem_desc(sP_u + (ks >> 2) * (AT_ROWS * 128) + h * 64 * 128 + (ks & 3) * 32, 16, 1024, SWZ_128B);
+          },
+          [&](int ks) { return make_smem_desc(sV + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, false);
+      named_bar_sync(1, 128);
+      if (tid == 0) mbar_arrive(&qkv_empty[st]);  // Q / K / V of this stage are consumed
       const float inv = row_ok ? 1.f / sum : 0.f;
       const long long grow = (long long)grp * S + j;
       __half* orow = p.out + grow * p.ldo + head * HDP;
 #pragma unroll
       for (int c0 = 0; c0 < HDP; c0 += 32) {
         uint32_t raw[32];
-        tmem_ld32(ts + c0, raw);
-        tmem_ld_wait();
+        ld_row32(arow + c0, raw);
         if (row_ok) {
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
@@ -303,17 +252,7 @@ __global__ void __launch_bounds__(AT_THREADS, 2)
           }
         }
       }
-      // scores and O of this stage are consumed: hand the TMEM stage back
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_empty[ss]);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
   }
 }
 
@@ -325,9 +264,7 @@ static int launch_attn(const CUtensorMap& tm, const AttnParams& p, size_t smem, 
     configured = true;
   }
   const int items = p.tiles * p.heads;
-  // the kernel is built for two resident CTAs per SM (__launch_bounds__(192, 2), <= 113 KB of shared memory each):
-  // one CTA's softmax / epilogue phase overlaps the other's TMA + MMA phase
-  const int slots = (smem <= 113 * 1024 ? 2 : 1) * num_sms();
+  const int slots = num_sms();
   attn_tc_kernel<HDP><<<items < slots ? items : slots, AT_THREADS, smem, st>>>(tm, p);
   return post_launch("attn_tc_kernel");
 }
@@ -375,11 +312,11 @@ extern "C" int fvit_attn_tc_fwd(const void* qkv, int64_t ldq, int32_t groups, in
 
 // =====================================================================================================
 // fvit_attn_tc_bwd: tensor-core backward of the attention core for S <= 64 (window slots of 16/32/64 rows).
-//   S  = Q K^T, dP = dO V^T                     (tcgen05, 128x128 each, TMEM columns [0,128) and [128,256))
+//   S  = Q K^T, dP = dO V^T                     (wgmma, 128x128 each, in turn in one fp32 shared-memory tile)
 //   per query row (one thread each): P = softmax(S*scale + bias), delta = sum_c P*dP, dS = P*(dP - delta);
 //       P and dS written as fp16 into two 128x128 swizzled operand tiles; dS accumulated into a per-CTA
 //       shared-memory copy of dbias[head] (flushed with global atomics when the head changes)
-//   dV = P^T dO, dK = dS^T Q (A = the tile read MN-major), dQ = dS K   -> TMEM, scaled, stored fp16.
+//   dV = P^T dO, dK = dS^T Q (A = the tile read MN-major), dQ = dS K   -> the same tile, scaled, stored fp16.
 // Scores / probabilities never touch HBM; per row the kernel reads 4*hdp*2 B and writes 3*hdp*2 B.
 namespace fvit {
 
@@ -401,47 +338,32 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
   constexpr uint32_t SBO_QKV = 8 * ROW_BYTES;
   constexpr int TILE_BYTES = AT_ROWS * HDP * 2;
   constexpr int STAGE_BYTES = 4 * TILE_BYTES;  // Q, K, V, dO
-  constexpr int NST = 2;
+  constexpr int NST = HDP == 32 ? 2 : 1;
   constexpr int P_OFF = NST * STAGE_BYTES;
   constexpr int DS_OFF = P_OFF + AT_ROWS * 128 * 2;
-  constexpr int BIAS_OFF = DS_OFF + AT_ROWS * 128 * 2;
+  constexpr int ACC_OFF = DS_OFF + AT_ROWS * 128 * 2;
+  constexpr int BIAS_OFF = ACC_OFF + AT_ACC_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = p.S;
   const int SS = (S * S * 4 + 15) & ~15;
   float* bias_s = reinterpret_cast<float*>(smem + BIAS_OFF);
+  float* acc = reinterpret_cast<float*>(smem + ACC_OFF);
   uint8_t* ctrl = smem + BIAS_OFF + SS;
   uint64_t* ld_full = reinterpret_cast<uint64_t*>(ctrl);  // [2]
   uint64_t* ld_empty = ld_full + 2;                        // [2]
-  uint64_t* sdp_full = ld_empty + 2;                       // [1]
-  uint64_t* pds_full = sdp_full + 1;                       // [1]
-  uint64_t* grads_full = pds_full + 1;                     // [1]
-  uint64_t* tmem_empty = grads_full + 1;                   // [1]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 1);
 
-  if (warp == 0 && lane == 0) {
+  if (warp == AT_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmap_qkv);
     tma_prefetch_desc(&tmap_do);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&ld_full[i], 1);
       mbar_init(&ld_empty[i], 1);
     }
-    mbar_init(sdp_full, 1);
-    mbar_init(pds_full, 4);
-    mbar_init(grads_full, 1);
-    mbar_init(tmem_empty, 4);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // scores / dP and the three gradient accumulators live in disjoint TMEM columns: the S / dP MMAs of item i+1 are
-  // issued while the softmax warps still drain the gradients of item i
-  const uint32_t tS = tmem_base, tDP = tmem_base + 128;
-  const uint32_t tDV = tmem_base + 256, tDK = tmem_base + 320, tDQ = tmem_base + 384;
 
   const int nslots = AT_ROWS / p.slot;
   // Item order: with at least one CTA per head every CTA stays on ONE head (CTA c: head c % heads, every n_h-th tile
@@ -462,11 +384,11 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
     }
   };
 
-  if (warp == 0) {
+  if (warp == AT_PRODUCER) {
     if (lane == 0) {
       for (int it = 0; it < n_items; ++it) {
-        const int st = it & 1;
-        const uint32_t ph = (it >> 1) & 1;
+        const int st = it % NST;
+        const uint32_t ph = (it / NST) & 1;
         int head, tile;
         item_of(it, head, tile);
         mbar_wait(&ld_empty[st], ph ^ 1);
@@ -482,57 +404,11 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t id_ss = make_idesc_f16(128, 128, 0, 0);
-      const uint32_t id_tn = make_idesc_f16(128, HDP, 1, 1);  // A = tile read MN-major (M = keys), B MN-major
-      const uint32_t id_dq = make_idesc_f16(128, HDP, 0, 1);
-      const uint32_t sP = smem_u32(smem + P_OFF), sDS = smem_u32(smem + DS_OFF);
-      for (int it = 0; it < n_items; ++it) {
-        const int st = it & 1;
-        const uint32_t ph = (it >> 1) & 1;
-        mbar_wait(&ld_full[st], ph);
-        // (S / dP of the previous item were consumed before its P / dS tiles were published: pds_full, waited below)
-        tc_fence_after();
-        const uint32_t sQ = smem_u32(smem + st * STAGE_BYTES);
-        const uint32_t sK = sQ + TILE_BYTES, sV = sQ + 2 * TILE_BYTES, sDO = sQ + 3 * TILE_BYTES;
-#pragma unroll
-        for (int k = 0; k < HDP / 16; ++k) {
-          umma_f16_ss(tS, make_smem_desc(sQ + k * 32, 16, SBO_QKV, SWZ), make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ),
-                      id_ss, k > 0 ? 1u : 0u);
-        }
-#pragma unroll
-        for (int k = 0; k < HDP / 16; ++k) {
-          umma_f16_ss(tDP, make_smem_desc(sDO + k * 32, 16, SBO_QKV, SWZ), make_smem_desc(sV + k * 32, 16, SBO_QKV, SWZ),
-                      id_ss, k > 0 ? 1u : 0u);
-        }
-        umma_commit(sdp_full);
-        mbar_wait(pds_full, it & 1);
-        mbar_wait(tmem_empty, (it & 1) ^ 1);  // the previous item's dV / dK / dQ have been read out
-        tc_fence_after();
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {  // K = 128 query rows in steps of 16
-          const uint64_t aP = make_smem_desc(sP + ks * 2048, AT_ROWS * 128, 1024, SWZ_128B);    // MN-major: LBO = next key atom
-          const uint64_t aDS = make_smem_desc(sDS + ks * 2048, AT_ROWS * 128, 1024, SWZ_128B);
-          const uint64_t bDO = make_smem_desc(sDO + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ);
-          const uint64_t bQ = make_smem_desc(sQ + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ);
-          umma_f16_ss(tDV, aP, bDO, id_tn, ks > 0 ? 1u : 0u);
-          umma_f16_ss(tDK, aDS, bQ, id_tn, ks > 0 ? 1u : 0u);
-        }
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {  // K = 128 keys
-          const uint64_t aDS = make_smem_desc(sDS + (ks >> 2) * (AT_ROWS * 128) + (ks & 3) * 32, 16, 1024, SWZ_128B);
-          const uint64_t bK = make_smem_desc(sK + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ);
-          umma_f16_ss(tDQ, aDS, bK, id_dq, ks > 0 ? 1u : 0u);
-        }
-        umma_commit(grads_full);
-        umma_commit(&ld_empty[st]);
-      }
-    }
   } else {
     const int quad = warp & 3;
     const int r = quad * 32 + lane;
-    const int tid = threadIdx.x - 64;
+    const int tid = threadIdx.x;
+    const float* arow = acc + r * AT_ACC_LD;
     const int slot = p.slot;
     const int sl = r / slot;
     const int j = r - sl * slot;
@@ -594,10 +470,17 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
         named_bar_sync(1, 128);
         staged_head = head;
       }
-      mbar_wait(sdp_full, it & 1);
-      tc_fence_after();
-      const uint32_t ts = tS + ((uint32_t)(quad * 32) << 16);
-      const uint32_t tdp = tDP + ((uint32_t)(quad * 32) << 16);
+      const int st = it % NST;
+      mbar_wait(&ld_full[st], (it / NST) & 1);
+      const uint32_t sQ = smem_u32(smem + st * STAGE_BYTES);
+      const uint32_t sK = sQ + TILE_BYTES, sV = sQ + 2 * TILE_BYTES, sDO = sQ + 3 * TILE_BYTES;
+      const uint32_t sPu = smem_u32(sP), sDSu = smem_u32(sDS);
+      named_bar_sync(1, 128);  // the previous item's gradient reads of the accumulator tile are done
+      wg_mma_128<128, 0, 0, HDP / 16>(
+          acc, AT_ACC_LD,
+          [&](int h, int k) { return make_smem_desc(sQ + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
+          [&](int k) { return make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ); }, false);
+      named_bar_sync(1, 128);
       const float* brow = bias_s + (row_ok ? j : 0) * S;
       const bool use_bias = p.bias != nullptr;
       float e[64];
@@ -607,8 +490,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
         if (ch < nch) {
           const int c0 = wlo + 32 * ch;
           uint32_t raw[32];
-          tmem_ld32(ts + c0, raw);
-          tmem_ld_wait();
+          ld_row32(arow + c0, raw);
 #pragma unroll
           for (int u = 0; u < 32; ++u) {
             const int kk = c0 + u - lo;
@@ -632,14 +514,19 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
         sum += v;
       }
       const float inv = row_ok ? 1.f / sum : 0.f;
+      named_bar_sync(1, 128);  // every score read is done: dP = dO V^T overwrites the tile
+      wg_mma_128<128, 0, 0, HDP / 16>(
+          acc, AT_ACC_LD,
+          [&](int h, int k) { return make_smem_desc(sDO + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
+          [&](int k) { return make_smem_desc(sV + k * 32, 16, SBO_QKV, SWZ); }, false);
+      named_bar_sync(1, 128);
       float delta = 0.f;
 #pragma unroll
       for (int ch = 0; ch < 2; ++ch) {
         if (ch < nch) {
           const int c0 = wlo + 32 * ch;
           uint32_t raw[32];
-          tmem_ld32(tdp + c0, raw);
-          tmem_ld_wait();
+          ld_row32(arow + c0, raw);
 #pragma unroll
           for (int u = 0; u < 32; ++u) {
             e[32 * ch + u] *= inv;  // normalised probability
@@ -652,8 +539,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
         if (ch < nch) {
           const int c0 = wlo + 32 * ch;
           uint32_t raw[32];
-          tmem_ld32(tdp + c0, raw);
-          tmem_ld_wait();
+          ld_row32(arow + c0, raw);
           uint32_t pkp[16], pkd[16];
 #pragma unroll
           for (int u = 0; u < 32; u += 2) {
@@ -681,24 +567,35 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
         }
       }
       fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pds_full);
       // gradients: row r of dV / dK is key r, of dQ is query r — the same token of the window
-      mbar_wait(grads_full, it & 1);
-      tc_fence_after();
       const long long grow = (long long)grp * S + j;
       __half* orow = p.dqkv + grow * p.lddq + head * HDP;
       const int Cp = p.heads * HDP;
-#pragma unroll
+#pragma unroll 1
       for (int which = 0; which < 3; ++which) {
-        const uint32_t tsrc = (which == 0 ? tDQ : (which == 1 ? tDK : tDV)) + ((uint32_t)(quad * 32) << 16);
+        named_bar_sync(1, 128);  // P / dS are complete, the previous tile reads are done
+        if (which == 0) {        // dQ = dS K
+          wg_mma_128<HDP, 0, 1, 8>(
+          acc, AT_ACC_LD,
+              [&](int h, int ks) {
+                return make_smem_desc(sDSu + (ks >> 2) * (AT_ROWS * 128) + h * 64 * 128 + (ks & 3) * 32, 16, 1024, SWZ_128B);
+              },
+              [&](int ks) { return make_smem_desc(sK + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, false);
+        } else {                 // dK = dS^T Q, dV = P^T dO: A read MN-major (M = keys), K = 128 query rows
+          const uint32_t sA = which == 1 ? sDSu : sPu;
+          const uint32_t sB = which == 1 ? sQ : sDO;
+          wg_mma_128<HDP, 1, 1, 8>(
+          acc, AT_ACC_LD,
+              [&](int h, int ks) { return make_smem_desc(sA + h * (AT_ROWS * 128) + ks * 2048, AT_ROWS * 128, 1024, SWZ_128B); },
+              [&](int ks) { return make_smem_desc(sB + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, false);
+        }
+        named_bar_sync(1, 128);
+        if (which == 2 && tid == 0) mbar_arrive(&ld_empty[st]);  // Q / K / V / dO of this stage are consumed
         const float mul = which == 2 ? 1.f : p.scale;
 #pragma unroll
         for (int c0 = 0; c0 < HDP; c0 += 32) {
           uint32_t raw[32];
-          tmem_ld32(tsrc + c0, raw);
-          tmem_ld_wait();
+          ld_row32(arow + c0, raw);
           if (row_ok) {
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
@@ -714,17 +611,8 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tmem_empty);
     }
     flush_dbias(staged_head);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -777,7 +665,7 @@ extern "C" int fvit_attn_tc_bwd(const void* qkv, int64_t ldq, const void* dout, 
     if (rc) return rc;
   }
   const size_t ss = ((size_t)S * S * 4 + 15) / 16 * 16;
-  const size_t smem = 1024 + (size_t)2 * 4 * AT_ROWS * hdp * 2 + 2 * AT_ROWS * 128 * 2 + ss + 128;
+  const size_t smem = 1024 + (size_t)(hdp == 32 ? 2 : 1) * 4 * AT_ROWS * hdp * 2 + 2 * AT_ROWS * 128 * 2 + AT_ACC_BYTES + ss + 128;
   FVIT_CHECK(smem <= 227 * 1024, "fvit_attn_tc_bwd: needs %zu B of shared memory", smem);
   if (hdp == 64) return launch_attn_bwd<64>(tq, td, p, smem, (cudaStream_t)stream);
   return launch_attn_bwd<32>(tq, td, p, smem, (cudaStream_t)stream);

@@ -1,8 +1,8 @@
-"""Build libfvit_sm100.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libfvit_sm100.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 Usage: python -m fastervit_b200.csrc.build [--force] [--verbose]
-The .so is written next to the Python package (fastervit_b200/libfvit_sm100.so) so that it
-travels with the repo snapshot to the GPU box; objects go to fastervit_b200/csrc/build/.
+The .so is written next to the Python package (fastervit_b200/libfvit_sm100.so), where lib.py loads it from;
+objects go to fastervit_b200/csrc/build/.
 """
 from __future__ import annotations
 
@@ -17,7 +17,7 @@ from pathlib import Path
 CSRC = Path(__file__).resolve().parent
 PKG = CSRC.parent
 ROOT = PKG.parent
-# A/B builds: FVIT_BUILD_DEFINES="-DFVIT_GEMM_NEPI=12" FVIT_BUILD_OUT=libfvit_sm100_e12.so python -m fastervit_b200.csrc.build
+# A/B builds: FVIT_BUILD_DEFINES="-D..." FVIT_BUILD_OUT=libfvit_sm100_ab.so python -m fastervit_b200.csrc.build
 # (select at run time with FVIT_LIB=<path>); the default build takes neither.
 _EXTRA = os.environ.get("FVIT_BUILD_DEFINES", "").split()
 _OUT = os.environ.get("FVIT_BUILD_OUT", "libfvit_sm100.so")
@@ -25,7 +25,7 @@ LIB_PATH = PKG / _OUT
 OBJ_DIR = CSRC / ("build" if _OUT == "libfvit_sm100.so" else "build_" + Path(_OUT).stem)
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -84,7 +84,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     newest = max(o.stat().st_mtime for o in objs)
     if force or not LIB_PATH.exists() or LIB_PATH.stat().st_mtime < newest:
         cmd = [_nvcc(), "-shared", "-o", str(LIB_PATH), *map(str, objs),
-               "-gencode", "arch=compute_100a,code=sm_100a"]
+               "-gencode", "arch=compute_90a,code=sm_90a"]
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:
             raise RuntimeError(f"link failed:\n{res.stdout}\n{res.stderr}")

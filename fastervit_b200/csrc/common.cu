@@ -30,9 +30,9 @@ int num_sms() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     cudaDeviceProp p;
-    if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 148;
+    if (cudaGetDeviceProperties(&p, dev) != cudaSuccess) return 132;
     n = p.multiProcessorCount;
   }
   const int lim = g_sm_limit.load(std::memory_order_relaxed);

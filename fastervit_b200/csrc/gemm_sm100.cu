@@ -1,13 +1,13 @@
-// fvit_gemm: persistent, warp-specialised tcgen05 GEMM for sm_100a.
+// fvit_gemm: persistent, warp-specialised wgmma GEMM for sm_90a.
 //
-//   warp 0      : TMA producer (one elected lane) — cp.async.bulk.tensor boxes into a ring of
-//                 128B-swizzled shared-memory stages, mbarrier complete_tx signalling
-//   warp 1      : TMEM allocator + MMA issuer (one elected lane) — tcgen05.mma.kind::f16, M=128,
-//                 N = tile_n (runtime, multiple of 16), K=16 per instruction, fp32 accumulators in
-//                 TMEM, double-buffered (2 x 256 columns) so the epilogue of tile i overlaps the
-//                 main loop of tile i+1
-//   warps 2..9  : epilogue — tcgen05.ld (32 lanes x 32b x 32 columns), shared-memory transpose, fused
-//                 scale/shift/activation/layer-scale/residual, optional per-column statistics,
+//   warp 8      : TMA producer (one lane) — cp.async.bulk.tensor boxes into a ring of 128B-swizzled
+//                 shared-memory stages, mbarrier complete_tx signalling; it runs ahead into the next
+//                 tiles while the consumers work on their epilogue
+//   warps 0..7  : two consumer warpgroups — wgmma.mma_async m64 x N x 16 (N = the MMA width of the
+//                 tile, 32 / 64 / 96 / 128), warpgroup g owns rows [64g, 64g + 64) of the 128-row tile
+//                 with fp32 accumulators in registers; at the end of a tile both write them to a
+//                 shared-memory accumulator tile, and the eight warps run the epilogue from there:
+//                 fused scale/shift/activation/layer-scale/residual, optional per-column statistics,
 //                 row-map scatter, coalesced 16-byte global accesses
 //
 // The A operand of K-block kb is the 2-D box at row (m0 + tap_shift[tap]) of plane tap_plane[tap]:
@@ -27,26 +27,18 @@ namespace fvit {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 x 16-bit = 128 B: one SWIZZLE_128B row
-constexpr int UMMA_K = 16;
-// 12 epilogue warps: the epilogue is latency- and issue-bound (TMEM load, shared-memory transpose, global loads of the
-// residual / aux rows), three warps per scheduler hide it better than two -- measured r02f: fv4 fwd+bwd GEMM time
-// 47.5 -> 46.5 ms, fv0 14.7 -> 14.1 ms (A/B of two builds: -DFVIT_GEMM_NEPI=8 vs 12)
-#ifndef FVIT_GEMM_NEPI
-#define FVIT_GEMM_NEPI 12
-#endif
-constexpr int NEPI = FVIT_GEMM_NEPI;            // epilogue warps: a multiple of 4 (one TMEM lane quadrant each)
+constexpr int MMA_K = 16;
+constexpr int NEPI = 8;                         // consumer warps: two warpgroups, each owning 64 rows of the tile
 constexpr int EPI_THREADS = 32 * NEPI;
-constexpr int GEMM_THREADS = 64 + EPI_THREADS;  // TMA warp + MMA warp + the epilogue warps
-static_assert(NEPI % 4 == 0 && NEPI >= 8 && NEPI <= 16, "epilogue warps come in groups of four");
+constexpr int GEMM_THREADS = EPI_THREADS + 32;  // consumers + the TMA warp
 constexpr int MAX_STAGES = 8;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
-constexpr int TMEM_COLS = 512;
-constexpr int MAX_ACC = 8;  // accumulator stages in TMEM: 512 / (64 | 128 | 256 columns)
+constexpr int MAX_TILE_N = 128;             // widest MMA of the kernel (the accumulator tile lives in shared memory)
 constexpr int SMEM_BUDGET = 227 * 1024;
-constexpr int SMEM_CTRL_BYTES = 1024;  // barriers + tmem base, placed after the stage ring
+constexpr int SMEM_CTRL_BYTES = 1024;  // barriers, placed after the stage ring
 constexpr int SMEM_ALIGN_SLACK = 1024;
-constexpr int STG_LD = 36;  // floats per staging row: 32 + 4 pad -> conflict-free float4 access both ways
-constexpr int SMEM_STG_BYTES = NEPI * 32 * STG_LD * 4;  // one 32x32 fp32 staging tile per epilogue warp
+constexpr int ACC_LD = MAX_TILE_N + 4;  // floats per accumulator row: conflict-free float4 rows (4 banks apart)
+constexpr int SMEM_ACC_BYTES = BM * ACC_LD * 4;
 constexpr int STATS_MAX_N = 1024;                    // widest GEMM with per-column statistics (BatchNorm channels)
 constexpr int SMEM_STATS_BYTES = 2 * STATS_MAX_N * 4;
 
@@ -62,9 +54,7 @@ struct GemmParams {
   int b_ntaps, tiles_per_tap;  // >1: N tiles enumerate (tap, n tile); tap t reads B rows shifted by tap_shift[t]
   int atomic_out;  // split-K style accumulation: atomicAdd(alpha * acc) into out_f32
   int stages;
-  int cg;  // 1: one CTA per 128-row tile; 2: CTA pair (tcgen05 cta_group::2) per 256-row tile, B split over the pair
-  int acc_stride, nacc;  // TMEM columns per accumulator stage and number of stages
-  uint32_t idesc;
+  int mma_n;  // MMA width: tile_n rounded up to 32 / 64 / 96 / 128 (columns >= tile_n are computed and dropped)
   int tap_shift[16];
   int tap_plane[16];
   // epilogue
@@ -113,16 +103,16 @@ __device__ __forceinline__ uint32_t pack2_16(float a, float b, int bf16) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// 256-bit global accesses (sm_100: one full 32-byte sector per lane and instruction)
+// 32-byte global accesses as two 16-byte vector accesses (one full sector per lane)
 __device__ __forceinline__ void st_global_256(void* ptr, const uint32_t (&v)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(v[0]), "r"(v[1]), "r"(v[2]),
-               "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
+  uint4* q = reinterpret_cast<uint4*>(ptr);
+  q[0] = make_uint4(v[0], v[1], v[2], v[3]);
+  q[1] = make_uint4(v[4], v[5], v[6], v[7]);
 }
 __device__ __forceinline__ void ld_global_256(const void* ptr, uint32_t (&v)[8]) {
-  asm volatile("ld.global.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "l"(ptr));
+  const uint4* q = reinterpret_cast<const uint4*>(ptr);
+  const uint4 a = q[0], b = q[1];
+  v[0] = a.x, v[1] = a.y, v[2] = a.z, v[3] = a.w, v[4] = b.x, v[5] = b.y, v[6] = b.z, v[7] = b.w;
 }
 __device__ __forceinline__ float2 unpack2_16(uint32_t w, int bf16) {
   if (bf16) return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
@@ -190,7 +180,7 @@ enum : uint32_t {
   EF_RS = 1u << 12,
   EF_OSUM = 1u << 13,        // per-column sum of the rounded 16-bit output (bias gradient of the next layer)
   EF_PREGRAD = 1u << 14,     // out_pre16 receives gelu'(v) (consumed by FVIT_ACT_MUL_AUX in the backward pass)
-  EF_DIRECT = 1u << 15,      // 16-bit outputs only: row-per-thread epilogue straight from TMEM (no staging tile), 32-byte stores
+  EF_DIRECT = 1u << 15,      // 16-bit outputs only: row-per-thread epilogue, 32-byte stores
 };
 // work unit -> (M tile, N tile, K split). Plain GEMMs keep the K splits of a tile adjacent; the tap-in-N mode
 // walks all tiles of one K range first so concurrently running CTAs share the A / B slices in L2.
@@ -208,61 +198,107 @@ __device__ __forceinline__ void decode_work(const GemmParams& p, int w, int& tm,
   tm = t / p.tiles_n;
 }
 
-// CG = 1: one CTA per 128-row tile (no cluster instruction is compiled in); CG = 2: CTA pair (cluster launch).
-template <uint32_t FEAT, int CG>
+// Main loop of one work unit for MMA width N: the consumer warpgroup g accumulates rows [64g, 64g + 64) of the tile
+// over K blocks [kb0, kb1) and leaves them in the shared-memory accumulator tile. One K block's MMAs stay in flight
+// while the next block's are issued; each warp releases a ring stage once its warpgroup's MMAs on it have completed.
+template <int N, int TA, int TB, int BF16>
+__device__ __forceinline__ void gemm_mainloop(const GemmParams& p, uint8_t* smem, int stage_bytes, uint64_t* full_bar,
+                                              uint64_t* empty_bar, int& stage, uint32_t& phase, int kb0, int kb1,
+                                              float* accbuf) {
+  const int g = (threadIdx.x >> 7) & 1;
+  const int lane = threadIdx.x & 31;
+  // K-major SW128: SBO = 1024 (8 rows x 128 B), LBO unused; MN-major SW128: LBO = BK*128 (next 64-wide MN atom),
+  // SBO = 1024 (next 8 K rows). Rows 64..127 of A: 64 K-major rows on (8 KB) or the second 64-wide MN atom (8 KB).
+  constexpr uint32_t a_lbo = TA ? BK * 128 : 16;
+  constexpr uint32_t b_lbo = TB ? BK * 128 : 16;
+  constexpr uint32_t a_kstep = TA ? MMA_K * 128 : MMA_K * 2;
+  constexpr uint32_t b_kstep = TB ? MMA_K * 128 : MMA_K * 2;
+  float d[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  int prev = -1;  // ring stage of the K block whose MMAs are still in flight
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = smem_u32(smem + stage * stage_bytes) + g * 8192;
+    const uint32_t sb = smem_u32(smem + stage * stage_bytes) + A_STAGE_BYTES;
+    auto mma = [&](int k) {
+      Wgmma<N, TA, TB, BF16>::mma(d, make_smem_desc(sa + k * a_kstep, a_lbo, 1024, SWZ_128B),
+                                  make_smem_desc(sb + k * b_kstep, b_lbo, 1024, SWZ_128B), 1u);
+    };
+    // a tap's last K-block is zero beyond kc (TMA out-of-bounds fill / zero-padded weights): its all-zero
+    // 16-wide steps are not issued (K = 196 per conv tap: 13 instead of 16 MMAs; K = 784: 49 instead of 52)
+    const int nk = (kb + 1) % p.kb_per_tap == 0 ? p.k_tail16 : BK / MMA_K;
+    // (each case is a complete wgmma group: a branch between the MMAs of one group would serialize them)
+    switch (nk) {
+      case 1: wgmma_fence(); mma(0); wgmma_commit(); break;
+      case 2: wgmma_fence(); mma(0); mma(1); wgmma_commit(); break;
+      case 3: wgmma_fence(); mma(0); mma(1); mma(2); wgmma_commit(); break;
+      default: wgmma_fence(); mma(0); mma(1); mma(2); mma(3); wgmma_commit(); break;
+    }
+    wgmma_wait1();  // the previous K block's MMAs are complete
+    if (prev >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    }
+    prev = stage;
+    if (++stage == p.stages) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  wgmma_wait0();
+  if (prev >= 0) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+  }
+  acc_store<N>(accbuf + g * 64 * ACC_LD, ACC_LD, d);
+}
+
+template <int TA, int TB, int BF16>
+__device__ __forceinline__ void gemm_mainloop_n(const GemmParams& p, uint8_t* smem, int stage_bytes, uint64_t* full_bar,
+                                                uint64_t* empty_bar, int& stage, uint32_t& phase, int kb0, int kb1,
+                                                float* accbuf) {
+  switch (p.mma_n) {
+    case 32: gemm_mainloop<32, TA, TB, BF16>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf); break;
+    case 64: gemm_mainloop<64, TA, TB, BF16>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf); break;
+    case 96: gemm_mainloop<96, TA, TB, BF16>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf); break;
+    default: gemm_mainloop<128, TA, TB, BF16>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf); break;
+  }
+}
+
+template <uint32_t FEAT>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-    gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                        const __grid_constant__ CUtensorMap tmap_b,
-                        const __grid_constant__ GemmParams p) {
+    gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                      const __grid_constant__ CUtensorMap tmap_b,
+                      const __grid_constant__ GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // SW128 atoms
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  // CTA pair: this CTA stages its 128 rows of A and its half of the B tile; the leader issues M = 256 MMAs that
-  // read both CTAs' shared memory at the same offsets and write 128 accumulator rows into each CTA's TMEM
-  constexpr int cg = CG;
-  uint32_t cta_rank = 0u;
-  if constexpr (CG == 2) cta_rank = cluster_ctarank();
-  const bool leader = cta_rank == 0;
-  const int unit0 = blockIdx.x / cg, nunits = gridDim.x / cg;  // work units are dealt to CTAs / CTA pairs
-  const int b_cols = p.tile_n / cg;                            // B rows (N columns) staged by this CTA
-  // MN-major B is staged as whole 64-column atoms (the MMA reads the first b_cols columns of them)
-  const int b_stage_bytes = (p.b_mn ? ((b_cols + 63) & ~63) : b_cols) * BK * 2;
+  const int unit0 = blockIdx.x, nunits = gridDim.x;  // work units are dealt to CTAs round-robin
+  // MN-major B is staged as whole 64-column atoms (the MMA reads the first mma_n columns of them)
+  const int b_stage_bytes = (p.b_mn ? ((p.mma_n + 63) & ~63) : p.mma_n) * BK * 2;
   const int stage_bytes = A_STAGE_BYTES + b_stage_bytes;
   uint8_t* ctrl = smem + p.stages * stage_bytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ctrl);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
-  uint64_t* acc_full = empty_bar + MAX_STAGES;
-  uint64_t* acc_empty = acc_full + MAX_ACC;
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(acc_empty + MAX_ACC);
+  float* accbuf = reinterpret_cast<float*>(ctrl + SMEM_CTRL_BYTES);
 
-  if (warp == 0 && lane == 0) {
+  if (warp == NEPI && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < p.nacc; ++s) {
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], NEPI * cg);  // the leader's copy collects the epilogue warps of both CTAs
+      mbar_init(&empty_bar[s], NEPI);  // one arrival per consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if constexpr (CG == 2) tmem_alloc_cg2(tmem_base_slot, TMEM_COLS);
-    else tmem_alloc(tmem_base_slot, TMEM_COLS);
-  }
-  tc_fence_before();
-  if constexpr (CG == 2) cluster_sync_all();  // peer barriers are initialised before any remote arrive / TMA signal
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
+  __syncthreads();
 
   const int work_total = p.tiles_m * p.tiles_n * p.split_k;
 
-  if (warp == 0) {
+  if (warp == NEPI) {
     // ===================================================================== TMA producer
     if (lane == 0) {
       int stage = 0;
@@ -270,7 +306,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       for (int w = unit0; w < work_total; w += nunits) {
         int tm, tn, split;
         decode_work(p, w, tm, tn, split);
-        const int m0 = (tm * cg + (int)cta_rank) * BM;
+        const int m0 = tm * BM;
         int n0 = tn * p.tile_n;
         int b_shift = p.b_row_off;
         if (p.b_ntaps > 1) {
@@ -278,126 +314,49 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           n0 = (tn - tap * p.tiles_per_tap) * p.tile_n;
           b_shift += p.tap_shift[tap];
         }
-        n0 += (int)cta_rank * b_cols;
         const int kb0 = (int)((long long)p.num_kb * split / p.split_k);
         const int kb1 = (int)((long long)p.num_kb * (split + 1) / p.split_k);
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * stage_bytes;
           uint8_t* sb = sa + A_STAGE_BYTES;
-          // both CTAs' boxes complete on the leader's barrier, which expects the bytes of the whole pair
-          if (leader) mbar_expect_tx(&full_bar[stage], (uint32_t)(stage_bytes * cg));
-          if constexpr (CG == 1) {
-            if (!p.a_mn) {
-              const int tap = kb / p.kb_per_tap;
-              const int kc0 = (kb - tap * p.kb_per_tap) * BK;
-              tma_load_3d(sa, &tmap_a, &full_bar[stage], kc0, m0 + p.tap_shift[tap], p.tap_plane[tap]);
-            } else {
-              // A stored [K rows][M cols]: two 64-wide MN atoms of BK rows each
-              tma_load_3d(sa, &tmap_a, &full_bar[stage], m0, kb * BK + p.a_row_off, 0);
-              tma_load_3d(sa + BK * 128, &tmap_a, &full_bar[stage], m0 + 64, kb * BK + p.a_row_off, 0);
-            }
-            if (!p.b_mn) {
-              tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BK, n0);
-            } else {
-              for (int j = 0; j < (b_cols + 63) / 64; ++j)
-                tma_load_2d(sb + j * BK * 128, &tmap_b, &full_bar[stage], n0 + j * 64, kb * BK + b_shift);
-            }
+          mbar_expect_tx(&full_bar[stage], (uint32_t)(A_STAGE_BYTES + (p.b_mn ? ((p.tile_n + 63) / 64) * BK * 128
+                                                                               : p.tile_n * BK * 2)));
+          if (!p.a_mn) {
+            const int tap = kb / p.kb_per_tap;
+            const int kc0 = (kb - tap * p.kb_per_tap) * BK;
+            tma_load_3d(sa, &tmap_a, &full_bar[stage], kc0, m0 + p.tap_shift[tap], p.tap_plane[tap]);
           } else {
-            const uint32_t fb = mapa_shared(smem_u32(&full_bar[stage]), 0);  // (only instantiated for CG == 2)
-            if (!p.a_mn) {
-              const int tap = kb / p.kb_per_tap;
-              const int kc0 = (kb - tap * p.kb_per_tap) * BK;
-              tma_load_3d_cg2(sa, &tmap_a, fb, kc0, m0 + p.tap_shift[tap], p.tap_plane[tap]);
-            } else {
-              tma_load_3d_cg2(sa, &tmap_a, fb, m0, kb * BK + p.a_row_off, 0);
-              tma_load_3d_cg2(sa + BK * 128, &tmap_a, fb, m0 + 64, kb * BK + p.a_row_off, 0);
-            }
-            if (!p.b_mn) {
-              tma_load_2d_cg2(sb, &tmap_b, fb, kb * BK, n0);
-            } else {
-              for (int j = 0; j < (b_cols + 63) / 64; ++j)
-                tma_load_2d_cg2(sb + j * BK * 128, &tmap_b, fb, n0 + j * 64, kb * BK + b_shift);
-            }
+            // A stored [K rows][M cols]: two 64-wide MN atoms of BK rows each
+            tma_load_3d(sa, &tmap_a, &full_bar[stage], m0, kb * BK + p.a_row_off, 0);
+            tma_load_3d(sa + BK * 128, &tmap_a, &full_bar[stage], m0 + 64, kb * BK + p.a_row_off, 0);
+          }
+          if (!p.b_mn) {
+            tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BK, n0);
+          } else {
+            for (int j = 0; j < (p.tile_n + 63) / 64; ++j)
+              tma_load_2d(sb + j * BK * 128, &tmap_b, &full_bar[stage], n0 + j * 64, kb * BK + b_shift);
           }
           if (++stage == p.stages) {
             stage = 0;
             phase ^= 1;
           }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer
-    if (lane == 0 && leader) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      // descriptor templates: K-major SW128: SBO = 1024 (8 rows x 128 B), LBO unused;
-      // MN-major SW128: LBO = BK*128 (next 64-wide MN atom), SBO = 1024 (next 8 K rows).
-      const uint32_t a_lbo = p.a_mn ? BK * 128 : 16;
-      const uint32_t b_lbo = p.b_mn ? BK * 128 : 16;
-      const uint32_t a_kstep = p.a_mn ? UMMA_K * 128 : UMMA_K * 2;
-      const uint32_t b_kstep = p.b_mn ? UMMA_K * 128 : UMMA_K * 2;
-      for (int w = unit0; w < work_total; w += nunits) {
-        int tm_, tn_, split;
-        decode_work(p, w, tm_, tn_, split);
-        const int kb0 = (int)((long long)p.num_kb * split / p.split_k);
-        const int kb1 = (int)((long long)p.num_kb * (split + 1) / p.split_k);
-        mbar_wait(&acc_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * p.acc_stride;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * stage_bytes);
-          const uint32_t sb = sa + A_STAGE_BYTES;
-          // a tap's last K-block is zero beyond kc (TMA out-of-bounds fill / zero-padded weights): its all-zero
-          // 16-wide steps are not issued (K = 196 per conv tap: 13 instead of 16 MMAs; K = 784: 49 instead of 52)
-          const int nk = (kb + 1) % p.kb_per_tap == 0 ? p.k_tail16 : BK / UMMA_K;
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            if (k >= nk) break;
-            const uint64_t adesc = make_smem_desc(sa + k * a_kstep, a_lbo, 1024, SWZ_128B);
-            const uint64_t bdesc = make_smem_desc(sb + k * b_kstep, b_lbo, 1024, SWZ_128B);
-            if constexpr (CG == 2) umma_f16_ss_cg2(d_tmem, adesc, bdesc, p.idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            else umma_f16_ss(d_tmem, adesc, bdesc, p.idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          // frees the smem stage (in both CTAs of a pair) once these MMAs retire
-          if constexpr (CG == 2) umma_commit_cg2(&empty_bar[stage]);
-          else umma_commit(&empty_bar[stage]);
-          if (++stage == p.stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        // accumulator complete -> epilogue warps (of both CTAs)
-        if constexpr (CG == 2) umma_commit_cg2(&acc_full[acc]);
-        else umma_commit(&acc_full[acc]);
-        if (++acc == p.nacc) {
-          acc = 0;
-          acc_phase ^= 1;
         }
       }
     }
   } else {
-    // ===================================================================== epilogue warps
-    // 8 warps: warp w owns TMEM lane quadrant (w & 3) (32 rows of the tile) and every second
-    // 32-column chunk ((w - 2) >> 2 selects even / odd chunks). Per chunk a warp
-    //   1. issues its residual / aux global loads (addresses do not depend on the accumulator),
-    //   2. pulls the accumulators row-per-thread with tcgen05.ld and transposes them through a padded
-    //      shared-memory staging tile,
+    // ===================================================================== consumer warpgroups
+    // Per work unit: main loop (wgmma into registers) -> accumulator tile in shared memory -> epilogue. In the
+    // epilogue warp w owns rows 32*(w & 3) .. +32 of the tile and every second 32-column chunk ((w >> 2) selects
+    // even / odd chunks). Per chunk a warp
+    //   1. issues its residual / aux global loads,
+    //   2. reads the accumulators of its chunk from the shared-memory tile,
     //   3. works "coalesced": one instruction covers 4 rows x 128 contiguous bytes (8 lanes x float4
     //      per row), so residual loads and fp32 / fp16 stores are full-line accesses.
-    // The epilogue is bound by global-memory latency, hence the loads hoisted ahead of the TMEM read
-    // and the 256 threads: ~32 KB of residual reads are in flight per SM.
-    const int ew = warp - 2;
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may access
-    const int chunk_par = ew >> 2;
-    float* stg = reinterpret_cast<float*>(ctrl + SMEM_CTRL_BYTES) + ew * (32 * STG_LD);
+    const int quad = warp & 3;  // 32-row quarter of the tile this warp's epilogue covers
+    const int chunk_par = warp >> 2;
     // per-CTA partial BatchNorm statistics (sum | sum of squares), flushed with one atomic per column at the end
-    float* stat_s = reinterpret_cast<float*>(ctrl + SMEM_CTRL_BYTES + SMEM_STG_BYTES);
+    float* stat_s = reinterpret_cast<float*>(ctrl + SMEM_CTRL_BYTES + SMEM_ACC_BYTES);
     const int sub = lane >> 3;   // row within a 4-row group
     const int c4 = lane & 7;     // which float4 of the 32-column chunk
     constexpr bool GENERIC = (FEAT & EF_GENERIC) != 0;
@@ -417,22 +376,37 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     const bool osum = GENERIC ? (p.osum != nullptr) : ((FEAT & EF_OSUM) != 0);
     const float alpha = has_aptr ? p.alpha * __ldg(p.alpha_ptr) : p.alpha;
     if (stats) {
-      for (int i = threadIdx.x - 64; i < 2 * p.n; i += GEMM_THREADS - 64) stat_s[i] = 0.f;
+      for (int i = threadIdx.x; i < 2 * p.n; i += EPI_THREADS) stat_s[i] = 0.f;
       asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");  // the epilogue warps only
     }
     if (osum) {  // tile-local column sums: stat_s[0 .. tile_n)
-      if (threadIdx.x - 64 < 256) stat_s[threadIdx.x - 64] = 0.f;
+      stat_s[threadIdx.x] = 0.f;
       asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
     }
     const float osum_alpha = (osum && p.osum_alpha) ? __ldg(p.osum_alpha) : 1.f;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    uint32_t acc_empty_leader = 0u;
-    if constexpr (CG == 2) acc_empty_leader = mapa_shared(smem_u32(&acc_empty[0]), 0);
+    int stage = 0;
+    uint32_t phase = 0;
     for (int w = unit0; w < work_total; w += nunits) {
       int tm, tn, split_;
       decode_work(p, w, tm, tn, split_);
-      const int row_base = (tm * cg + (int)cta_rank) * BM + quad * 32;
+      const int row_base = tm * BM + quad * 32;
+      {
+        const int kb0 = (int)((long long)p.num_kb * split_ / p.split_k);
+        const int kb1 = (int)((long long)p.num_kb * (split_ + 1) / p.split_k);
+        asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");  // the previous tile's epilogue is done with accbuf
+        if (GENERIC && p.bf16) {
+          if (!p.a_mn && !p.b_mn) gemm_mainloop_n<0, 0, 1>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
+          else if (!p.a_mn) gemm_mainloop_n<0, 1, 1>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
+          else if (!p.b_mn) gemm_mainloop_n<1, 0, 1>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
+          else gemm_mainloop_n<1, 1, 1>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
+        } else {
+          if (!p.a_mn && !p.b_mn) gemm_mainloop_n<0, 0, 0>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
+          else if (!p.a_mn) gemm_mainloop_n<0, 1, 0>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
+          else if (!p.b_mn) gemm_mainloop_n<1, 0, 0>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
+          else gemm_mainloop_n<1, 1, 0>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
+        }
+        asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");  // accumulator tile complete
+      }
       int n0 = tn * p.tile_n;
       int n_end = min(p.n, n0 + p.tile_n);
       if (p.b_ntaps > 1) {  // output columns [tap * n, (tap + 1) * n)
@@ -450,12 +424,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         for (int k = 0; k < 8; ++k) orow[k] = __shfl_sync(0xffffffffu, my_orow, 4 * k + sub);
       }
 
-      bool waited = false;
-      const uint32_t taddr = tmem_base + acc * p.acc_stride + ((uint32_t)(quad * 32) << 16);
+      const float* arow = accbuf + (quad * 32 + lane) * ACC_LD;  // this lane's accumulator row (row-per-thread reads)
 
       if constexpr ((FEAT & EF_DIRECT) != 0) {
         // Row-per-thread epilogue for launches that only write 16-bit outputs (qkv / fc1 / data gradients): lane l
-        // owns tile row quad*32 + l, computes on the 32 accumulator columns tcgen05.ld hands it and stores them as
+        // owns tile row quad*32 + l, computes on 32 accumulator columns of its row and stores them as
         // two 32-byte sectors per output -- no staging tile, no per-row address math, one bounds check per 16 columns.
         // (n, the leading dimensions and the base pointers are multiples of 16 elements: checked by the launcher.)
         const int my_row = row_base + lane;
@@ -473,21 +446,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             ld_global_256(arow16 + nbase, axw[0]);
             if (nvalid > 16) ld_global_256(arow16 + nbase + 16, axw[1]);
           }
-          if (!waited) {
-            mbar_wait(&acc_full[acc], acc_phase);
-            tc_fence_after();
-            waited = true;
-          }
           uint32_t raw[32];
-          if (nvalid > 16) {
-            tmem_ld32(taddr + c0, raw);
-          } else {
-            uint32_t lo[16];
-            tmem_ld16(taddr + c0, lo);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) raw[i] = lo[i], raw[16 + i] = 0u;
+          for (int i = 0; i < 8; ++i) {
+            const float4 v = *reinterpret_cast<const float4*>(arow + c0 + 4 * i);
+            raw[4 * i] = __float_as_uint(v.x), raw[4 * i + 1] = __float_as_uint(v.y);
+            raw[4 * i + 2] = __float_as_uint(v.z), raw[4 * i + 3] = __float_as_uint(v.w);
           }
-          tmem_ld_wait();
           float osv[32];  // rounded outputs for the column sums
 #pragma unroll
           for (int hf = 0; hf < 2; ++hf) {
@@ -632,40 +597,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           asc = ld_vec4_guard(p.aux_scale + col, n_end - col, 1.f);
           ash = ld_vec4_guard(p.aux_shift + col, n_end - col, 0.f);
         }
-        // ---- 2. accumulators: TMEM -> registers -> staging tile
-        if (!waited) {
-          mbar_wait(&acc_full[acc], acc_phase);
-          tc_fence_after();
-          waited = true;
-        }
-        {
-          uint32_t raw[32];
-          if (c0 + 32 <= p.tile_n) {
-            tmem_ld32(taddr + c0, raw);
-          } else {  // tile_n is a multiple of 16: last half chunk
-            uint32_t lo[16];
-            tmem_ld16(taddr + c0, lo);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              raw[i] = lo[i];
-              raw[16 + i] = 0u;
-            }
-          }
-          tmem_ld_wait();
-          float4* srow = reinterpret_cast<float4*>(stg + lane * STG_LD);
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            srow[j] = make_float4(__uint_as_float(raw[4 * j]), __uint_as_float(raw[4 * j + 1]),
-                                  __uint_as_float(raw[4 * j + 2]), __uint_as_float(raw[4 * j + 3]));
-        }
-        __syncwarp();
-        // ---- 3. coalesced epilogue math + stores
+        // ---- 2./3. accumulators straight from the shared-memory tile; coalesced epilogue math + stores
+        const float* stg = accbuf + (quad * 32) * ACC_LD + c0;
         float4 s1 = make_float4(0.f, 0.f, 0.f, 0.f), s2 = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
           const int rl = 4 * k + sub;  // row within the warp's 32
           const bool ok = cany && orow[k] >= 0;
-          float4 v = *reinterpret_cast<const float4*>(stg + rl * STG_LD + 4 * c4);
+          float4 v = *reinterpret_cast<const float4*>(stg + rl * ACC_LD + 4 * c4);
           if (atomic_out) {
             v.x *= alpha, v.y *= alpha, v.z *= alpha, v.w *= alpha;
             if (ok) {
@@ -767,7 +706,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             }
           }
         }
-        __syncwarp();
         if (osum) {
 #pragma unroll
           for (int o = 8; o <= 16; o <<= 1) {
@@ -799,35 +737,20 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
         }
       }
-      if (!waited) {  // this warp had no chunk in the tile: still consume the phase
-        mbar_wait(&acc_full[acc], acc_phase);
-        tc_fence_after();
-      }
       if (osum) {  // flush this tile's column sums: one global atomic per column per tile
         asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-        const int lc = threadIdx.x - 64;
+        const int lc = threadIdx.x;
         if (lc < p.tile_n && n0 + lc < n_end) {
           const float a = stat_s[lc];
           if (a != 0.f) atomicAdd(p.osum + n0 + lc, a * osum_alpha);
         }
-        if (lc < 256) stat_s[lc] = 0.f;
+        stat_s[lc] = 0.f;
         asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-      }
-      // hand the accumulator stage back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (CG == 2) mbar_arrive_cluster(acc_empty_leader + 8u * acc);
-        else mbar_arrive(&acc_empty[acc]);
-      }
-      if (++acc == p.nacc) {
-        acc = 0;
-        acc_phase ^= 1;
       }
     }
     if (stats) {
       asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-      for (int i = threadIdx.x - 64; i < p.n; i += GEMM_THREADS - 64) {
+      for (int i = threadIdx.x; i < p.n; i += EPI_THREADS) {
         const float a = stat_s[i], b = stat_s[p.n + i];
         if (a != 0.f || b != 0.f) {
           atomicAdd(p.col_sum + i, a);
@@ -836,111 +759,22 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       }
     }
   }
-
-  tc_fence_before();
-  __syncwarp();                     // role loops leave lane 0 behind: reconverge before the aligned barrier
-  if constexpr (CG == 2) cluster_sync_all();  // the leader's MMAs read the peer's shared memory / TMEM until the very end
-  else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (CG == 2) tmem_dealloc_cg2(tmem_base, TMEM_COLS);
-    else tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
 // ------------------------------------------------------------------------------------------ host
-// Cost model for (cta_group, tile_n): waves of work units over the CTAs / CTA pairs, each unit costing its MMA time
-// (~ tile_n per K block; a pair retires a 256-row tile in the time one CTA needs for 128 rows, and its operand
-// traffic per flop is 2/3 of the single-CTA tile's) plus a fixed part for the A stream / epilogue setup.
-struct TileChoice {
-  int cg, tile_n;
-};
-static double cg2_gain() {  // relative main-loop time of the pair per 128 rows (FVIT_GEMM_CG2_GAIN to tune)
-  static double g = -1.0;
-  if (g < 0) {
-    const char* e = getenv("FVIT_GEMM_CG2_GAIN");
-    g = e ? atof(e) : 0.8;
-  }
-  return g;
-}
-static int forced_cg() {  // FVIT_GEMM_CG=1|2 forces the mode where legal (A/B experiments)
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("FVIT_GEMM_CG");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
-static int cost_model() {  // FVIT_GEMM_COST=0: the round-1 wave model (A/B); default: the clock model below
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("FVIT_GEMM_COST");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
-// (measured r02k, fv4 / fv0 fwd+bwd and fv0 / ar0 forward: the wave model below stays the default -- the clock model
-// wins only on the N <= 64 stem / level-0 GEMMs, by not pairing CTAs there, which the wave model now does too, and
-// loses 0.3 ms each on the qkv projection (picks 192 instead of 256) and the fc2 weight gradient (pairs M = 784))
-// Clock model of one work unit (SM clocks): per 64-deep K block the tensor pipe needs ~2*tile_n clocks for 128 rows
-// (4096 MAC/clk/SM), the operand stream needs bytes_per_CTA * concurrently_streaming_CTAs / 6300 B/clk (chip-wide
-// L2 -> SM delivery, B300_MICROARCH.md "LTS throughput cap"; the measured ceiling of this kernel's main loop), and the
-// epilogue ~1500 + 12 * tile_n clocks per tile, overlapped with the next unit's main loop except for the last unit.
-// Narrow tiles on all 148 SMs are L2-bound (a 128 x 96 tile streams 140 B/clk per SM): fewer, wider tiles win for the
-// small-M GEMMs of the carrier branch.
-static double unit_clocks(int cg, int bn, int num_kb, long long active_ctas) {
-  const double mma = (cg == 2 ? 3.6 : 2.0) * bn;  // (pair main loop measured: 1250 TF/s on 8192^3 = 3.7 * tile_n clocks per K block)
-  const double bytes = (128.0 + (double)bn / cg) * 128.0;
-  const double l2 = bytes * (double)active_ctas / 6300.0;
-  return num_kb * (mma > l2 ? mma : l2);
-}
-static TileChoice pick_tile_clk(int m, int n, int split_k, int num_kb, int sms, int want_cg, int want_tile_n) {
-  TileChoice best{1, 16};
+// Wave model of the tile width: waves of work units over the SMs, each unit costing its MMA time (~ tile_n per K
+// block) plus a fixed part for the A stream / epilogue setup. MMA widths are 32 / 64 / 96 / 128.
+static int pick_tile_n(int m, int n, int split_k, int sms) {
+  int best = 32;
   double best_cost = 1e30;
-  for (int cg = 1; cg <= 2; ++cg) {
-    if (want_cg && cg != want_cg) continue;
-    if (cg == 2 && m <= BM) continue;
-    const int tiles_m = ceil_div(m, BM * cg);
-    const int step = 16 * cg;
-    for (int bn = step; bn <= 256; bn += step) {
-      if (want_tile_n > 0 && bn != want_tile_n) continue;
-      const int tiles_n = ceil_div(n, bn);
-      const long long work = (long long)tiles_m * tiles_n * split_k;
-      const int slots = sms / cg;
-      const long long waves = (work + slots - 1) / slots;
-      const long long active = (work < slots ? work : slots) * cg;
-      const int kb = num_kb / (split_k > 0 ? split_k : 1) > 0 ? num_kb / (split_k > 0 ? split_k : 1) : 1;
-      const double main = unit_clocks(cg, bn, kb, active);
-      const double epi = 1500.0 + 12.0 * bn;
-      const double cost = (double)waves * (main > epi ? main : epi) + epi + 2500.0;
-      if (cost < best_cost - 1e-9) {
-        best_cost = cost;
-        best = TileChoice{cg, bn};
-      }
-    }
-  }
-  return best;
-}
-static TileChoice pick_tile(int m, int n, int split_k, int sms, int want_cg, int want_tile_n) {
-  TileChoice best{1, 16};
-  double best_cost = 1e30;
-  for (int cg = 1; cg <= 2; ++cg) {
-    if (want_cg && cg != want_cg) continue;
-    if (cg == 2 && m <= BM) continue;  // the second CTA of the pair would only see padding rows
-    if (cg == 2 && n <= 64 && !want_cg) continue;  // nothing to share: B is a few KB, the pair only adds its barriers
-    const int tiles_m = ceil_div(m, BM * cg);
-    const int step = 16 * cg;  // each CTA of a pair stages tile_n / 2 columns of B: keep that a multiple of 16
-    for (int bn = step; bn <= 256; bn += step) {
-      if (want_tile_n > 0 && bn != want_tile_n) continue;
-      const int tiles_n = ceil_div(n, bn);
-      const long long work = (long long)tiles_m * tiles_n * split_k;
-      const int slots = sms / cg;
-      const long long waves = (work + slots - 1) / slots;
-      const double cost = (double)waves * (bn * (cg == 2 ? cg2_gain() : 1.0) + 48.0);
-      if (cost < best_cost - 1e-9) {
-        best_cost = cost;
-        best = TileChoice{cg, bn};
-      }
+  const int tiles_m = ceil_div(m, BM);
+  for (int bn = 32; bn <= MAX_TILE_N; bn += 32) {
+    const long long work = (long long)tiles_m * ceil_div(n, bn) * split_k;
+    const long long waves = (work + sms - 1) / sms;
+    const double cost = (double)waves * (bn + 48.0);
+    if (cost < best_cost - 1e-9) {
+      best_cost = cost;
+      best = bn;
     }
   }
   return best;
@@ -984,17 +818,13 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   FVIT_CHECK(!a->out_colsum || (a->out_f16 && !a->col_sum && split_k == 1 && b_ntaps == 1),
              "fvit_gemm: out_colsum needs out_f16, no BN statistics, no split-K");
 
+  FVIT_CHECK(a->tile_n == 0 || (a->tile_n >= 16 && a->tile_n <= 256 && a->tile_n % 16 == 0),
+             "fvit_gemm: tile_n=%d invalid", a->tile_n);
+  FVIT_CHECK(a->cta_group >= 0 && a->cta_group <= 2, "fvit_gemm: cta_group=%d invalid", a->cta_group);
   const int sms = num_sms();
-  int want_cg = a->cta_group == 1 || a->cta_group == 2 ? a->cta_group : forced_cg();
-  if (want_cg == 2 && (a->m <= BM || (a->tile_n > 0 && a->tile_n % 32 != 0))) want_cg = 1;
-  const int num_kb_all = ceil_div(a->kc, BK) * a->ntaps;
-  const TileChoice tc = cost_model()
-                            ? pick_tile_clk(a->m, a->n, split_k * b_ntaps, num_kb_all * b_ntaps, sms, want_cg,
-                                            a->tile_n > 0 ? a->tile_n : 0)
-                            : pick_tile(a->m, a->n, split_k * b_ntaps, sms, want_cg, a->tile_n > 0 ? a->tile_n : 0);
-  const int tile_n = tc.tile_n, cg = tc.cg;
-  FVIT_CHECK(tile_n >= 16 && tile_n <= 256 && tile_n % (16 * cg) == 0, "fvit_gemm: tile_n=%d invalid (cta_group %d)",
-             tile_n, cg);
+  // a requested width above the widest MMA is split into two equal tiles (multiples of 16)
+  int tile_n = a->tile_n > 0 ? a->tile_n : pick_tile_n(a->m, a->n, split_k * b_ntaps, sms);
+  if (tile_n > MAX_TILE_N) tile_n = ceil_div(tile_n, 32) * 16;
 
   GemmParams p;
   memset(&p, 0, sizeof(p));
@@ -1009,15 +839,15 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
       kskip = e ? atoi(e) : 1;
     }
     const int tail = a->kc - (p.kb_per_tap - 1) * BK;  // 1..64 real columns in the last block
-    p.k_tail16 = kskip ? ceil_div(tail, UMMA_K) : BK / UMMA_K;
+    p.k_tail16 = kskip ? ceil_div(tail, MMA_K) : BK / MMA_K;
   }
   p.a_mn = a->a_mn_major ? 1 : 0;
   p.b_mn = a->b_mn_major ? 1 : 0;
   p.a_row_off = a->a_row_off;
   p.b_row_off = a->b_row_off;
   p.tile_n = tile_n;
-  p.cg = cg;
-  p.tiles_m = ceil_div(a->m, BM * cg);
+  p.mma_n = ceil_div(tile_n, 32) * 32;
+  p.tiles_m = ceil_div(a->m, BM);
   p.tiles_n = ceil_div(a->n, tile_n);
   p.b_ntaps = a->b_ntaps > 1 ? a->b_ntaps : 1;
   p.tiles_per_tap = p.tiles_n;
@@ -1025,16 +855,12 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   p.split_k = split_k < p.num_kb ? split_k : p.num_kb;
   if (p.split_k < 1) p.split_k = 1;
   p.atomic_out = split_k > 1 ? 1 : 0;
-  const int b_cols = tile_n / cg;  // B columns staged per CTA
-  const int stage_bytes = A_STAGE_BYTES + (a->b_mn_major ? ((b_cols + 63) & ~63) : b_cols) * BK * 2;
+  const int stage_bytes = A_STAGE_BYTES + (a->b_mn_major ? ((p.mma_n + 63) & ~63) : p.mma_n) * BK * 2;
   const int stats_bytes = a->col_sum ? SMEM_STATS_BYTES : (a->out_colsum ? 256 * 4 : 0);
-  int stages = (SMEM_BUDGET - SMEM_CTRL_BYTES - SMEM_ALIGN_SLACK - SMEM_STG_BYTES - stats_bytes) / stage_bytes;
+  int stages = (SMEM_BUDGET - SMEM_CTRL_BYTES - SMEM_ALIGN_SLACK - SMEM_ACC_BYTES - stats_bytes) / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   FVIT_CHECK(stages >= 2, "fvit_gemm: not enough shared memory for 2 stages");
   p.stages = stages;
-  p.acc_stride = tile_n <= 64 ? 64 : (tile_n <= 128 ? 128 : 256);
-  p.nacc = TMEM_COLS / p.acc_stride;
-  p.idesc = make_idesc_f16(BM * cg, tile_n, p.a_mn, p.b_mn, a->bf16 ? 1u : 0u);
   for (int i = 0; i < 16; ++i) {
     p.tap_shift[i] = i < (b_ntaps > 1 ? b_ntaps : a->ntaps) ? a->tap_shift[i] : 0;
     p.tap_plane[i] = i < a->ntaps ? a->tap_plane[i] : 0;
@@ -1093,17 +919,16 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   if (!p.b_mn) {
     const uint64_t kdim = a->ntaps == 1 ? (uint64_t)a->kc : (uint64_t)p.num_kb * BK;
     rc = get_tmap(&tmb, a->b, kdim, (uint64_t)a->n, 1, (uint64_t)a->ldb * 2, 0, BK,
-                  (uint32_t)b_cols, 2);
+                  (uint32_t)tile_n, 2);
   } else {
     rc = get_tmap(&tmb, a->b, (uint64_t)a->n, (uint64_t)a->b_rows, 1, (uint64_t)a->ldb * 2, 0, 64,
                   BK, 2);
   }
   if (rc) return rc;
 
-  const int smem_bytes = stages * stage_bytes + SMEM_CTRL_BYTES + SMEM_ALIGN_SLACK + SMEM_STG_BYTES + stats_bytes;
+  const int smem_bytes = stages * stage_bytes + SMEM_CTRL_BYTES + SMEM_ALIGN_SLACK + SMEM_ACC_BYTES + stats_bytes;
   const long long work = (long long)p.tiles_m * p.tiles_n * p.split_k;
-  const int slots = sms / cg;
-  const int grid = (int)(work < slots ? work : slots) * cg;
+  const int grid = (int)(work < sms ? work : sms);
   // feature mask of this call; launch the matching specialisation if one was instantiated
   uint32_t feat = ((uint32_t)a->act << EF_ACT_SHIFT);
   if (a->resid && !p.atomic_out) feat |= EF_RESID;
@@ -1117,6 +942,7 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   if (a->row_scale) feat |= EF_RS;
   if (a->out_colsum) feat |= EF_OSUM;
   if (p.pre_is_grad) feat |= EF_PREGRAD;
+  const bool needs_generic = a->bf16 != 0;  // bf16 operands: only the generic kernel instantiates their MMAs
   {
     // row-per-thread epilogue (EF_DIRECT): 16-bit outputs only, everything a lane touches in 32-byte pieces
     static int direct = -1;  // FVIT_GEMM_DIRECT=0: staging-tile epilogue everywhere (A/B)
@@ -1151,40 +977,16 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
       }
     }
   }
-  const bool needs_generic = false;
-#define FVIT_GEMM_LAUNCH(F)                                                                            \
-  do {                                                                                                 \
-    if (cg == 1) {                                                                                     \
-      auto kfn = gemm_tcgen05_kernel<(F), 1>;                                                          \
-      static bool attr_set = false;                                                                    \
-      if (!attr_set) {                                                                                 \
-        FVIT_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET)); \
-        attr_set = true;                                                                               \
-      }                                                                                                \
-      kfn<<<grid, GEMM_THREADS, smem_bytes, (cudaStream_t)stream>>>(tma, tmb, p);                      \
-      return post_launch("gemm_tcgen05_kernel");                                                       \
-    }                                                                                                  \
-    auto kfn2 = gemm_tcgen05_kernel<(F), 2>;                                                           \
-    static bool attr_set2 = false;                                                                     \
-    if (!attr_set2) {                                                                                  \
-      FVIT_CUDA(cudaFuncSetAttribute(kfn2, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET)); \
-      attr_set2 = true;                                                                                \
-    }                                                                                                  \
-    cudaLaunchConfig_t cfg;                                                                            \
-    memset(&cfg, 0, sizeof(cfg));                                                                      \
-    cfg.gridDim = dim3((unsigned)grid), cfg.blockDim = dim3(GEMM_THREADS);                             \
-    cfg.dynamicSmemBytes = (size_t)smem_bytes, cfg.stream = (cudaStream_t)stream;                      \
-    cudaLaunchAttribute attr[1];                                                                       \
-    attr[0].id = cudaLaunchAttributeClusterDimension;                                                  \
-    attr[0].val.clusterDim.x = 2, attr[0].val.clusterDim.y = 1, attr[0].val.clusterDim.z = 1;          \
-    cfg.attrs = attr, cfg.numAttrs = 1;                                                                \
-    cudaError_t le_ = cudaLaunchKernelEx(&cfg, kfn2, tma, tmb, p);                                     \
-    if (le_ != cudaSuccess) {                                                                          \
-      (void)cudaGetLastError(); /* do not leave the error behind for the next launch */                \
-      return set_error("launch of the CTA-pair gemm_tcgen05_kernel (grid %d, %d B smem) failed: %s", grid, smem_bytes, \
-                       cudaGetErrorString(le_));                                                       \
-    }                                                                                                  \
-    return post_launch("gemm_tcgen05_kernel");                                                         \
+#define FVIT_GEMM_LAUNCH(F)                                                                          \
+  do {                                                                                               \
+    auto kfn = gemm_wgmma_kernel<(F)>;                                                               \
+    static bool attr_set = false;                                                                    \
+    if (!attr_set) {                                                                                 \
+      FVIT_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BUDGET)); \
+      attr_set = true;                                                                               \
+    }                                                                                                \
+    kfn<<<grid, GEMM_THREADS, smem_bytes, (cudaStream_t)stream>>>(tma, tmb, p);                      \
+    return post_launch("gemm_wgmma_kernel");                                                         \
   } while (0)
 #define FVIT_ACTF(x) ((uint32_t)(x) << EF_ACT_SHIFT)
   if (!needs_generic) {

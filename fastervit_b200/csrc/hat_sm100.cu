@@ -1,20 +1,20 @@
-// fvit_hat_attn_fwd: the fused hierarchical-attention kernel of WindowAttention.forward (fv.py:557-565) for sm_100a —
-// QKV projection, softmax(Q K^T * scale + relative-position bias) and the V contraction in ONE tcgen05 kernel; the
+// fvit_hat_attn_fwd: the fused hierarchical-attention kernel of WindowAttention.forward (fv.py:557-565) for sm_90a —
+// QKV projection, softmax(Q K^T * scale + relative-position bias) and the V contraction in ONE wgmma kernel; the
 // [tokens, 3C] qkv matrix and the score / probability matrices never exist in HBM (inference), or qkv is written once
 // and never read back (training, where the backward pass needs it).
 //
 // Work item = (tile of 128 token rows = gpt whole windows in slots of 16/32/64/128 rows, head); head-major order so the
 // head's weight slice [3*hdp, C] and bias [S, S] stay hot in L2 / shared memory.
 //
-//   warp 0     : TMA producer — per 64-wide K block the (window_size^2 + ct_size^2) x 64 activation boxes of the tile's
+//   warp 4     : TMA producer — per 64-wide K block the (window_size^2 + ct_size^2) x 64 activation boxes of the tile's
 //                windows and the head's W_q / W_k / W_v boxes into a ring of 128B-swizzled stages
-//   warp 1     : projection MMA issuer — [Q | K | V](128 x 3*hdp, fp32 in TMEM, double buffered) = X W_h^T over C
-//   warp 2     : attention MMA issuer — S = Q K^T (128 x 128) and O = P V from the fp16 operand tiles the epilogue
-//                warps wrote to shared memory
-//   warps 3..6 : epilogue — one thread per token row: (1) Q, K, V accumulators + qkv bias -> fp16 -> swizzled UMMA
-//                operand tiles (and optionally the qkv matrix for the backward pass); (2) softmax over the window's keys
-//                (block-diagonal mask, bias from shared memory, exp2), P as fp16 operand; (3) O / rowsum -> fp16 out.
-// The projection of item i+1 runs on the tensor core while the epilogue warps are busy with item i.
+//   warps 0..3 : one warpgroup — (1) [Q | K | V] = X W_h^T over C (wgmma, register accumulators) + qkv bias -> fp16
+//                straight from the accumulator fragments into the swizzled Q / K / V operand tiles (and optionally the
+//                qkv matrix for the backward pass); (2) S = Q K^T into an fp32 score tile, softmax with one thread per
+//                token row (block-diagonal mask, bias from shared memory, exp2), P as fp16 operand; (3) O = P V into the
+//                score tile, O / rowsum -> fp16 out.
+// The score tile shares its shared memory with the operand ring: the producer starts an item's loads once the previous
+// item's O has been read out (ring_free).
 #include <cuda_fp16.h>
 
 #include "../../include/fvit.h"
@@ -23,16 +23,20 @@
 
 namespace fvit {
 
-constexpr int HT_THREADS = 224;
+constexpr int HT_THREADS = 160;
 constexpr int HT_ROWS = 128;
 constexpr int HT_BK = 64;
 constexpr int HT_MAX_STAGES = 4;
+constexpr int HT_PRODUCER = 4;   // the TMA warp; warps 0..3 are the compute warpgroup
+constexpr int HT_ACC_LD = 132;   // floats per row of the fp32 score tile
+constexpr int HT_ACC_BYTES = HT_ROWS * HT_ACC_LD * 4;
 
 struct HatParams {
   int groups, S, heads, gpt, tiles, slot;
   int num_kb;   // ceil(C / 64)
   int k_tail16; // 16-wide MMA steps with real columns in the last K-block (the rest is TMA zero fill: not issued)
   int stages;
+  int ring_bytes;  // operand ring / score tile region
   int Cp;       // heads * hdp
   float scale_log2e;
   const float* qkv_bias;  // [3 * Cp] head-padded, or null
@@ -43,10 +47,6 @@ struct HatParams {
   long long ldq;
   int rows_total;
 };
-
-__device__ __forceinline__ void ht_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
 
 template <int HDP>
 __global__ void __launch_bounds__(HT_THREADS, 1)
@@ -59,51 +59,39 @@ __global__ void __launch_bounds__(HT_THREADS, 1)
   constexpr int B_BYTES = 3 * HDP * HT_BK * 2;        // 24 KB / 12 KB
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   constexpr int OPER_BYTES = HT_ROWS * HDP * 2;       // one of Q / K / V as fp16 operand tile
-  constexpr int NQKV = 3 * HDP;                       // accumulator columns per stage
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = p.S;
-  uint8_t* s_oper = smem + p.stages * STAGE_BYTES;         // Q, K, V operand tiles
-  uint8_t* s_p = s_oper + 3 * OPER_BYTES;                  // P: 128 x 128 fp16 (two 64-wide K atoms)
+  float* sacc = reinterpret_cast<float*>(smem);             // score / O tile, aliases the operand ring
+  uint8_t* s_oper = smem + p.ring_bytes;                    // Q, K, V operand tiles
+  uint8_t* s_p = s_oper + 3 * OPER_BYTES;                   // P: 128 x 128 fp16 (two 64-wide K atoms)
   float* bias_s = reinterpret_cast<float*>(s_p + HT_ROWS * 128 * 2);
   uint8_t* ctrl = reinterpret_cast<uint8_t*>(bias_s) + ((S * S * 4 + 15) & ~15);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ctrl);   // [HT_MAX_STAGES]
   uint64_t* empty_bar = full_bar + HT_MAX_STAGES;           // [HT_MAX_STAGES]
-  uint64_t* acc_full = empty_bar + HT_MAX_STAGES;           // [2]
-  uint64_t* acc_empty = acc_full + 2;                       // [2]
-  uint64_t* qkv_ready = acc_empty + 2;
-  uint64_t* s_full = qkv_ready + 1;
-  uint64_t* p_full = s_full + 1;
-  uint64_t* o_full = p_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 1);
+  uint64_t* ring_free = empty_bar + HT_MAX_STAGES;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == HT_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmap_x);
     tma_prefetch_desc(&tmap_w);
-    for (int i = 0; i < p.stages; ++i) mbar_init(&full_bar[i], 1), mbar_init(&empty_bar[i], 1);
-    for (int i = 0; i < 2; ++i) mbar_init(&acc_full[i], 1), mbar_init(&acc_empty[i], 4);
-    mbar_init(qkv_ready, 4), mbar_init(s_full, 1), mbar_init(p_full, 4), mbar_init(o_full, 1);
+    for (int i = 0; i < p.stages; ++i) mbar_init(&full_bar[i], 1), mbar_init(&empty_bar[i], 4);
+    mbar_init(ring_free, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_acc[2] = {tmem_base, tmem_base + NQKV};
-  const uint32_t tmem_S = tmem_base + 384;  // scores; O overwrites its first HDP columns
 
   const int items = p.tiles * p.heads;
   const int nslots = HT_ROWS / p.slot;
 
-  if (warp == 0) {
+  if (warp == HT_PRODUCER) {
     // ===================================================================== TMA producer
     if (lane == 0) {
       int stage = 0;
-      uint32_t phase = 0;
-      for (int w = blockIdx.x; w < items; w += gridDim.x) {
+      uint32_t phase = 0, it = 0;
+      for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
         const int head = w / p.tiles, tile = w % p.tiles;
+        mbar_wait(ring_free, (it & 1) ^ 1);  // the previous item's score tile has been read out
         for (int kb = 0; kb < p.num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * STAGE_BYTES;
@@ -118,62 +106,11 @@ __global__ void __launch_bounds__(HT_THREADS, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================================================== projection MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_f16(128, NQKV, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0, it = 0;
-      for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
-        const int a = it & 1;
-        mbar_wait(&acc_empty[a], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES), sb = sa + A_BYTES;
-          const int nk = kb + 1 == p.num_kb ? p.k_tail16 : HT_BK / 16;
-#pragma unroll
-          for (int k = 0; k < HT_BK / 16; ++k) {
-            if (k >= nk) break;
-            umma_f16_ss(tmem_acc[a], make_smem_desc(sa + k * 32, 16, 1024, SWZ_128B),
-                        make_smem_desc(sb + k * 32, 16, 1024, SWZ_128B), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == p.stages) stage = 0, phase ^= 1;
-        }
-        umma_commit(&acc_full[a]);
-      }
-    }
-  } else if (warp == 2) {
-    // ===================================================================== attention MMA issuer
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_f16(128, 128, 0, 0);
-      const uint32_t idesc_o = make_idesc_f16(128, HDP, 0, 1);  // B = V, MN-major
-      const uint32_t sQ = smem_u32(s_oper), sK = sQ + OPER_BYTES, sV = sK + OPER_BYTES, sP = smem_u32(s_p);
-      uint32_t it = 0;
-      for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
-        mbar_wait(qkv_ready, it & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < HDP / 16; ++k)
-          umma_f16_ss(tmem_S, make_smem_desc(sQ + k * 32, 16, SBO_QKV, SWZ), make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ),
-                      idesc_s, k > 0 ? 1u : 0u);
-        umma_commit(s_full);
-        mbar_wait(p_full, it & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks)  // 128 keys in steps of 16
-          umma_f16_ss(tmem_S, make_smem_desc(sP + (ks >> 2) * (HT_ROWS * 128) + (ks & 3) * 32, 16, 1024, SWZ_128B),
-                      make_smem_desc(sV + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ), idesc_o, ks > 0 ? 1u : 0u);
-        umma_commit(o_full);
-      }
-    }
   } else {
-    // ===================================================================== epilogue warps
+    // ===================================================================== compute warpgroup
     const int quad = warp & 3;
     const int r = quad * 32 + lane;    // row in tile
-    const int tid = threadIdx.x - 96;  // 0..127 among the epilogue threads
+    const int tid = threadIdx.x;       // 0..127
     const int slot = p.slot;
     const int sl = r / slot;
     const int j = r - sl * slot;       // token index inside the window
@@ -181,19 +118,21 @@ __global__ void __launch_bounds__(HT_THREADS, 1)
     const int wlo = slot >= 32 ? lo : quad * 32;
     const int wn = slot >= 32 ? S : 32;
     const int nch = (wn + 31) / 32;
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
+    const float* arow = sacc + r * HT_ACC_LD;
+    const uint32_t sQ = smem_u32(s_oper), sK = sQ + OPER_BYTES, sV = sK + OPER_BYTES, sPu = smem_u32(s_p);
     // columns of P outside the warp's windows are never written: zero them once
     for (int c = 0; c < 128; c += 8) {
       if (c + 8 <= wlo || c >= wlo + 32 * nch)
         *reinterpret_cast<uint4*>(s_p + (c >> 6) * (HT_ROWS * 128) + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4)) =
             make_uint4(0, 0, 0, 0);
     }
-    // byte offset of 16-byte chunk c8 of this thread's row inside a Q / K / V operand tile
-    auto oper_off = [&](int c8) -> uint32_t {
-      if (HDP == 64) return (uint32_t)(r * 128 + ((c8 ^ (r & 7)) << 4));
-      return (uint32_t)(r * 64 + ((c8 ^ ((r >> 1) & 3)) << 4));
+    // byte offset of element (row, col) inside a Q / K / V operand tile (128B / 64B swizzle)
+    auto oper_off = [&](int row, int col) -> uint32_t {
+      if (HDP == 64) return (uint32_t)(row * 128 + ((((col >> 3) ^ (row & 7))) << 4) + (col & 7) * 2);
+      return (uint32_t)(row * 64 + ((((col >> 3) ^ ((row >> 1) & 3))) << 4) + (col & 7) * 2);
     };
-    uint32_t it = 0;
+    int stage = 0;
+    uint32_t phase = 0, it = 0;
     int staged_head = -1;
     for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
       const int head = w / p.tiles, tile = w % p.tiles;
@@ -201,7 +140,7 @@ __global__ void __launch_bounds__(HT_THREADS, 1)
       const bool row_ok = j < S && sl < p.gpt && grp < p.groups;
       const long long grow = (long long)grp * S + j;
       if (p.bias && head != staged_head) {
-        ht_bar_sync(1, 128);
+        named_bar_sync(1, 128);
         const float* bsrc = p.bias + (long long)head * S * S;
         const int n = S * S;
         for (int i0 = tid; i0 < n; i0 += 128 * 8) {
@@ -217,58 +156,83 @@ __global__ void __launch_bounds__(HT_THREADS, 1)
             if (i < n) bias_s[i] = tmp[u] * 1.4426950408889634f;
           }
         }
-        ht_bar_sync(1, 128);
+        named_bar_sync(1, 128);
         staged_head = head;
       }
-      // ---- (1) projection accumulators -> fp16 operand tiles (+ qkv bias, + optional global copy)
-      const int a = it & 1;
-      mbar_wait(&acc_full[a], (it >> 1) & 1);
-      tc_fence_after();
+      // ---- (1) projection: [Q | K | V] rows 64h .. 64h + 63 in registers, K blocks from the ring
+      {
+        float d[2][3][HDP / 2];
 #pragma unroll
-      for (int which = 0; which < 3; ++which) {
-        uint8_t* dst = s_oper + which * OPER_BYTES;
-        const float* qb = p.qkv_bias ? p.qkv_bias + which * p.Cp + head * HDP : nullptr;
-        __half* grow_ptr = (p.qkv_out && row_ok) ? p.qkv_out + grow * p.ldq + which * p.Cp + head * HDP : nullptr;
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int c0 = 0; c0 < HDP; c0 += 32) {
-          uint32_t raw[32];
-          tmem_ld32(tmem_acc[a] + lane_off + which * HDP + c0, raw);
-          tmem_ld_wait();
+          for (int which = 0; which < 3; ++which)
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint32_t o4[4];
+            for (int u = 0; u < HDP / 2; ++u) d[h][which][u] = 0.f;
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES), sb = sa + A_BYTES;
+          const int nk = kb + 1 == p.num_kb ? p.k_tail16 : HT_BK / 16;
+          auto step = [&](int k) {
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const int c = q * 8 + 2 * u;
-              const float b0 = qb ? __ldg(qb + c0 + c) : 0.f, b1 = qb ? __ldg(qb + c0 + c + 1) : 0.f;
-              const __half2 hh = __floats2half2_rn(__uint_as_float(raw[c]) + b0, __uint_as_float(raw[c + 1]) + b1);
-              o4[u] = *reinterpret_cast<const uint32_t*>(&hh);
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int which = 0; which < 3; ++which)
+                Wgmma<HDP, 0, 0, 0>::mma(d[h][which], make_smem_desc(sa + h * 8192 + k * 32, 16, 1024, SWZ_128B),
+                                         make_smem_desc(sb + which * (HDP * 128) + k * 32, 16, 1024, SWZ_128B), 1u);
+          };
+          // (each case is a complete wgmma group: a branch between the MMAs of one group would serialize them)
+          switch (nk) {
+            case 1: wgmma_fence(); step(0); wgmma_commit(); break;
+            case 2: wgmma_fence(); step(0); step(1); wgmma_commit(); break;
+            case 3: wgmma_fence(); step(0); step(1); step(2); wgmma_commit(); break;
+            default: wgmma_fence(); step(0); step(1); step(2); step(3); wgmma_commit(); break;
+          }
+          wgmma_wait0();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[stage]);
+          if (++stage == p.stages) stage = 0, phase ^= 1;
+        }
+        // accumulator fragments (+ qkv bias) -> fp16 operand tiles (+ optional global copy of the qkv rows)
+        const int t = tid & 127;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int half8 = 0; half8 < 2; ++half8) {
+            const int row = h * 64 + (t >> 5) * 16 + ((t & 31) >> 2) + half8 * 8;
+            const int rsl = row / slot, rj = row - rsl * slot, rgrp = tile * p.gpt + rsl;
+            const bool rok = rj < S && rsl < p.gpt && rgrp < p.groups;
+            __half* gq = (p.qkv_out && rok) ? p.qkv_out + ((long long)rgrp * S + rj) * p.ldq + head * HDP : nullptr;
+#pragma unroll
+            for (int which = 0; which < 3; ++which) {
+              const float* qb = p.qkv_bias ? p.qkv_bias + which * p.Cp + head * HDP : nullptr;
+              uint8_t* dst = s_oper + which * OPER_BYTES;
+#pragma unroll
+              for (int jj = 0; jj < HDP / 8; ++jj) {
+                const int col = jj * 8 + 2 * (t & 3);
+                const float b0 = qb ? __ldg(qb + col) : 0.f, b1 = qb ? __ldg(qb + col + 1) : 0.f;
+                const __half2 hh = __floats2half2_rn(d[h][which][4 * jj + 2 * half8] + b0, d[h][which][4 * jj + 2 * half8 + 1] + b1);
+                *reinterpret_cast<__half2*>(dst + oper_off(row, col)) = hh;
+                if (gq) *reinterpret_cast<__half2*>(gq + which * p.Cp + col) = hh;
+              }
             }
-            const uint4 v4 = make_uint4(o4[0], o4[1], o4[2], o4[3]);
-            *reinterpret_cast<uint4*>(dst + oper_off((c0 >> 3) + q)) = v4;
-            if (grow_ptr) *reinterpret_cast<uint4*>(grow_ptr + c0 + q * 8) = v4;
           }
         }
       }
       fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&acc_empty[a]);
-        mbar_arrive(qkv_ready);
-      }
-      // ---- (2) softmax over the window's keys
-      mbar_wait(s_full, it & 1);
-      tc_fence_after();
-      const uint32_t ts = tmem_S + lane_off;
+      named_bar_sync(1, 128);  // Q / K / V complete; the previous item's O reads are done
+      // ---- (2) scores and softmax over the window's keys
+      wg_mma_128<128, 0, 0, HDP / 16>(
+          sacc, HT_ACC_LD,
+          [&](int h, int k) { return make_smem_desc(sQ + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
+          [&](int k) { return make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ); }, false);
+      named_bar_sync(1, 128);
       const float* brow = bias_s + (row_ok ? j : 0) * S;
       const bool use_bias = p.bias != nullptr;
       float mx = -INFINITY;
       for (int ch = 0; ch < nch; ++ch) {
         const int c0 = wlo + 32 * ch;
         uint32_t raw[32];
-        tmem_ld32(ts + c0, raw);
-        tmem_ld_wait();
+        ld_row32(arow + c0, raw);
 #pragma unroll
         for (int u = 0; u < 32; ++u) {
           const int kk = c0 + u - lo;
@@ -283,8 +247,7 @@ __global__ void __launch_bounds__(HT_THREADS, 1)
       for (int ch = 0; ch < nch; ++ch) {
         const int c0 = wlo + 32 * ch;
         uint32_t raw[32];
-        tmem_ld32(ts + c0, raw);
-        tmem_ld_wait();
+        ld_row32(arow + c0, raw);
         uint32_t pk[16];
 #pragma unroll
         for (int u = 0; u < 32; u += 2) {
@@ -310,19 +273,21 @@ __global__ void __launch_bounds__(HT_THREADS, 1)
         }
       }
       fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      // ---- (3) O epilogue
-      mbar_wait(o_full, it & 1);
-      tc_fence_after();
+      named_bar_sync(1, 128);  // P complete, score reads done
+      // ---- (3) O = P V, epilogue
+      wg_mma_128<HDP, 0, 1, 8>(
+          sacc, HT_ACC_LD,  // 128 keys in steps of 16
+          [&](int h, int ks) {
+            return make_smem_desc(sPu + (ks >> 2) * (HT_ROWS * 128) + h * 64 * 128 + (ks & 3) * 32, 16, 1024, SWZ_128B);
+          },
+          [&](int ks) { return make_smem_desc(sV + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, false);
+      named_bar_sync(1, 128);
       const float inv = row_ok ? 1.f / sum : 0.f;
       __half* orow = p.out + grow * p.ldo + head * HDP;
 #pragma unroll
       for (int c0 = 0; c0 < HDP; c0 += 32) {
         uint32_t raw[32];
-        tmem_ld32(ts + c0, raw);
-        tmem_ld_wait();
+        ld_row32(arow + c0, raw);
         if (row_ok) {
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
@@ -337,14 +302,9 @@ __global__ void __launch_bounds__(HT_THREADS, 1)
           }
         }
       }
-      tc_fence_before();  // the next item's score MMA may overwrite the stage once qkv_ready is signalled again
+      named_bar_sync(1, 128);
+      if (tid == 0) mbar_arrive(ring_free);  // the score tile is read out: the ring may take the next item's loads
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -356,7 +316,9 @@ static int launch_hat(const CUtensorMap& tx, const CUtensorMap& tw, HatParams& p
   if (stages > HT_MAX_STAGES) stages = HT_MAX_STAGES;
   FVIT_CHECK(stages >= 2, "fvit_hat_attn_fwd: S=%d leaves no room for a 2-stage operand ring", p.S);
   p.stages = stages;
-  const size_t smem = fixed + (size_t)stages * STAGE_BYTES;
+  p.ring_bytes = stages * STAGE_BYTES > HT_ACC_BYTES ? stages * STAGE_BYTES : HT_ACC_BYTES;
+  const size_t smem = fixed + (size_t)p.ring_bytes;
+  FVIT_CHECK(smem <= 227 * 1024, "fvit_hat_attn_fwd: S=%d needs %zu B of shared memory", p.S, smem);
   static bool configured = false;
   if (!configured) {
     FVIT_CUDA(cudaFuncSetAttribute(hat_attn_kernel<HDP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));

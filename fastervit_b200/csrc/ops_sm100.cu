@@ -451,8 +451,8 @@ __global__ void __launch_bounds__(256)
 // ------------------------------------------------------------------------------ attention core (SIMT)
 // One CTA per (group of S tokens, head): P = softmax(q k^T * scale + bias[h]) ; out = P v.
 // qkv fp16 [rows, 3C] (q | k | v, head-major inside each), out fp16 [rows, C]. fp32 math throughout.
-// Generic in S and head_dim; used for every attention shape until the tcgen05 path takes over the
-// hot shapes.
+// Generic in S and head_dim; serves the shapes the tensor-core attention kernels do not cover
+// (head dims above 64, windows the key-loop kernel cannot stage).
 __global__ void attn_core_simt_kernel(const __half* __restrict__ qkv, long long ldq, int S, int hd,
                                       int heads, int C, const float* __restrict__ bias, float scale,
                                       __half* __restrict__ out, long long ldo,

@@ -1,11 +1,12 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma /
-// commit / ld / fences) and UMMA shared-memory + instruction descriptors.
-// Hand-written; bit layouts follow the PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor"
-// tables (same fields CUTLASS names in cute/arch/mma_sm100_desc.hpp).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma (fences, shared-memory
+// descriptors, accumulator fragments). Hand-written; the descriptor layout follows the PTX ISA "matrix descriptor"
+// table of wgmma.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace fvit {
 
@@ -85,133 +86,17 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const void* tmap, uint64_
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; single-thread issue.
-__device__ __forceinline__ void umma_f16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 32-bit, 16 consecutive columns: thread t of the warp gets lane (base_lane + t).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
+// ---------------------------------------------------------------- wgmma (one warpgroup = 128 threads)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
-// ---------------------------------------------------------------- CTA pairs (cta_group::2)
-// Two CTAs of a cluster on one TPC share a tcgen05.mma: M = 256 (each CTA owns 128 rows of A and of the TMEM
-// accumulator) and each CTA stages only half of the B tile. The leader (cluster rank 0) issues the MMAs; operands
-// in the peer's shared memory are addressed by the same CTA-local offsets.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `local` (a shared::cta address of this CTA) in the CTA of rank `rank`
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t local, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA loads whose completion is signalled on an mbarrier of either CTA of the pair (bar = shared::cluster address)
-__device__ __forceinline__ void tma_load_2d_cg2(void* dst, const void* tmap, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(tmap), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_cg2(void* dst, const void* tmap, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss_cg2(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on the mbarrier at the same CTA-local offset in both CTAs of the pair once the MMAs issued so far retire.
-__device__ __forceinline__ void umma_commit_cg2(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-      : "memory");
-}
-
-// ---------------------------------------------------------------- UMMA descriptors
 // Shared-memory matrix descriptor (64 bit):
 //  [0,14) start address >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte offset >> 4
-//  [46,48) version (1 on sm_100) | [49,52) base offset | [61,64) swizzle (0 none, 2 128B, 4 64B, 6 32B)
+//  [49,52) base offset | [62,64) layout (0 none, 1 128B, 2 64B, 3 32B swizzle)
+// K-major SW128: SBO = 1024 (8 rows x 128 B), LBO unused; MN-major SW128: LBO = next 64-wide MN atom, SBO = next
+// 8 K rows. The SWZ_* values below are the layout field shifted to bit 61.
 enum : uint32_t { SWZ_NONE = 0, SWZ_128B = 2, SWZ_64B = 4, SWZ_32B = 6 };
 
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes,
@@ -220,18 +105,79 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
   d |= static_cast<uint64_t>(swizzle & 7) << 61;
   return d;
 }
 
-// Instruction descriptor for kind::f16 (fp16 or bf16 operands, fp32 accumulate):
-//  [4,6) D fmt (1 = f32) | [7,10) A fmt | [10,13) B fmt (0 = f16, 1 = bf16) | 15 A major | 16 B major
-//  (0 = K-major, 1 = MN-major) | [17,23) N >> 3 | [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                      uint32_t b_mn_major, uint32_t bf16 = 0) {
-  return (1u << 4) | (bf16 << 7) | (bf16 << 10) | (a_mn_major << 15) | (b_mn_major << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
+// Accumulator fragment of an m64nN wgmma <-> rows [0, 64) of a row-major fp32 tile in shared memory: thread t of
+// the warpgroup holds rows 16*(t/32) + (t%32)/4 (+8), columns 8j + 2*(t%4) (+1).
+template <int N>
+__device__ __forceinline__ void acc_store(float* buf, int ld, const float (&d)[N / 2]) {
+  const int t = threadIdx.x & 127;
+  float* r0 = buf + ((t >> 5) * 16 + ((t & 31) >> 2)) * ld + 2 * (t & 3);
+  float* r1 = r0 + 8 * ld;
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    *reinterpret_cast<float2*>(r0 + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(r1 + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
+}
+template <int N>
+__device__ __forceinline__ void acc_load(const float* buf, int ld, float (&d)[N / 2]) {
+  const int t = threadIdx.x & 127;
+  const float* r0 = buf + ((t >> 5) * 16 + ((t & 31) >> 2)) * ld + 2 * (t & 3);
+  const float* r1 = r0 + 8 * ld;
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const float2 a = *reinterpret_cast<const float2*>(r0 + 8 * j);
+    const float2 b = *reinterpret_cast<const float2*>(r1 + 8 * j);
+    d[4 * j] = a.x, d[4 * j + 1] = a.y, d[4 * j + 2] = b.x, d[4 * j + 3] = b.y;
+  }
+}
+
+// D[128 x N] (+)= sum_k A_k B_k (fp16 operands, fp32 accumulate), computed by the calling warpgroup as two m64
+// halves and left in buf (row-major fp32, leading dimension ld), K = 16 * KSTEPS. adesc(h, k) is the descriptor of
+// rows [64h, 64h + 64) of A for K step k, bdesc(k) that of B. With accumulate, buf holds the previous D.
+// Every thread of the warpgroup calls this; the caller synchronises the warpgroup before others read buf.
+template <int N, int TA, int TB, int KSTEPS, class FA, class FB>
+__device__ __forceinline__ void wg_mma_128(float* buf, int ld, FA adesc, FB bdesc, bool accumulate) {
+#pragma unroll 1
+  for (int h = 0; h < 2; ++h) {
+    float d[N / 2];
+    if (accumulate) {
+      acc_load<N>(buf + h * 64 * ld, ld, d);
+    } else {
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < KSTEPS; ++k) Wgmma<N, TA, TB, 0>::mma(d, adesc(h, k), bdesc(k), 1u);
+    wgmma_commit();
+    wgmma_wait0();
+    acc_store<N>(buf + h * 64 * ld, ld, d);
+  }
+}
+
+// 32 / 16 consecutive fp32 values of an accumulator row (row-per-thread reads of a tile left by wg_mma_128)
+__device__ __forceinline__ void ld_row32(const float* src, uint32_t (&r)[32]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4 v = reinterpret_cast<const float4*>(src)[i];
+    r[4 * i] = __float_as_uint(v.x), r[4 * i + 1] = __float_as_uint(v.y);
+    r[4 * i + 2] = __float_as_uint(v.z), r[4 * i + 3] = __float_as_uint(v.w);
+  }
+}
+__device__ __forceinline__ void ld_row16(const float* src, uint32_t (&r)[16]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float4 v = reinterpret_cast<const float4*>(src)[i];
+    r[4 * i] = __float_as_uint(v.x), r[4 * i + 1] = __float_as_uint(v.y);
+    r[4 * i + 2] = __float_as_uint(v.z), r[4 * i + 3] = __float_as_uint(v.w);
+  }
+}
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 }  // namespace fvit

@@ -1598,7 +1598,7 @@ int fvit_ln_bwd(const void* dy16, int64_t lddy, const int32_t* dy_map, const voi
     const __half* dyh = (const __half*)dy16;
     const __half* xhh = (const __half*)xhat16;
     const int nvl = (C / 8 + 31) / 32;
-    static int prefetch_g = -1;  // fetch g with the operands instead of after the warp reductions (r02h: 4.42 -> 4.22 ms per fv4 step); FVIT_LN_PREFETCH=0 = A/B
+    static int prefetch_g = -1;  // fetch g with the operands instead of after the warp reductions ; FVIT_LN_PREFETCH=0 = A/B
     if (prefetch_g < 0) {
       const char* e = getenv("FVIT_LN_PREFETCH");
       prefetch_g = e ? atoi(e) : 1;

@@ -108,9 +108,8 @@ class Plan:
         self.op_flops: dict[int, float] = {}  # op index -> algorithmic FLOPs (GEMM launches)
         # FVIT_FUSED_HAT=0 falls back to the three-launch attention (qkv GEMM, attention core, proj GEMM) for A/B runs
         # FVIT_FUSED_HAT: "0" = always the three-launch attention (qkv GEMM, attention core, proj GEMM), "1" = the fused
-        # kernel wherever it applies; default = fused for 64-wide (padded) heads, where its one epilogue warpgroup keeps
-        # up with the projection MMAs (fv4 forward: 4.19 ms vs 2.48 + 1.95 ms; measured r02d) — with 32-wide heads the
-        # per-item projection is 4x shorter and the two-CTA-per-SM attention core wins (fv0: 1.80 vs 0.66 + 0.99 ms)
+        # kernel wherever it applies; default = fused for 64-wide (padded) heads, where the projection is long enough to
+        # amortise the kernel's serial projection / softmax phases; 32-wide heads take the three-launch attention
         import os
         self.fused_hat = os.environ.get("FVIT_FUSED_HAT", "auto")
         self.use_graphs = os.environ.get("FVIT_CUDA_GRAPH", "1") != "0" and device.type == "cuda"
@@ -120,8 +119,7 @@ class Plan:
         self.side_branches = sb in ("1", "3")
         self.prep_branches = sb in ("1", "2")
         # weight-gradient GEMMs as side-branch launches too (engine_train.py: _side_from / _before_write): their CTAs fill
-        # the tails of the data-gradient chain's persistent grids (r02s: fv4 step 73.4 -> 72.7 ms, fv0 24.8 -> 24.3 ms).
-        # FVIT_WGRAD_SIDE=0 = A/B switch. Decided at plan build: the markers are inert when side branches are off.
+        # the tails of the data-gradient chain's persistent grids. FVIT_WGRAD_SIDE=0 = A/B switch. Decided at plan build: the markers are inert when side branches are off.
         self.wgrad_side = os.environ.get("FVIT_WGRAD_SIDE", "1") == "1"
         self._graphs: dict = {}
         self._x_static = None
@@ -471,7 +469,7 @@ class Plan:
     @staticmethod
     def _attn_kind(S: int, hdp: int) -> str:
         """Which attention core serves a window sequence of S tokens with padded head dim hdp: "tile" (one 128-row
-        tcgen05 tile, fvit_attn_tc_fwd), "loop" (key-loop tcgen05 kernel for longer windows: its TMA-staged bias rows
+        wgmma tile, fvit_attn_tc_fwd), "loop" (key-loop wgmma kernel for longer windows: its TMA-staged bias rows
         need S % 4 == 0) or "simt" (generic fallback for geometries neither covers)."""
         if hdp > 64:
             return "simt"
@@ -873,7 +871,7 @@ class Engine:
     def _plan(self, x: torch.Tensor) -> Plan:
         if not x.is_cuda:
             raise L.FvitError("FasterViT (fastervit_b200) runs on CUDA only: move the model and input to a "
-                              "B200 (`.cuda()`); there is no CPU / PyTorch fallback path")
+                              "CUDA device (`.cuda()`); there is no CPU / PyTorch fallback path")
         if x.dim() != 4 or x.dtype != torch.float32:
             raise L.FvitError(f"expected a float32 [B, C, H, W] tensor, got {tuple(x.shape)} {x.dtype}")
         p0 = next(self.model.parameters())

@@ -26,6 +26,13 @@ from .engine_train_conv import ConvPartEmitters
 from .engine_train_levels import TokenLevelEmitters
 
 
+def _sm_count() -> int:
+    """SMs of the current device; plans built without one (host-side tests) assume an H100 SXM's 132."""
+    if torch.cuda.is_available():
+        return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    return 132
+
+
 class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
     def __init__(self, model, B: int, H: int, W: int, device):
         self.bwd_ops: list[tuple] = []
@@ -164,9 +171,8 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
 
     def _side_set(self, data_parallel: bool):
         """Launches that go to the side branch. Under a gradient all-reduce the weight-gradient GEMMs stay there too: a
-        second persistent grid does compete with NCCL's CTAs for the SMs the capped launches leave free, but measured on
-        2 x B200 (profiles/r02v_ddp_n2.txt) the step is 75.1 ms with them against 76.8 ms without (73.0 ms on one GPU of
-        the same box). FVIT_WGRAD_SIDE_DDP=0 keeps them on the main branch (A/B switch)."""
+        second persistent grid does compete with NCCL's CTAs for the SMs the capped launches leave free.
+        FVIT_WGRAD_SIDE_DDP=0 keeps them on the main branch (A/B switch)."""
         if not self.side_branches:
             return None
         if data_parallel and os.environ.get("FVIT_WGRAD_SIDE_DDP", "1") != "1":
@@ -179,13 +185,14 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
             self.bwd_ops.append(("wait_side", tuple(ptrs), "wait_side"))
 
     def _split_k(self, m: int, n: int, k_rows: int, ntaps: int = 1) -> int:
-        tiles = ((m + 127) // 128) * ((n + 255) // 256) * ntaps
+        tiles = ((m + 127) // 128) * ((n + 127) // 128) * ntaps
         kb = (k_rows + 63) // 64
+        sms = _sm_count()
         best, best_cost = 1, float("inf")
         for sk in range(1, max(1, min(64, kb // 8)) + 1):
-            # time model (us): waves of CTAs x (K blocks of one unit x 0.26 us per 128x256x64 block + epilogue);
-            # the split-K epilogue is a pass of fp32 vector reductions into L2 (~10 us per tile, measured)
-            cost = -(-tiles * sk // 148) * (kb / sk * 0.26 + (10.0 if sk > 1 else 3.0))
+            # time model (us): waves of CTAs x (K blocks of one unit x ~0.26 us per 128x128x64 block + epilogue);
+            # the split-K epilogue is a pass of fp32 vector reductions into L2 (~10 us per tile)
+            cost = -(-tiles * sk // sms) * (kb / sk * 0.26 + (10.0 if sk > 1 else 3.0))
             if cost < best_cost - 1e-9:
                 best, best_cost = sk, cost
         return best
@@ -274,7 +281,7 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         # enqueued, so NCCL (its own stream) overlaps the rest of the backward pass. The launch list is cut at the
         # bucket points: every segment is one CUDA graph (like the single-GPU backward), the all-reduces in between are
         # ordinary NCCL calls -- collectives captured INTO a graph work too, but live graphs holding NCCL work make
-        # destroy_process_group() hang at exit (seen on 2 x B200, r02j), so they stay outside.
+        # destroy_process_group() hang at exit, so they stay outside.
         self._dlogits[:, :self._ncls].copy_(dlogits)
         red = GradBucketReducer(self.gflat, None if grp is True else grp)
         if getattr(self, "_ar_shadow", None) is None:
@@ -310,18 +317,18 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         """{backward op index: SM cap} for the launches that run while a bucket's all-reduce is in flight. NCCL's CTAs
         cannot co-reside with a GEMM CTA (227 KB of shared memory, one per SM): a full-width persistent grid launched
         into the reduction would run its last CTAs as a second wave, doubling that launch. The window is estimated at
-        plan time: bucket bytes over the measured all-reduce bus bandwidth (B200_PROFILING.md: 725 GB/s at 8 ranks)
-        against the launches' algorithmic FLOPs at the model's typical 700 TFLOP/s; those launches are capped to
-        148 - FVIT_NCCL_CTAS SMs (default 16 = NCCL_MAX_CTAS set by enable_grad_allreduce callers such as bench.py)."""
+        plan time: bucket bytes over the all-reduce bus bandwidth against the launches' algorithmic FLOPs at the
+        model's typical 700 TFLOP/s; those launches are capped to (SM count) - FVIT_NCCL_CTAS SMs (default 16 =
+        NCCL_MAX_CTAS set by enable_grad_allreduce callers such as bench.py)."""
         import os
         reserve = int(os.environ.get("FVIT_NCCL_CTAS", "16"))
         if world <= 1 or reserve <= 0:
             return {}
-        cap = max(8, 148 - reserve)
+        sms = _sm_count()
+        cap = max(8, sms - reserve)
         shadow: dict[int, int] = {}
-        # all-reduce bus bandwidth with NCCL_MAX_CTAS = 16: 8 ranks ~600 GB/s (NVLS), fewer ranks ring over fewer links
-        # (timeline at 2 ranks, profiles/r02h_ddp_timeline.json: the 790 MB level-2 bucket shadows ~6 ms of launches)
-        # -- measured once per plan on the idle fabric (GradBucketReducer.measure_busbw); the table is the fallback
+        # all-reduce bus bandwidth: measured once per plan on the idle fabric (GradBucketReducer.measure_busbw); the
+        # table is the fallback
         if not busbw or busbw <= 0:
             busbw = {2: 200e9, 3: 300e9, 4: 400e9}.get(world, 600e9)
         self.ar_busbw = busbw
@@ -428,7 +435,7 @@ class GradBucketReducer:
 
 def allreduce_mean_(flat: torch.Tensor, group=None) -> torch.Tensor:
     """Data parallel (train.py:542-551): the ONE exchange of the path — the flat gradient buffer is averaged
-    over the ranks with a single all-reduce (NCCL over NVLink/NVSwitch on the B200 box; gloo in the CPU
+    over the ranks with a single all-reduce (NCCL over NVLink / NVSwitch on GPUs; gloo in the CPU
     tests). BatchNorm statistics stay per-GPU like the reference (sync_bn: false)."""
     import torch.distributed as dist
     if not dist.is_available() or not dist.is_initialized():

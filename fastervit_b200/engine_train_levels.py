@@ -417,10 +417,9 @@ def _emit_head_bwd(self, feat: dict) -> None:
 
 
 def _emit_attn_core_bwd(self, at: dict, dao, dqkv, groups: int, S: int) -> None:
-    """backward of the attention core: the tcgen05 tile kernel (S <= 64), the tcgen05 key-loop kernel (S > 128: needs the
+    """backward of the attention core: the wgmma tile kernel (S <= 64), the wgmma key-loop kernel (S > 64: needs the
     forward's output and log-sum-exp; per-pair partial dQ reduced into an fp32 scratch matrix -- any-res S = 148, the
-    14 x 14 ... 48 x 48 windows of the 21k models) or the generic SIMT kernel. (fvit_attn_loop_bwd, the two-tile variant
-    that keeps all of dQ in TMEM, measured 25 % slower on S = 148 / 196 than the eight-softmax-warp kernel: r02t.)"""
+    14 x 14 ... 48 x 48 windows of the 21k models) or the generic SIMT kernel."""
     attn = at["attn"]
     h, hd, hdp, Cp = attn.num_heads, at["hd"], at["hdp"], at["Cp"]
     ops = self.bwd_ops
@@ -446,7 +445,7 @@ def _attn_bwd_entry(S: int, hdp: int, use_tc: bool) -> str:
     """tensor-core attention backward when the tile fits (S <= 64, head slices of 32/64, shared memory budget)"""
     if use_tc and S <= 64 and hdp in (32, 64):
         ss = (S * S * 4 + 15) // 16 * 16
-        if 1024 + 2 * 4 * 128 * hdp * 2 + 2 * 128 * 128 * 2 + 2 * ss + 128 <= 227 * 1024:
+        if 1024 + (2 if hdp == 32 else 1) * 4 * 128 * hdp * 2 + 2 * 128 * 128 * 2 + 128 * 132 * 4 + ss + 128 <= 227 * 1024:
             return "fvit_attn_tc_bwd"
     return "fvit_attn_core_bwd"
 

@@ -101,7 +101,6 @@ _OP_SIGS: dict[str, list] = {
     "fvit_attn_tc_fwd": [_P, _L, _I, _I, _I, _I, _P, _F, _P, _L, _P],
     "fvit_hat_attn_fwd": [_P, _L, _I, _P, _L, _P, _I, _I, _I, _I, _P, _F, _P, _L, _P, _L, _P],
     "fvit_attn_loop_fwd": [_P, _L, _I, _I, _I, _I, _P, _F, _P, _L, _P, _P],
-    "fvit_attn_loop_bwd": [_P, _L, _P, _L, _P, _L, _P, _I, _I, _I, _I, _P, _F, _P, _L, _P, _P],
     "fvit_attn_loop_bwd_long": [_P, _L, _P, _L, _P, _L, _P, _I, _I, _I, _I, _P, _F, _P, _L, _P, _P, _L, _P],
     "fvit_cast_headpad_f16": [_P, _L, _P, _L, _I, _I, _I, _I, _I, _I, _P],
     "fvit_vec_headpad_f32": [_P, _P, _I, _I, _I, _P],

@@ -1,4 +1,4 @@
-"""FasterViT nn.Module whose forward/backward run on the sm_100a kernels of libfvit_sm100.so.
+"""FasterViT nn.Module whose forward/backward run on the sm_90a (H100) kernels of libfvit_sm100.so.
 
 The module tree below exists to own the parameters and buffers under exactly the names, shapes and
 dtypes of the reference `state_dict` (fastervit/models/faster_vit.py, SURVEY.md App. C), so reference
@@ -209,7 +209,7 @@ class FasterViTLayer(_Holder):
 class FasterViT(nn.Module):
     """Drop-in for the reference `FasterViT` (fv.py:846-972 / fvar.py:873-1002): same constructor
     signature, attributes (`num_classes`, `patch_embed`, `levels`, `norm`, `avgpool`, `head`), methods
-    and state_dict; forward/backward execute on B200 kernels."""
+    and state_dict; forward/backward execute on the library's H100 kernels."""
 
     def __init__(self, dim, in_dim, depths, window_size, ct_size, mlp_ratio, num_heads, resolution=224,
                  drop_path_rate=0.2, in_chans=3, num_classes=1000, qkv_bias=True, qk_scale=None,

@@ -40,7 +40,7 @@ def _ru(x: int, m: int) -> int:
 def _require_cuda(t: torch.Tensor, what: str) -> None:
     if not t.is_cuda:
         raise L.FvitError(f"{what} runs on CUDA only (fastervit_b200 has no CPU fallback): move the model to a "
-                          "B200 first")
+                          "CUDA device first")
 
 
 def _device_guard(dev):

@@ -30,7 +30,7 @@ def _make_entrypoint(name: str):
     def entry(pretrained=False, **kwargs):
         return build_model(name, pretrained=pretrained, **kwargs)
     entry.__name__ = entry.__qualname__ = name
-    entry.__doc__ = f"FasterViT entrypoint `{name}` (B200-native); kwargs override {sorted(MODEL_SPECS[name]['defaults'])}."
+    entry.__doc__ = f"FasterViT entrypoint `{name}` (H100-native); kwargs override {sorted(MODEL_SPECS[name]['defaults'])}."
     return entry
 
 

@@ -1,4 +1,4 @@
-/* fvit.h — C ABI of libfvit_sm100.so: the B200 (sm_100a) kernels behind FasterViT.forward/backward.
+/* fvit.h — C ABI of libfvit_sm100.so: the H100 (sm_90a) kernels behind FasterViT.forward/backward.
  *
  * The reference (NVlabs/FasterViT) has no FFI: its hot path is torch.nn modules in
  * fastervit/models/faster_vit.py. Each entry point below replaces the ATen/cuDNN/cuBLAS call sequence
@@ -93,7 +93,7 @@ typedef struct fvit_gemm_args {
   int32_t b_ntaps;       /* 0/1 = off. > 1 (conv weight gradient): the logical output has b_ntaps * n columns; column
                             block t is A^T-style product with B's K rows shifted by tap_shift[t] (A and B MN-major,
                             ntaps == 1): dW[co][t*n + ci] = sum_q dz[q][co] * x[q + tap_shift[t]][ci] */
-  int32_t tile_n;        /* 0 = auto; else multiple of 16 in [16, 256] */
+  int32_t tile_n;        /* 0 = auto; else multiple of 16 in [16, 256] (wider than 128: split into two tiles) */
   /* epilogue */
   float alpha;
   int32_t act;
@@ -125,8 +125,8 @@ typedef struct fvit_gemm_args {
   const float* aux_shift; /* convolution output, scale/shift = that BatchNorm's batch-statistics affine) */
   int32_t pre_is_grad;    /* with act == FVIT_ACT_GELU and out_pre16: store gelu'(v) there instead of v, so the
                              backward GEMM's epilogue is a plain multiply (FVIT_ACT_MUL_AUX) */
-  int32_t cta_group;      /* 0 = chosen by the library; 1 = one CTA per 128-row tile; 2 = CTA pair per 256-row tile
-                             (tcgen05 cta_group::2, each CTA stages half of the B tile; needs m > 128) */
+  int32_t cta_group;      /* 0, 1 or 2; accepted for source compatibility: sm_90a has no CTA-pair MMA, every call
+                             runs one CTA per 128-row tile */
 } fvit_gemm_args;
 
 int fvit_gemm(const fvit_gemm_args* args, void* stream);
@@ -197,16 +197,16 @@ int fvit_attn_core_fwd(const void* qkv, int64_t ldq, int32_t groups, int32_t S, 
                        int32_t head_dim, const float* bias, float scale, void* out, int64_t ldo,
                        float* probs_out, void* stream);
 
-/* Tensor-core version of the same attention core (tcgen05: S = QK^T and O = PV with fp32 accumulators
- * in tensor memory, TMA-staged head slices, per-row softmax by the epilogue warps; scores and
- * probabilities never leave the SM). qkv fp16 [groups*S, 3*heads*hdp] with head_dim zero-padded to
+/* Tensor-core version of the same attention core (wgmma: S = QK^T and O = PV with fp32 accumulators
+ * staged in shared memory, TMA-staged head slices, per-row softmax; scores and probabilities never
+ * leave the SM). qkv fp16 [groups*S, 3*heads*hdp] with head_dim zero-padded to
  * hdp in {32, 64}; out fp16 [groups*S, heads*hdp]; S <= 128. bias fp32 [heads, S, S] or NULL. */
 int fvit_attn_tc_fwd(const void* qkv, int64_t ldq, int32_t groups, int32_t S, int32_t heads, int32_t hdp,
                      const float* bias, float scale, void* out, int64_t ldo, void* stream);
 
 /* The fused hierarchical-attention kernel (north star; WindowAttention.forward faster_vit.py:557-565 with the qkv Linear
  * of faster_vit.py:546): out = softmax((x Wq^T + bq)(x Wk^T + bk)^T * scale + bias)(x Wv^T + bv) per window and head
- * in ONE tcgen05 kernel. xn16 [groups*S, C] is the LayerNorm-ed fp16 activation (norm1 / hat_norm1 output, row stride
+ * in ONE wgmma kernel. xn16 [groups*S, C] is the LayerNorm-ed fp16 activation (norm1 / hat_norm1 output, row stride
  * ldx), wqkv16 the head-padded packed qkv weight [3*heads*hdp, C] (fvit_cast_headpad_f16; row stride ldw), qkv_bias
  * its padded bias [3*heads*hdp] or NULL, bias the relative-position bias [heads, S, S] or NULL. S <= 128, hdp in
  * {32, 64}. out [groups*S, heads*hdp] as fvit_attn_tc_fwd. qkv_out (optional, [groups*S, 3*heads*hdp] fp16) receives
@@ -218,7 +218,7 @@ int fvit_hat_attn_fwd(const void* xn16, int64_t ldx, int32_t C, const void* wqkv
 /* Key-loop tensor-core attention core for window sequences longer than one 128-row tile (any-res level 2:
  * S = 12*12 + 4 = 148, faster_vit_any_res.py:805-817; 21k windows S = 196 .. 2304, faster_vit.py:1253-1418):
  * work item = (window, head, 128 query rows); key tiles of 128 are visited twice (row maxima, then probabilities and
- * O += P V in TMEM). Same qkv / out layout as fvit_attn_tc_fwd; bias [heads, S, S] fp32 is staged by TMA, so
+ * O += P V in an fp32 shared-memory accumulator). Same qkv / out layout as fvit_attn_tc_fwd; bias [heads, S, S] fp32 is staged by TMA, so
  * S % 4 == 0 is required when a bias is given. lse (optional, [groups*S, heads] fp32) receives the log2-domain
  * log-sum-exp of the scaled, biased scores (saved for the backward pass). */
 int fvit_attn_loop_fwd(const void* qkv, int64_t ldq, int32_t groups, int32_t S, int32_t heads, int32_t hdp,
@@ -324,27 +324,19 @@ int fvit_ln_bwd(const void* dy16, int64_t lddy, const int32_t* dy_map, const voi
 int fvit_attn_core_bwd(const void* qkv, int64_t ldq, const void* dout, int64_t lddo, int32_t groups, int32_t S,
                        int32_t heads, int32_t head_dim, int32_t hdp, const float* bias, float scale, void* dqkv,
                        int64_t lddq, float* dbias, void* stream);
-/* Tensor-core version for S <= 64 and hdp in {32, 64} (tcgen05: S = QK^T, dP = dO V^T, then dV = P^T dO,
+/* Tensor-core version for S <= 64 and hdp in {32, 64} (wgmma: S = QK^T, dP = dO V^T, then dV = P^T dO,
  * dK = dS^T Q, dQ = dS K with the P / dS tiles read as MN-major / K-major operands); same contract. */
 int fvit_attn_tc_bwd(const void* qkv, int64_t ldq, const void* dout, int64_t lddo, int32_t groups, int32_t S,
                      int32_t heads, int32_t head_dim, int32_t hdp, const float* bias, float scale, void* dqkv,
                      int64_t lddq, float* dbias, void* stream);
-/* Tensor-core backward for 128 < S <= 256 (S % 4 == 0), the mirror of fvit_attn_loop_fwd: item = (window, head), two
- * key tiles x two query tiles, dV / dK / dQ_0 / dQ_1 accumulate in TMEM; needs the forward's output `out` (for
- * delta = rowsum(dO * O)) and its log-sum-exp vector `lse`. Same dqkv / dbias contract as fvit_attn_core_bwd.
- * (The scratch-free variant: the training plans launch fvit_attn_loop_bwd_long for every S > 128, which measured
- * 25 % faster on S = 148 / 196.) */
-int fvit_attn_loop_bwd(const void* qkv, int64_t ldq, const void* dout, int64_t lddo, const void* out, int64_t ldo,
-                       const float* lse, int32_t groups, int32_t S, int32_t heads, int32_t hdp, const float* bias,
-                       float scale, void* dqkv, int64_t lddq, float* dbias, void* stream);
-/* The same backward for any S (S % 4 == 0; the training plans use it from 65 tokens on): the 24 x 24 / 32 x 32 / 48 x 48 windows of the 21k models
- * (fv.py:1253-1418, WindowAttention.forward fv.py:557-568 differentiated). Key tiles outside, query tiles inside; dV_j /
- * dK_j accumulate in TMEM over the query loop, the per-pair partial dQ_i = dS K_j is added to the row of the fp32
+/* Tensor-core backward for windows longer than the tile kernel takes, the mirror of fvit_attn_loop_fwd (any S with
+ * S % 4 == 0; the training plans use it from 65 tokens on): any-res S = 148, the 24 x 24 / 32 x 32 / 48 x 48 windows of
+ * the 21k models (fv.py:1253-1418, WindowAttention.forward fv.py:557-568 differentiated). Needs the forward's output
+ * `out` (for delta = rowsum(dO * O)) and its log-sum-exp vector `lse`. Key tiles outside, query tiles inside; dV_j /
+ * dK_j accumulate in registers over the query loop, the per-pair partial dQ_i = dS K_j is added to the row of the fp32
  * scratch matrix dq_scratch[groups * S, ld_scratch >= heads * hdp] its owning thread keeps (16-byte stores for the
  * first key tile, 16-byte reductions afterwards: no initialisation needed) and converted to fp16 at the end of the
- * item. Eight softmax warps (two per TMEM lane quarter, 64 score columns each); a pair's bias values are requested
- * before the wait for its score MMAs. Same dqkv / dbias contract as fvit_attn_core_bwd; dq_scratch holds no result
- * afterwards. */
+ * item. Same dqkv / dbias contract as fvit_attn_core_bwd; dq_scratch holds no result afterwards. */
 int fvit_attn_loop_bwd_long(const void* qkv, int64_t ldq, const void* dout, int64_t lddo, const void* out, int64_t ldo,
                             const float* lse, int32_t groups, int32_t S, int32_t heads, int32_t hdp, const float* bias,
                             float scale, void* dqkv, int64_t lddq, float* dbias, float* dq_scratch, int64_t ld_scratch,

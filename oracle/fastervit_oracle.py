@@ -1,7 +1,7 @@
 """CPU oracle for FasterViT.forward — TEST INFRASTRUCTURE, not product code.
 
 A functional restatement (plain torch CPU ops, fp32 or fp64) of the reference algorithm in
-/root/reference/fastervit/models/faster_vit.py ("fv.py") and faster_vit_any_res.py ("fvar.py"),
+the reference's fastervit/models/faster_vit.py ("fv.py") and faster_vit_any_res.py ("fvar.py"),
 driven by a reference-schema state_dict. Only tests/, __graft_entry__.smoke() and bench.py's
 cpu_baseline / --impl reference legs may import this module; the product (fastervit_b200/) never does.
 

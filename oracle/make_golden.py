@@ -1,16 +1,17 @@
-"""Generate tests/golden/*.pt from the UNMODIFIED reference (build container only).
+"""Generate tests/golden/*.pt from the UNMODIFIED reference (a checkout of NVlabs/FasterViT).
 
-    python oracle/make_golden.py [case ...]
+    FASTERVIT_REFERENCE=<path to the reference checkout> python oracle/make_golden.py [case ...]
 
-Imports /root/reference/fastervit behind the 5-symbol timm stand-in (oracle/ref_shim), fills the
+Imports <reference>/fastervit behind the 5-symbol timm stand-in (oracle/ref_shim), fills the
 reference model's own state_dict with deterministic synthetic weights (oracle synth_fill_), runs the
 reference module in fp64 (eval forward; train-mode forward + CrossEntropy backward, drop_path_rate=0)
 and stores logits, loss, per-level activation samples and per-parameter gradient samples. It also runs
 the oracle restatement on the same weights and asserts agreement, which is what pins the oracle.
-The GPU box has no /root/reference: tests read only the committed fixtures.
+The tests never need the reference: they read only the committed fixtures.
 """
 from __future__ import annotations
 
+import os
 import sys
 import time
 import warnings
@@ -21,7 +22,10 @@ import torch
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 sys.path.insert(0, str(ROOT / "oracle" / "ref_shim"))
-sys.path.insert(0, "/root/reference")
+_REF = os.environ.get("FASTERVIT_REFERENCE")
+if not _REF or not Path(_REF, "fastervit").is_dir():
+    raise SystemExit("make_golden.py: set FASTERVIT_REFERENCE to a checkout of NVlabs/FasterViT")
+sys.path.insert(0, _REF)
 warnings.filterwarnings("ignore")
 
 from oracle import fastervit_oracle as O  # noqa: E402
@@ -30,6 +34,7 @@ from oracle.configs import CASES  # noqa: E402
 SEED_W, SEED_X, SEED_T = 1234, 1, 2
 GOLDEN = ROOT / "tests" / "golden"
 MAX_SAMPLE = 512
+GRAD_SAMPLE_STEP = {"fv4": 2}  # 649 gradient tensors: half of each strided sample
 
 
 def sample(t: torch.Tensor) -> torch.Tensor:
@@ -113,6 +118,12 @@ def run_case(case: str) -> None:
         out["train"] = {"batch": b_train, "target": target, "logits": lt.detach().clone(),
                         "loss": loss.item(), "grads": {k: summarize(g) for k, g in grads.items()},
                         "bn_after": {k: summarize(v) for k, v in bn_after.items()}}
+        # every GRAD_SAMPLE_STEP-th point of each gradient sample (the fixture stays under 1 MB)
+        step = GRAD_SAMPLE_STEP.get(case, 1)
+        if step > 1:
+            for d in out["train"]["grads"].values():
+                d["sample"] = d["sample"][::step].clone()
+            out["train"]["grad_sample_step"] = step
         lo_loss, lo_logits, lo_grads = O.loss_and_grads(sd_o, cfg, xt, target, training=True)
         e1 = ((lo_logits - lt.detach()).abs().max() / lt.detach().abs().max()).item()
         # analytically-zero gradients (biases feeding a train-mode BatchNorm, the key bias of a
@@ -129,7 +140,7 @@ def run_case(case: str) -> None:
 
     GOLDEN.mkdir(parents=True, exist_ok=True)
     path = GOLDEN / f"{case}.pt"
-    torch.save(out, path)
+    torch.save(out, path, _use_new_zipfile_serialization=False)  # (the legacy format has no per-tensor padding)
     print(f"{case}: {path.name} {path.stat().st_size / 1024:.0f} KiB, params {out['n_params']:,}, "
           f"oracle-vs-ref eval {err:.2e}"
           + (f", train logits {out['train']['oracle_vs_ref']['logits']:.2e}, grads "

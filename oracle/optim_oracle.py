@@ -1,7 +1,7 @@
 """CPU oracle for the optimizer step of the training loop — TEST INFRASTRUCTURE, not product code.
 
 Restates, on plain torch CPU tensors (fp64 by default), the arithmetic the reference's training loop runs either
-side of `loss.backward()` (/root/reference/fastervit/train.py:879-899):
+side of `loss.backward()` (the reference's fastervit/train.py:879-899):
 
   * `clip_coef`  — `utils.dispatch_clip_grad(..., mode='norm')` = torch.nn.utils.clip_grad_norm_ (train.py:889-892)
   * `adamw_step` — `optimizer.step()` for `--opt adamw` (TRAINING.md:28): torch.optim.AdamW, single-tensor form

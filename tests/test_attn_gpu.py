@@ -1,4 +1,4 @@
-"""GPU parity of the attention cores (tcgen05 fvit_attn_tc_fwd and the generic SIMT fvit_attn_core_fwd)
+"""GPU parity of the attention cores (wgmma fvit_attn_tc_fwd and the generic SIMT fvit_attn_core_fwd)
 against fp32 torch math on the same fp16 q, k, v. Tolerance 2e-3 max-rel: P is rounded to fp16 before
 the PV product in the tensor-core kernel (same as the reference under fp16 autocast)."""
 import pytest
@@ -97,7 +97,7 @@ def test_attn_simt_matches_torch(S, heads, hd, groups):
                                                (60, 8, 32, 5), (36, 4, 24, 13), (53, 8, 32, 1024)])
 @pytest.mark.parametrize("tc", [True, False])
 def test_attn_backward_matches_autograd(S, heads, hd, groups, tc):
-    """dq, dk, dv and dbias of both backward kernels (tcgen05 / SIMT) vs torch autograd in fp32."""
+    """dq, dk, dv and dbias of both backward kernels (wgmma / SIMT) vs torch autograd in fp32."""
     from fastervit_b200 import lib
     lib.load()
     hdp = 32 if hd <= 32 else 64
@@ -133,55 +133,14 @@ def test_attn_backward_matches_autograd(S, heads, hd, groups, tc):
     assert err < 4e-3, ("dbias", err)
 
 
-@pytest.mark.parametrize("S,heads,hd,groups", [(148, 8, 32, 30), (196, 16, 49, 4), (144, 4, 24, 5), (256, 2, 64, 3),
-                                               (132, 3, 32, 7), (148, 8, 32, 200)])
-def test_attn_loop_backward_matches_autograd(S, heads, hd, groups):
-    """dq, dk, dv and dbias of the key-loop tensor-core backward (128 < S <= 256) vs torch autograd in fp32; the
-    forward kernel supplies O and the log-sum-exp rows like the training launch list does."""
-    from fastervit_b200 import lib
-    lib.load()
-    hdp = 32 if hd <= 32 else 64
-    g = torch.Generator(device="cuda").manual_seed(S * 17 + heads + hd)
-    qkv = torch.zeros(groups * S, 3, heads, hdp, device="cuda")
-    qkv[..., :hd] = torch.randn(groups * S, 3, heads, hd, device="cuda", generator=g)
-    qkv16 = qkv.reshape(groups * S, 3 * heads * hdp).half()
-    bias = (torch.randn(heads, S, S, device="cuda", generator=g) * 2 + 4).requires_grad_(True)
-    do = torch.zeros(groups * S, heads, hdp, device="cuda")
-    do[..., :hd] = torch.randn(groups * S, heads, hd, device="cuda", generator=g)
-    do16 = do.reshape(groups * S, heads * hdp).half()
-    scale = hd ** -0.5
-    x = qkv16.float().view(groups, S, 3, heads, hdp)[..., :hd].clone().requires_grad_(True)
-    q, k, v = x.permute(2, 0, 3, 1, 4)
-    p = ((q @ k.transpose(-2, -1)) * scale + bias[None]).softmax(-1)
-    o = (p @ v).permute(0, 2, 1, 3)
-    o.backward(do16.float().view(groups, S, heads, hdp)[..., :hd])
-    ref = torch.zeros(groups, S, 3, heads, hdp, device="cuda")
-    ref[..., :hd] = x.grad
-    ref = ref.reshape(groups * S, 3 * heads * hdp)
-    out16 = torch.zeros(groups * S, heads * hdp, device="cuda", dtype=torch.half)
-    lse = torch.zeros(groups * S, heads, device="cuda")
-    lib.call("fvit_attn_loop_fwd", qkv16.data_ptr(), qkv16.stride(0), groups, S, heads, hdp, bias.data_ptr(), scale,
-             out16.data_ptr(), out16.stride(0), lse.data_ptr())
-    dqkv = torch.full((groups * S, 3 * heads * hdp), float("nan"), device="cuda", dtype=torch.half)
-    dbias = torch.zeros(heads, S, S, device="cuda")
-    lib.call("fvit_attn_loop_bwd", qkv16.data_ptr(), qkv16.stride(0), do16.data_ptr(), do16.stride(0), out16.data_ptr(),
-             out16.stride(0), lse.data_ptr(), groups, S, heads, hdp, bias.data_ptr(), scale, dqkv.data_ptr(), dqkv.stride(0),
-             dbias.data_ptr())
-    torch.cuda.synchronize()
-    assert torch.isfinite(dqkv.float()).all()
-    for w, nm in enumerate("qkv"):
-        sl = slice(w * heads * hdp, (w + 1) * heads * hdp)
-        err = ((dqkv[:, sl].float() - ref[:, sl]).abs().max() / ref[:, sl].abs().max()).item()
-        assert err < 4e-3, (nm, err)
-    err = ((dbias - bias.grad).abs().max() / bias.grad.abs().max()).item()
-    assert err < 4e-3, ("dbias", err)
-
-
 @pytest.mark.parametrize("S,heads,hd,groups", [(576, 4, 24, 3), (260, 2, 32, 5), (384, 3, 49, 2), (1024, 2, 64, 2),
                                                (148, 8, 32, 9), (576, 16, 49, 150), (2304, 1, 32, 1),
-                                               (68, 4, 16, 12), (104, 8, 32, 7), (128, 2, 64, 5), (100, 3, 49, 200)])
+                                               (68, 4, 16, 12), (104, 8, 32, 7), (128, 2, 64, 5), (100, 3, 49, 200),
+                                               (196, 16, 49, 4), (144, 4, 24, 5), (256, 2, 64, 3), (132, 3, 32, 7),
+                                               (148, 8, 32, 200)])
 def test_attn_loop_long_backward_matches_autograd(S, heads, hd, groups):
-    """fvit_attn_loop_bwd_long (any number of 128-row tiles: the 21k models' 576 / 1024 / 2304-token windows): dq, dk,
+    """fvit_attn_loop_bwd_long (any number of 128-row tiles: the any-res S = 148 windows, the 21k models' 576 / 1024 /
+    2304-token windows): dq, dk,
     dv and dbias vs torch autograd in fp32. dq goes through the fp32 scratch matrix (NaN-filled here: the kernel must
     not depend on its contents)."""
     from fastervit_b200 import lib
@@ -235,7 +194,7 @@ def test_attn_loop_long_backward_matches_autograd(S, heads, hd, groups):
                                                  (53, 8, 32, 1024, 256), (85, 4, 16, 4, 64)])
 @pytest.mark.parametrize("save_qkv", [False, True])
 def test_fused_hat_attention_matches_unfused_math(S, heads, hd, groups, C, save_qkv):
-    """fvit_hat_attn_fwd (QKV projection + softmax(QK^T + bias) + PV in one tcgen05 kernel) against fp32 torch on
+    """fvit_hat_attn_fwd (QKV projection + softmax(QK^T + bias) + PV in one wgmma kernel) against fp32 torch on
     the same fp16 activations / head-padded weights, with q, k, v rounded to fp16 as the kernel's operand tiles are."""
     from fastervit_b200 import lib
     lib.load()

@@ -1,4 +1,4 @@
-"""GPU parity: FasterViT forward on the sm_100a kernels vs the golden logits produced by the unmodified
+"""GPU parity: FasterViT forward on the sm_90a kernels vs the golden logits produced by the unmodified
 reference in fp64 (tests/golden/*.pt, see oracle/make_golden.py). Tolerance: the north-star's
 "outputs within 1e-3 rel" measured as max|d|/max|ref| and as relative L2."""
 import pytest
