@@ -1,14 +1,17 @@
 // fvit_gemm: persistent, warp-specialised wgmma GEMM for sm_90a.
 //
-//   warp 8      : TMA producer (one lane) — cp.async.bulk.tensor boxes into a ring of 128B-swizzled
-//                 shared-memory stages, mbarrier complete_tx signalling; it runs ahead into the next
-//                 tiles while the consumers work on their epilogue
-//   warps 0..7  : two consumer warpgroups — wgmma.mma_async m64 x N x 16 (N = the MMA width of the
-//                 tile, 32 / 64 / 96 / 128), warpgroup g owns rows [64g, 64g + 64) of the 128-row tile
-//                 with fp32 accumulators in registers; at the end of a tile both write them to a
-//                 shared-memory accumulator tile, and the eight warps run the epilogue from there:
-//                 fused scale/shift/activation/layer-scale/residual, optional per-column statistics,
-//                 row-map scatter, coalesced 16-byte global accesses
+//   warp 12     : TMA producer (one lane; warps 13..15 of its warpgroup only give their registers to the
+//                 epilogue) — cp.async.bulk.tensor boxes into a ring of 128B-swizzled shared-memory stages,
+//                 mbarrier complete_tx signalling; it runs ahead into the next tiles
+//   warps 0..7  : two MMA warpgroups — wgmma.mma_async m64 x N x 16, warpgroup g owns rows [64g, 64g + 64)
+//                 of the 128-row tile with fp32 accumulators in registers. N is the tile's width rounded up
+//                 to 16, per work unit: a partial last N tile issues only the columns it has. At the end of
+//                 a unit both wait for acc_empty, write the accumulators to the shared-memory accumulator
+//                 tile, arrive on acc_full and start the next unit's K loop at once
+//   warps 8..11 : the epilogue warpgroup — waits for acc_full, runs the epilogue from the accumulator tile
+//                 (fused scale/shift/activation/layer-scale/residual, optional per-column statistics,
+//                 row-map scatter, coalesced 16-byte global accesses) and arrives on acc_empty after its
+//                 last read of the tile, so one unit's epilogue overlaps the next unit's MMAs
 //
 // The A operand of K-block kb is the 2-D box at row (m0 + tap_shift[tap]) of plane tap_plane[tap]:
 // with 9 taps this is an im2col-free 3x3 convolution over a zero-bordered NHWC activation matrix
@@ -17,7 +20,8 @@
 #include <cuda_bf16.h>
 
 #include <mutex>
-#include <unordered_map>
+#include <map>
+#include <tuple>
 
 #include "../../include/fvit.h"
 #include "common.h"
@@ -28,9 +32,16 @@ namespace fvit {
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 x 16-bit = 128 B: one SWIZZLE_128B row
 constexpr int MMA_K = 16;
-constexpr int NEPI = 8;                         // consumer warps: two warpgroups, each owning 64 rows of the tile
+constexpr int MMA_WARPS = 8;                    // two MMA warpgroups, each owning 64 rows of the tile
+constexpr int MMA_THREADS = 32 * MMA_WARPS;
+constexpr int NEPI = 4;                         // epilogue warps: one warpgroup
 constexpr int EPI_THREADS = 32 * NEPI;
-constexpr int GEMM_THREADS = EPI_THREADS + 32;  // consumers + the TMA warp
+constexpr int TMA_WARP = MMA_WARPS + NEPI;      // first warp of the producer warpgroup (its other 3 warps idle)
+constexpr int GEMM_THREADS = MMA_THREADS + EPI_THREADS + 128;
+// Registers per thread (launch: 128). Every SM sub-partition holds one warp of each warpgroup, so the producer's
+// surplus goes to the epilogue: 40 + 128 + 128 + 216 = 4 x 128.
+constexpr uint32_t PRODUCER_REGS = 40;
+constexpr uint32_t EPILOGUE_REGS = 216;
 constexpr int MAX_STAGES = 8;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
 constexpr int MAX_TILE_N = 128;             // widest MMA of the kernel (the accumulator tile lives in shared memory)
@@ -54,7 +65,6 @@ struct GemmParams {
   int b_ntaps, tiles_per_tap;  // >1: N tiles enumerate (tap, n tile); tap t reads B rows shifted by tap_shift[t]
   int atomic_out;  // split-K style accumulation: atomicAdd(alpha * acc) into out_f32
   int stages;
-  int mma_n;  // MMA width: tile_n rounded up to 32 / 64 / 96 / 128 (columns >= tile_n are computed and dropped)
   int tap_shift[16];
   int tap_plane[16];
   // epilogue
@@ -198,13 +208,28 @@ __device__ __forceinline__ void decode_work(const GemmParams& p, int w, int& tm,
   tm = t / p.tiles_n;
 }
 
-// Main loop of one work unit for MMA width N: the consumer warpgroup g accumulates rows [64g, 64g + 64) of the tile
+// Output columns [n0, n_end) of work unit tile tn (with taps in N: columns [tap * n, (tap + 1) * n) hold tap tap).
+__device__ __forceinline__ void unit_cols(const GemmParams& p, int tn, int& n0, int& n_end) {
+  n0 = tn * p.tile_n;
+  n_end = min(p.n, n0 + p.tile_n);
+  if (p.b_ntaps > 1) {
+    const int tap = tn / p.tiles_per_tap;
+    n0 = tap * p.n + (tn - tap * p.tiles_per_tap) * p.tile_n;
+    n_end = min((tap + 1) * p.n, n0 + p.tile_n);
+  }
+}
+
+// Main loop of one work unit for MMA width N: the MMA warpgroup g accumulates rows [64g, 64g + 64) of the tile
 // over K blocks [kb0, kb1) and leaves them in the shared-memory accumulator tile. One K block's MMAs stay in flight
 // while the next block's are issued; each warp releases a ring stage once its warpgroup's MMAs on it have completed.
+// The accumulator tile is written once the epilogue has released it (acc_empty of the previous unit, acc_parity =
+// the parity of this CTA's unit count) and handed over through acc_full. Columns >= N of the tile keep the values
+// of an earlier unit: the epilogue only reads the unit's valid columns.
 template <int N, int TA, int TB, int BF16>
 __device__ __forceinline__ void gemm_mainloop(const GemmParams& p, uint8_t* smem, int stage_bytes, uint64_t* full_bar,
                                               uint64_t* empty_bar, int& stage, uint32_t& phase, int kb0, int kb1,
-                                              float* accbuf) {
+                                              float* accbuf, uint64_t* acc_full, uint64_t* acc_empty,
+                                              uint32_t acc_parity) {
   const int g = (threadIdx.x >> 7) & 1;
   const int lane = threadIdx.x & 31;
   // K-major SW128: SBO = 1024 (8 rows x 128 B), LBO unused; MN-major SW128: LBO = BK*128 (next 64-wide MN atom),
@@ -251,19 +276,30 @@ __device__ __forceinline__ void gemm_mainloop(const GemmParams& p, uint8_t* smem
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[prev]);
   }
+  mbar_wait(acc_empty, acc_parity ^ 1);  // the epilogue has read the previous unit's tile
   acc_store<N>(accbuf + g * 64 * ACC_LD, ACC_LD, d);
+  mbar_arrive(acc_full);
 }
 
 template <int TA, int TB, int BF16>
-__device__ __forceinline__ void gemm_mainloop_n(const GemmParams& p, uint8_t* smem, int stage_bytes, uint64_t* full_bar,
-                                                uint64_t* empty_bar, int& stage, uint32_t& phase, int kb0, int kb1,
-                                                float* accbuf) {
-  switch (p.mma_n) {
-    case 32: gemm_mainloop<32, TA, TB, BF16>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf); break;
-    case 64: gemm_mainloop<64, TA, TB, BF16>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf); break;
-    case 96: gemm_mainloop<96, TA, TB, BF16>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf); break;
-    default: gemm_mainloop<128, TA, TB, BF16>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf); break;
+__device__ __forceinline__ void gemm_mainloop_n(int mma_n, const GemmParams& p, uint8_t* smem, int stage_bytes,
+                                                uint64_t* full_bar, uint64_t* empty_bar, int& stage, uint32_t& phase,
+                                                int kb0, int kb1, float* accbuf, uint64_t* acc_full,
+                                                uint64_t* acc_empty, uint32_t acc_parity) {
+#define FVIT_MAINLOOP(N)                                                                                              \
+  gemm_mainloop<N, TA, TB, BF16>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf, acc_full, \
+                                 acc_empty, acc_parity)
+  switch (mma_n) {
+    case 16: FVIT_MAINLOOP(16); break;
+    case 32: FVIT_MAINLOOP(32); break;
+    case 48: FVIT_MAINLOOP(48); break;
+    case 64: FVIT_MAINLOOP(64); break;
+    case 80: FVIT_MAINLOOP(80); break;
+    case 96: FVIT_MAINLOOP(96); break;
+    case 112: FVIT_MAINLOOP(112); break;
+    default: FVIT_MAINLOOP(128); break;
   }
+#undef FVIT_MAINLOOP
 }
 
 template <uint32_t FEAT>
@@ -277,30 +313,35 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   const int lane = threadIdx.x & 31;
 
   const int unit0 = blockIdx.x, nunits = gridDim.x;  // work units are dealt to CTAs round-robin
-  // MN-major B is staged as whole 64-column atoms (the MMA reads the first mma_n columns of them)
-  const int b_stage_bytes = (p.b_mn ? ((p.mma_n + 63) & ~63) : p.mma_n) * BK * 2;
+  // MN-major B is staged as whole 64-column atoms (the MMA reads the first columns of them)
+  const int b_stage_bytes = (p.b_mn ? ((p.tile_n + 63) & ~63) : p.tile_n) * BK * 2;
   const int stage_bytes = A_STAGE_BYTES + b_stage_bytes;
   uint8_t* ctrl = smem + p.stages * stage_bytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ctrl);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
+  uint64_t* acc_full = empty_bar + MAX_STAGES;  // accumulator tile written (MMA warpgroups -> epilogue)
+  uint64_t* acc_empty = acc_full + 1;           // accumulator tile read (epilogue -> MMA warpgroups)
   float* accbuf = reinterpret_cast<float*>(ctrl + SMEM_CTRL_BYTES);
 
-  if (warp == NEPI && lane == 0) {
+  if (warp == TMA_WARP && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], NEPI);  // one arrival per consumer warp
+      mbar_init(&empty_bar[s], MMA_WARPS);  // one arrival per MMA warp
     }
+    mbar_init(acc_full, MMA_THREADS);  // every thread arrives after its own accumulator stores
+    mbar_init(acc_empty, EPI_THREADS);  // every thread arrives after its own accumulator reads
     fence_mbar_init();
   }
   __syncthreads();
 
   const int work_total = p.tiles_m * p.tiles_n * p.split_k;
 
-  if (warp == NEPI) {
+  if (warp >= TMA_WARP) {
     // ===================================================================== TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == TMA_WARP && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int w = unit0; w < work_total; w += nunits) {
@@ -344,17 +385,46 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         }
       }
     }
+  } else if (warp < MMA_WARPS) {
+    // ===================================================================== MMA warpgroups
+    int stage = 0;
+    uint32_t phase = 0;
+    uint32_t acc_parity = 0;
+    for (int w = unit0; w < work_total; w += nunits, acc_parity ^= 1) {
+      int tm, tn, split_;
+      decode_work(p, w, tm, tn, split_);
+      int n0, n_end;
+      unit_cols(p, tn, n0, n_end);
+      const int mma_n = (n_end - n0 + 15) & ~15;  // a partial last N tile issues only its own columns
+      const int kb0 = (int)((long long)p.num_kb * split_ / p.split_k);
+      const int kb1 = (int)((long long)p.num_kb * (split_ + 1) / p.split_k);
+#define FVIT_MAINLOOP_N(TA, TB, BF)                                                                        \
+  gemm_mainloop_n<TA, TB, BF>(mma_n, p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf, \
+                              acc_full, acc_empty, acc_parity)
+      if ((FEAT & EF_GENERIC) && p.bf16) {
+        if (!p.a_mn && !p.b_mn) FVIT_MAINLOOP_N(0, 0, 1);
+        else if (!p.a_mn) FVIT_MAINLOOP_N(0, 1, 1);
+        else if (!p.b_mn) FVIT_MAINLOOP_N(1, 0, 1);
+        else FVIT_MAINLOOP_N(1, 1, 1);
+      } else {
+        if (!p.a_mn && !p.b_mn) FVIT_MAINLOOP_N(0, 0, 0);
+        else if (!p.a_mn) FVIT_MAINLOOP_N(0, 1, 0);
+        else if (!p.b_mn) FVIT_MAINLOOP_N(1, 0, 0);
+        else FVIT_MAINLOOP_N(1, 1, 0);
+      }
+#undef FVIT_MAINLOOP_N
+    }
   } else {
-    // ===================================================================== consumer warpgroups
-    // Per work unit: main loop (wgmma into registers) -> accumulator tile in shared memory -> epilogue. In the
-    // epilogue warp w owns rows 32*(w & 3) .. +32 of the tile and every second 32-column chunk ((w >> 2) selects
-    // even / odd chunks). Per chunk a warp
+    // ===================================================================== epilogue warpgroup
+    // Per work unit: wait for the accumulator tile, run the epilogue from it, release it. Warp w of the group owns
+    // rows 32*w .. +32 of the tile and walks its 32-column chunks. Per chunk a warp
     //   1. issues its residual / aux global loads,
     //   2. reads the accumulators of its chunk from the shared-memory tile,
     //   3. works "coalesced": one instruction covers 4 rows x 128 contiguous bytes (8 lanes x float4
     //      per row), so residual loads and fp32 / fp16 stores are full-line accesses.
-    const int quad = warp & 3;  // 32-row quarter of the tile this warp's epilogue covers
-    const int chunk_par = warp >> 2;
+    setmaxnreg_inc<EPILOGUE_REGS>();
+    const int quad = warp - MMA_WARPS;  // 32-row quarter of the tile this warp's epilogue covers
+    const int et = threadIdx.x - MMA_THREADS;  // thread index within the epilogue warpgroup
     // per-CTA partial BatchNorm statistics (sum | sum of squares), flushed with one atomic per column at the end
     float* stat_s = reinterpret_cast<float*>(ctrl + SMEM_CTRL_BYTES + SMEM_ACC_BYTES);
     const int sub = lane >> 3;   // row within a 4-row group
@@ -376,45 +446,23 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     const bool osum = GENERIC ? (p.osum != nullptr) : ((FEAT & EF_OSUM) != 0);
     const float alpha = has_aptr ? p.alpha * __ldg(p.alpha_ptr) : p.alpha;
     if (stats) {
-      for (int i = threadIdx.x; i < 2 * p.n; i += EPI_THREADS) stat_s[i] = 0.f;
+      for (int i = et; i < 2 * p.n; i += EPI_THREADS) stat_s[i] = 0.f;
       asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");  // the epilogue warps only
     }
     if (osum) {  // tile-local column sums: stat_s[0 .. tile_n)
-      stat_s[threadIdx.x] = 0.f;
+      stat_s[et] = 0.f;
       asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
     }
     const float osum_alpha = (osum && p.osum_alpha) ? __ldg(p.osum_alpha) : 1.f;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int w = unit0; w < work_total; w += nunits) {
+    uint32_t acc_parity = 0;
+    for (int w = unit0; w < work_total; w += nunits, acc_parity ^= 1) {
       int tm, tn, split_;
       decode_work(p, w, tm, tn, split_);
       const int row_base = tm * BM + quad * 32;
-      {
-        const int kb0 = (int)((long long)p.num_kb * split_ / p.split_k);
-        const int kb1 = (int)((long long)p.num_kb * (split_ + 1) / p.split_k);
-        asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");  // the previous tile's epilogue is done with accbuf
-        if (GENERIC && p.bf16) {
-          if (!p.a_mn && !p.b_mn) gemm_mainloop_n<0, 0, 1>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
-          else if (!p.a_mn) gemm_mainloop_n<0, 1, 1>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
-          else if (!p.b_mn) gemm_mainloop_n<1, 0, 1>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
-          else gemm_mainloop_n<1, 1, 1>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
-        } else {
-          if (!p.a_mn && !p.b_mn) gemm_mainloop_n<0, 0, 0>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
-          else if (!p.a_mn) gemm_mainloop_n<0, 1, 0>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
-          else if (!p.b_mn) gemm_mainloop_n<1, 0, 0>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
-          else gemm_mainloop_n<1, 1, 0>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf);
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");  // accumulator tile complete
-      }
-      int n0 = tn * p.tile_n;
-      int n_end = min(p.n, n0 + p.tile_n);
-      if (p.b_ntaps > 1) {  // output columns [tap * n, (tap + 1) * n)
-        const int tap = tn / p.tiles_per_tap;
-        n0 = tap * p.n + (tn - tap * p.tiles_per_tap) * p.tile_n;
-        n_end = min((tap + 1) * p.n, n0 + p.tile_n);
-      }
-      // output rows of the 8 tile rows this lane touches (4k + sub), fetched once per tile
+      int n0, n_end;
+      unit_cols(p, tn, n0, n_end);
+      // output rows of the 8 tile rows this lane touches (4k + sub), fetched once per tile (before the wait: row_map
+      // reads do not depend on the accumulators)
       long long orow[8];
       {
         long long my_orow = -1;
@@ -423,6 +471,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 #pragma unroll
         for (int k = 0; k < 8; ++k) orow[k] = __shfl_sync(0xffffffffu, my_orow, 4 * k + sub);
       }
+      mbar_wait(acc_full, acc_parity);
 
       const float* arow = accbuf + (quad * 32 + lane) * ACC_LD;  // this lane's accumulator row (row-per-thread reads)
 
@@ -437,7 +486,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         uint16_t* const orow16 = reinterpret_cast<uint16_t*>(p.out_f16) + (my_orow >= 0 ? my_orow : 0) * p.ld_o16;
         uint16_t* const prow16 = reinterpret_cast<uint16_t*>(p.out_pre16) + (long long)my_row * p.ld_pre16;
         const uint16_t* const arow16 = reinterpret_cast<const uint16_t*>(p.aux) + (long long)my_row * p.ld_aux;
-        for (int c0 = chunk_par * 32; c0 < p.tile_n; c0 += 32 * (NEPI / 4)) {
+        for (int c0 = 0; c0 < p.tile_n; c0 += 32) {
           const int nbase = n0 + c0;
           if (nbase >= n_end) break;  // warp-uniform
           const int nvalid = min(min(32, n_end - nbase), p.tile_n - c0);   // 16 or 32
@@ -539,7 +588,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
         }
       } else
-      for (int c0 = chunk_par * 32; c0 < p.tile_n; c0 += 32 * (NEPI / 4)) {
+      for (int c0 = 0; c0 < p.tile_n; c0 += 32) {
         const int nbase = n0 + c0;
         if (nbase >= n_end) break;  // warp-uniform
         const int col = nbase + 4 * c4;            // first of this lane's 4 columns
@@ -737,9 +786,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
         }
       }
+      mbar_arrive(acc_empty);  // this thread's last read of the accumulator tile is done
       if (osum) {  // flush this tile's column sums: one global atomic per column per tile
         asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-        const int lc = threadIdx.x;
+        const int lc = et;
         if (lc < p.tile_n && n0 + lc < n_end) {
           const float a = stat_s[lc];
           if (a != 0.f) atomicAdd(p.osum + n0 + lc, a * osum_alpha);
@@ -750,7 +800,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     }
     if (stats) {
       asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-      for (int i = threadIdx.x; i < p.n; i += EPI_THREADS) {
+      for (int i = et; i < p.n; i += EPI_THREADS) {
         const float a = stat_s[i], b = stat_s[p.n + i];
         if (a != 0.f || b != 0.f) {
           atomicAdd(p.col_sum + i, a);
@@ -762,21 +812,48 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 }
 
 // ------------------------------------------------------------------------------------------ host
-// Wave model of the tile width: waves of work units over the SMs, each unit costing its MMA time (~ tile_n per K
-// block) plus a fixed part for the A stream / epilogue setup. MMA widths are 32 / 64 / 96 / 128.
-static int pick_tile_n(int m, int n, int split_k, int sms) {
+// Cost model of the tile width: the work units are dealt round-robin to min(units, SMs) persistent CTAs and the
+// busiest CTA decides. A unit costs the MMA columns it issues (~ MMA time per K block; a partial last N tile issues
+// its width rounded up to 16) plus a fixed part for the unit's A operand stream (16 KB per K block, the bytes of
+// 128 B columns). The fixed part, 160 columns, is fitted to tile_n 32 / 64 / 96 / 128 timings of four linear shapes
+// (M x N x K = 27136 x 784 x 784, 27136 x 3136 x 784, 27136 x 784 x 3136, 6272 x 1568 x 1568; fv4 levels 2 and 3) on
+// an H100 SXM at 400 W; times relative to tile_n 128:
+//   tile_n 32: 1.96 / 2.47 / 3.06 / 2.76   64: 1.27 / 1.39 / 1.56 / 1.61   96: 1.09 / 1.05 / 1.14 / 1.24
+// Units enumerate N tiles in decode_work's order. Cached per shape.
+static int pick_tile_n(int m, int n, int split_k, int b_ntaps, int sms) {
+  constexpr double kUnitFixed = 160.0;
+  static std::mutex mu;
+  static std::map<std::tuple<int, int, int, int, int>, int> cache;
+  const auto key = std::make_tuple(m, n, split_k, b_ntaps, sms);
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = cache.find(key);
+  if (it != cache.end()) return it->second;
   int best = 32;
   double best_cost = 1e30;
   const int tiles_m = ceil_div(m, BM);
   for (int bn = 32; bn <= MAX_TILE_N; bn += 32) {
-    const long long work = (long long)tiles_m * ceil_div(n, bn) * split_k;
-    const long long waves = (work + sms - 1) / sms;
-    const double cost = (double)waves * (bn + 48.0);
+    const int tiles_per_tap = ceil_div(n, bn);
+    const int tiles_n = tiles_per_tap * b_ntaps;
+    const int tail = (n - (tiles_per_tap - 1) * bn + 15) & ~15;
+    const long long nt = (long long)tiles_m * tiles_n;
+    const long long work = nt * split_k;
+    const int ctas = (int)(work < sms ? work : sms);
+    double cost = 0.0;
+    for (int c = 0; c < ctas; ++c) {
+      double busy = 0.0;
+      for (long long w = c; w < work; w += ctas) {
+        const long long t = b_ntaps > 1 ? w % nt : w / split_k;  // as decode_work
+        const int tn = (int)(t % tiles_n) % tiles_per_tap;      // N tile within its tap
+        busy += (tn == tiles_per_tap - 1 ? tail : bn) + kUnitFixed;
+      }
+      cost = busy > cost ? busy : cost;
+    }
     if (cost < best_cost - 1e-9) {
       best_cost = cost;
       best = bn;
     }
   }
+  cache.emplace(key, best);
   return best;
 }
 
@@ -823,7 +900,8 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   FVIT_CHECK(a->cta_group >= 0 && a->cta_group <= 2, "fvit_gemm: cta_group=%d invalid", a->cta_group);
   const int sms = num_sms();
   // a requested width above the widest MMA is split into two equal tiles (multiples of 16)
-  int tile_n = a->tile_n > 0 ? a->tile_n : pick_tile_n(a->m, a->n, split_k * b_ntaps, sms);
+  const int num_kb = ceil_div(a->kc, BK) * a->ntaps;
+  int tile_n = a->tile_n > 0 ? a->tile_n : pick_tile_n(a->m, a->n, split_k < num_kb ? split_k : num_kb, b_ntaps, sms);
   if (tile_n > MAX_TILE_N) tile_n = ceil_div(tile_n, 32) * 16;
 
   GemmParams p;
@@ -831,7 +909,7 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   p.m = a->m;
   p.n = a->n;
   p.kb_per_tap = ceil_div(a->kc, BK);
-  p.num_kb = p.kb_per_tap * a->ntaps;
+  p.num_kb = num_kb;
   {
     static int kskip = -1;  // FVIT_GEMM_KSKIP=0: issue the zero-filled K steps too (A/B)
     if (kskip < 0) {
@@ -846,7 +924,6 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   p.a_row_off = a->a_row_off;
   p.b_row_off = a->b_row_off;
   p.tile_n = tile_n;
-  p.mma_n = ceil_div(tile_n, 32) * 32;
   p.tiles_m = ceil_div(a->m, BM);
   p.tiles_n = ceil_div(a->n, tile_n);
   p.b_ntaps = a->b_ntaps > 1 ? a->b_ntaps : 1;
@@ -855,7 +932,7 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   p.split_k = split_k < p.num_kb ? split_k : p.num_kb;
   if (p.split_k < 1) p.split_k = 1;
   p.atomic_out = split_k > 1 ? 1 : 0;
-  const int stage_bytes = A_STAGE_BYTES + (a->b_mn_major ? ((p.mma_n + 63) & ~63) : p.mma_n) * BK * 2;
+  const int stage_bytes = A_STAGE_BYTES + (a->b_mn_major ? ((tile_n + 63) & ~63) : tile_n) * BK * 2;
   const int stats_bytes = a->col_sum ? SMEM_STATS_BYTES : (a->out_colsum ? 256 * 4 : 0);
   int stages = (SMEM_BUDGET - SMEM_CTRL_BYTES - SMEM_ALIGN_SLACK - SMEM_ACC_BYTES - stats_bytes) / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
