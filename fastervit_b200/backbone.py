@@ -4,9 +4,10 @@ level's Downsample (`xo`, fastervit.py:705-709), one BatchNorm2d `norm{i}` per r
 `forward_raw(x) -> tuple of [B, C_i, H_i, W_i]`, `forward(tensors, mask) -> {idx: (features, mask)}` with the padding
 mask resized to every level (fastervit.py:829-846), frozen stages (fastervit.py:803-815).
 
-The hot path is the same sm_90a launch list as classification: the wrapped model's eval plan is run up to the points
-where the level outputs are live and `fvit_feature_map_fwd` applies the level's folded BatchNorm while converting the
-token-major activation to NCHW. Variable input sizes go through the any-res entrypoints (one cached plan per shape; the
+The hot path is the same sm_90a launch list as classification: in eval the wrapped model's eval plan is run up to the
+points where the level outputs are live and `fvit_feature_map_fwd` applies the level's folded BatchNorm while
+converting the token-major activation to NCHW. In train mode a levels-mode train plan (engine_train.py) applies each
+norm{i} with batch statistics and differentiates through it (`fvit_feature_map_bwd`). Variable input sizes go through the any-res entrypoints (one cached plan per shape; the
 level geometry is padded to window multiples exactly as faster_vit_any_res.py:851-867 does).
 """
 from __future__ import annotations
@@ -53,12 +54,19 @@ class FasterViTBackbone(nn.Module):
         self._freeze_stages()
         return self
 
-    @torch.no_grad()
     def forward_raw(self, x: torch.Tensor) -> tuple:
-        """fastervit.py:816-827: tuple of the normalised level outputs, NCHW."""
+        """fastervit.py:816-827: tuple of the normalised level outputs, NCHW. Under .train() (detector fine-tuning,
+        dino/backbone.py:158-160) the body runs its training launch list up to the highest requested level, every
+        norm{i} normalises with batch statistics (running statistics updated) and the outputs are differentiable;
+        the frozen prefix runs on running statistics and gets no gradient."""
         if self.training:
-            raise L.FvitError("FasterViTBackbone runs the inference launch list (call .eval()); fine-tuning a detector "
-                              "end to end through the backbone is outside the classification hot path")
+            norms = [getattr(self, f"norm{i}") for i in self.out_indices]
+            return self.body._get_engine().forward_levels(x, self.out_indices, norms=norms,
+                                                          frozen_stages=self.frozen_stages)
+        with torch.no_grad():
+            return self._forward_raw_eval(x)
+
+    def _forward_raw_eval(self, x: torch.Tensor) -> tuple:
         feats = self.body.forward_levels(x, self.out_indices)
         outs = []
         for idx, f in zip(self.out_indices, feats):
@@ -74,7 +82,6 @@ class FasterViTBackbone(nn.Module):
             outs.append(out)
         return tuple(outs)
 
-    @torch.no_grad()
     def forward(self, tensors: torch.Tensor, mask: torch.Tensor | None = None) -> dict:
         """fastervit.py:829-846 without the NestedTensor wrapper type: {idx: (features, mask resized to the level)}."""
         outs = self.forward_raw(tensors)

@@ -868,7 +868,7 @@ class Engine:
             ptrs.append(t.data_ptr())
         return tuple(ptrs)
 
-    def _plan(self, x: torch.Tensor) -> Plan:
+    def _plan(self, x: torch.Tensor, spec: dict | None = None) -> Plan:
         if not x.is_cuda:
             raise L.FvitError("FasterViT (fastervit_b200) runs on CUDA only: move the model and input to a "
                               "CUDA device (`.cuda()`); there is no CPU / PyTorch fallback path")
@@ -886,23 +886,66 @@ class Engine:
             self._prepped.clear()
             self._ptr_sig = sig
         key = (tuple(x.shape), training, x.device.index)
+        norm_sig = ()
+        if spec is not None:
+            # dense train plans: one per (requested outputs, norms present, frozen prefix) besides the input shape
+            key += (spec["kind"], tuple((i, None if bn is None else id(bn)) for i, bn in spec.get("outs", ())),
+                    spec.get("frozen", -1))
+            # the level norms are not the model's own tensors (the backbone's norm{i}): the plan reads them through raw
+            # pointers too, so a reallocation of one of them (`bn.weight.data = ...`) rebuilds it
+            norm_sig = self._norm_sig(spec)
         plan = self.plans.get(key)
+        if plan is not None and getattr(plan, "_norm_sig", ()) != norm_sig:
+            del self.plans[key]
+            plan = None
         if plan is None:
             with torch.cuda.device(x.device):
                 if training:
                     from .engine_train import TrainPlan
-                    plan = TrainPlan(self.model, x.shape[0], x.shape[2], x.shape[3], x.device)
+                    plan = TrainPlan(self.model, x.shape[0], x.shape[2], x.shape[3], x.device, spec=spec)
                 else:
                     plan = Plan(self.model, x.shape[0], x.shape[2], x.shape[3], training, x.device)
+            plan._norm_sig = norm_sig
             self.plans[key] = plan
         return plan
 
+    @staticmethod
+    def _norm_sig(spec: dict) -> tuple:
+        """pointer signature of the level norms of a dense spec (fp32, dense, like the model's own tensors)"""
+        ptrs = []
+        for i, bn in spec.get("outs", ()):
+            if bn is None:
+                continue
+            for name in ("weight", "bias", "running_mean", "running_var"):
+                t = getattr(bn, name)
+                if t is None:
+                    continue
+                if t.dtype != torch.float32 or not t.is_contiguous():
+                    raise L.FvitError(f"the norm of level {i}: {name} must be a dense float32 tensor")
+                ptrs.append(t.data_ptr())
+        return tuple(ptrs)
+
+    def _dense_train(self, x: torch.Tensor, spec: dict) -> tuple:
+        """Train-mode forward of a pooled / levels plan: an autograd node whose backward runs the plan's backward
+        launch list from the output gradients (engine_train._DenseFunction)."""
+        plan = self._plan(x, spec)
+        from .engine_train import _DenseFunction
+        with torch.cuda.device(x.device):
+            if torch.is_grad_enabled() and any(p.requires_grad for p in plan.params):
+                return _DenseFunction.apply(plan, x, *plan.params)
+            plan.run_forward(x)
+            return tuple(o.clone() for o in plan.outputs)
+
     def forward(self, x: torch.Tensor, features_only: bool = False) -> torch.Tensor:
+        if self.model.training:
+            if features_only:
+                # forward_features under .train(): the final norm with batch statistics (fv.py:949-953)
+                return self._dense_train(x, dict(kind="levels", outs=((len(self.model.levels) - 1, self.model.norm),)))[0]
+            if not isinstance(self.model.head, nn.Linear):
+                # num_classes = 0: the pooled features (fv.py:955-958)
+                return self._dense_train(x, dict(kind="pooled"))[0]
         plan = self._plan(x)
         if plan.training:
-            if features_only:
-                raise L.FvitError("forward_features is an inference helper (call model.eval()); the autograd "
-                                  "training path is forward()")
             from .engine_train import _FasterViTFunction
             with torch.cuda.device(x.device):
                 if torch.is_grad_enabled() and any(p.requires_grad for p in plan.params):
@@ -931,12 +974,17 @@ class Engine:
             return plan.pooled[:, :self.model.num_features].float()
         return plan.logits.clone()
 
-    def forward_levels(self, x: torch.Tensor, out_indices: tuple) -> tuple:
-        """Eval forward that also returns each requested level's output before its Downsample as an NCHW fp32 map
-        (the launch list is run piecewise up to the marks where those activations are live)."""
+    def forward_levels(self, x: torch.Tensor, out_indices: tuple, norms=None, frozen_stages: int = -1) -> tuple:
+        """Each requested level's output before its Downsample as an NCHW fp32 map. Eval: the inference launch list is
+        run piecewise up to the marks where those activations are live (`norms` / `frozen_stages` are not used there).
+        Train: a levels-mode train plan, differentiable; `norms` = one BatchNorm2d (or None) per index applied with
+        batch statistics, `frozen_stages` = the backbone's frozen prefix (fastervit.py:801-812)."""
+        if self.model.training:
+            norms = tuple(norms) if norms is not None else (None,) * len(out_indices)
+            if len(norms) != len(out_indices) or not out_indices:
+                raise L.FvitError("forward_levels: give one norm (or None) per requested level, and at least one level")
+            return self._dense_train(x, dict(kind="levels", outs=tuple(zip(out_indices, norms)), frozen=int(frozen_stages)))
         plan = self._plan(x)
-        if plan.training:
-            raise L.FvitError("forward_levels is an inference helper (call model.eval())")
         with torch.cuda.device(x.device):
             wk = plan.weights_key()
             if self._prepped.get(id(plan)) != wk:

@@ -34,22 +34,60 @@ def _sm_count() -> int:
 
 
 class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
-    def __init__(self, model, B: int, H: int, W: int, device):
+    """Train-mode forward + backward launch lists. `spec` selects what the forward returns and the backward starts from:
+    None = the logits (classification step, fv.py:949-965); {"kind": "pooled"} = the pooled features of a
+    num_classes = 0 model (fv.py:955-958); {"kind": "levels", "outs": ((level, BatchNorm2d or None), ...),
+    "frozen": frozen_stages} = NCHW level outputs taken before each level's Downsample, each optionally through a
+    batch-statistics BatchNorm2d (forward_levels, forward_features, FasterViTBackbone; the backbone's frozen prefix,
+    downstream/.../dino/fastervit.py:801-812, runs its BatchNorms on running statistics and gets no backward)."""
+
+    def __init__(self, model, B: int, H: int, W: int, device, spec: dict | None = None):
         self.bwd_ops: list[tuple] = []
         self.fwd_zero: list[torch.Tensor] = []   # accumulators zeroed before every forward (BN statistics)
         self.saved_levels: list[dict] = []
+        self.spec = spec
+        self.kind = None if spec is None else spec["kind"]
+        nlev = len(model.levels)
+        outs = tuple(spec.get("outs", ())) if spec is not None else ()
+        for i, bn in outs:
+            if not 0 <= i < nlev:
+                raise L.FvitError(f"out index {i} is not a level of this model (0 .. {nlev - 1})")
+            if bn is not None and (not isinstance(bn, torch.nn.BatchNorm2d) or bn.weight is None
+                                   or bn.running_mean is None or bn.momentum is None):
+                raise L.FvitError("level norms must be affine BatchNorm2d modules with running statistics and a momentum")
+        self.stop_level = max(i for i, _ in outs) if self.kind == "levels" else nlev - 1
+        fs = int(spec.get("frozen", -1)) if spec is not None else -1
+        self.stem_frozen = fs >= 0                       # fastervit.py:801-812
+        self.n_frozen_lv = fs - 1 if fs >= 2 else 0      # levels[0 .. fs-2]
+        frozen_mods = ([model.patch_embed] if self.stem_frozen else []) + [model.levels[i] for i in range(self.n_frozen_lv)]
+        self._frozen_bn = {id(b) for fm in frozen_mods for b in fm.modules() if isinstance(b, torch.nn.BatchNorm2d)}
+        self._frozen_params = {id(p) for fm in frozen_mods for p in fm.parameters()}
         super().__init__(model, B, H, W, True, device)
 
     # ------------------------------------------------------------------------------ infrastructure
     def _setup_train(self) -> None:
         m, nb = self.model, self.bufs
         self.params = [p for p in m.parameters()]
+        n_model = len(self.params)
+        # level norms that are not part of the model (the backbone's norm{i}) get flat-buffer slices after the model's,
+        # so that the data-parallel buckets reduce them too
+        known = {id(p) for p in self.params}
+        for _, bn in (self.spec or {}).get("outs", ()):
+            for p in (() if bn is None else (bn.weight, bn.bias)):
+                if id(p) not in known:
+                    known.add(id(p))
+                    self.params.append(p)
         offs, n = {}, 0
-        for p in self.params:
+        for k, p in enumerate(self.params):
+            if k == n_model:
+                self._n_model_flat = n         # end of the model's own slices
             offs[id(p)] = n
             n += _ru(p.numel(), 64)            # 256-byte aligned slices
+        if n_model == len(self.params):
+            self._n_model_flat = n
         self.gflat = nb.new("grad.flat", (n,), torch.float32)
         self._goff = offs
+        self._on_path = self._params_on_path()
         self.scratch_n = 0
         self._scratch_req: list[tuple[str, int]] = []
         self._bwd_side: set[int] = set()     # backward launches that run as a side branch (engine_train_levels.py)
@@ -62,6 +100,49 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
     def G(self, p: torch.Tensor) -> int:
         """device pointer of the flat-buffer gradient slice of parameter p"""
         return self.gflat.data_ptr() + 4 * self._goff[id(p)]
+
+    def _drop_rate(self, level: int) -> float:
+        """stochastic-depth rate of the next block (the schedule of fv.py:901, in block order). Blocks in the frozen
+        prefix run without it: the reference eval()s that prefix (fastervit.py:801-812), where DropPath is the
+        identity."""
+        rate = self.model.drop_path_rates[self._block_counter]
+        return 0.0 if level < self.n_frozen_lv else rate
+
+    def _params_on_path(self) -> set[int]:
+        """ids of the parameters the requested outputs depend on (the rest get no gradient: .grad stays None, as under
+        autograd). Levels mode: the stem and levels up to the highest requested one without its Downsample, the level
+        norms; not the frozen prefix, nor `norm` / `head` unless forward_features asked for `norm`."""
+        m = self.model
+        if self.kind != "levels":
+            return {id(p) for p in self.params}
+        on = set()
+        outs = self.spec["outs"]
+        for name, p in m.named_parameters():
+            if name.startswith("levels."):
+                li = int(name.split(".")[1])
+                if li < self.stop_level or (li == self.stop_level and not name.startswith(f"levels.{li}.downsample.")):
+                    on.add(id(p))
+            elif name.startswith("patch_embed."):
+                on.add(id(p))
+        for _, bn in outs:
+            if bn is not None:
+                on.update((id(bn.weight), id(bn.bias)))
+        return on - self._frozen_params
+
+    def grad_views_on_path(self) -> list:
+        """grad_views() with None for the parameters off the path of the requested outputs"""
+        return [g if id(p) in self._on_path else None for p, g in zip(self.params, self.grad_views())]
+
+    def _load_grads(self, grads) -> None:
+        """copy autograd's per-step output gradients into the static buffers the captured backward reads"""
+        if self.kind is None:
+            self._dlogits[:, :self._ncls].copy_(grads)
+        else:
+            for d, gr in zip(self.dense, grads):
+                if gr is None:      # autograd leaves the gradient of an unused output unset: zeros
+                    d["dy"].zero_()
+                else:
+                    d["dy"].copy_(gr)
 
     def grad_views(self) -> list[torch.Tensor]:
         """Per-parameter views of a *copy* of the flat gradient buffer: autograd's AccumulateGrad may keep
@@ -100,7 +181,7 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
             if isinstance(v, tuple) and len(v) == 2 and v[0] == "scr":
                 return self.scr.data_ptr() + 4 * v[1]
             return v
-        for lst in (self.ops, self.bwd_ops, self.prep_ops):
+        for lst in (self.ops, self.bwd_ops, self.prep_ops, self._scale_ops):
             for i, (fn, args, name) in enumerate(lst):
                 if isinstance(args, tuple):
                     lst[i] = (fn, tuple(res(a) for a in args), name)
@@ -113,6 +194,10 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         pro: list[tuple] = [("zero", self.gflat, "memset"), ("zero", self.scr, "memset")]
         for lv in self.lv:
             pro.append(("zero", lv["g"], "memset"))
+        if self.kind == "levels":
+            if self.feat["kind"] == "conv":   # the top level's gradient is accumulated into a cleared buffer
+                pro.append(("zero", self.feat["g"], "memset"))
+            pro.append(("zero", self._dense_acc, "memset"))
         self._bwd_prologue = pro
         self._branch_alpha_ops = []
         for slot, _ in self._branch_slots:
@@ -225,6 +310,7 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
     def _build(self) -> None:
         m, B = self.model, self.B
         self.bwd_flops: dict[int, float] = {}
+        self._scale_ops: list[tuple] = []   # levels mode: per-output statistics passes + the gradient-scale finalize
         self._setup_train()
         self._build_forward()
         self._build_backward()
@@ -255,22 +341,28 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
             self.run_captured("train forward", lambda: body(xs_))
         else:
             body(x)
-        return self.logits
+        return self.logits if self.kind is None else None   # (pooled / levels mode: self.outputs)
 
     def _bwd_start(self, dlogits: torch.Tensor | None) -> None:
         if dlogits is not None:
             self._dlogits[:, :self._ncls].copy_(dlogits)
         self.run_ops(self._bwd_prologue, None)
-        st = L.stream_ptr()
-        rc = self.lib.fvit_grad_scale_init(self._dlogits.data_ptr(), self._dlogits.numel(), 64.0, self.scal.data_ptr(), st)
-        if rc:
-            raise L.FvitError(self.lib.fvit_last_error().decode())
+        if self.kind == "levels":
+            # every requested output's statistics pass (with the max |dy| fused in), then S over all of them
+            self.run_ops(self._scale_ops, None)
+        else:
+            src = self._dlogits if self.kind is None else self._dpool_in
+            rc = self.lib.fvit_grad_scale_init(src.data_ptr(), src.numel(), 64.0, self.scal.data_ptr(), L.stream_ptr())
+            if rc:
+                raise L.FvitError(self.lib.fvit_last_error().decode())
         self.run_ops(self._branch_alpha_ops, None)
 
-    def run_backward(self, dlogits: torch.Tensor) -> None:
+    def run_backward(self, dlogits) -> None:
+        """backward launch list from the output gradient(s): the logits' (classification), the pooled features'
+        (pooled mode) or a list with one NCHW map gradient (or None) per requested level output"""
         grp = getattr(self.model, "_grad_allreduce", None)
         if grp is None:
-            self._dlogits[:, :self._ncls].copy_(dlogits)
+            self._load_grads(dlogits)
 
             def body():
                 self._bwd_start(None)
@@ -282,7 +374,7 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         # bucket points: every segment is one CUDA graph (like the single-GPU backward), the all-reduces in between are
         # ordinary NCCL calls -- collectives captured INTO a graph work too, but live graphs holding NCCL work make
         # destroy_process_group() hang at exit, so they stay outside.
-        self._dlogits[:, :self._ncls].copy_(dlogits)
+        self._load_grads(dlogits)
         red = GradBucketReducer(self.gflat, None if grp is True else grp)
         if getattr(self, "_ar_shadow", None) is None:
             self._ar_shadow = self._allreduce_shadow(red.world, red.measure_busbw())
@@ -475,3 +567,29 @@ class _FasterViTFunction(torch.autograd.Function):
                 "next forward, or use different plans / model copies for multi-view losses)")
         plan.run_backward(dlogits.contiguous().float())
         return (None, None, *plan.grad_views())
+
+
+class _DenseFunction(torch.autograd.Function):
+    """Autograd node of a pooled / levels-mode train plan: the outputs are copies of the plan's static output buffers;
+    backward copies their gradients into the plan's static gradient buffers and runs the backward launch list.
+    Parameters off the path of the outputs (and the frozen prefix) get None."""
+
+    @staticmethod
+    def forward(ctx, plan: TrainPlan, x: torch.Tensor, *params):
+        if x.requires_grad:
+            raise L.FvitError("the input requires grad, but the backward plan stops at the first convolution (no "
+                              "gradient w.r.t. the image is computed); detach the input")
+        ctx.plan = plan
+        plan.run_forward(x)
+        ctx.generation = plan.fwd_generation
+        return tuple(o.clone() for o in plan.outputs)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        plan: TrainPlan = ctx.plan
+        if ctx.generation != plan.fwd_generation:
+            raise L.FvitError(
+                "backward of a stale forward: another train-mode forward of the same input shape and outputs ran in "
+                "between and overwrote the saved activations of this one (call backward before the next forward)")
+        plan.run_backward([None if g is None else g.contiguous().float() for g in grads])
+        return (None, None, *plan.grad_views_on_path())

@@ -34,6 +34,13 @@ def _bn_train(self, name: str, bn: nn.BatchNorm2d, count: int, ls=None) -> dict:
 
 def _bn_finalize(self, d: dict, ls=None) -> None:
     bn = d["bn"]
+    if id(bn) in self._frozen_bn:
+        # frozen prefix (an eval()-ed module of the backbone, fastervit.py:801-812): running statistics, not updated
+        self._op(self.ops, "fvit_affine_fold", d["sc"].data_ptr(), d["sh"].data_ptr(), bn.num_features,
+                 bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+                 float(bn.eps), None, P(ls))
+        return
+    self._bn_batch_stats.append(bn)
     self._op(self.ops, "fvit_bn_finalize", d["st"][0].data_ptr(), d["st"][1].data_ptr(), float(d["count"]),
              bn.weight.data_ptr(), bn.bias.data_ptr(), float(bn.eps), float(bn.momentum), bn.running_mean.data_ptr(),
              bn.running_var.data_ptr(), P(ls), d["sc"].data_ptr(), d["sh"].data_ptr(), d["mu"].data_ptr(),
@@ -91,7 +98,7 @@ def _emit_conv_part_train(self) -> dict:
     Hc, Wc, Cc = H0, W0, dim
     prev = None
     for i, level in enumerate(m.levels):
-        if not level.conv:
+        if not level.conv or i > self.stop_level:
             break
         if i > 0:
             Hc, Wc, Cc = (Hc + 1) // 2, (Wc + 1) // 2, Cc * 2
@@ -99,6 +106,8 @@ def _emit_conv_part_train(self) -> dict:
             self._emit_downsample_train(i - 1, prev, lvl)
         self._emit_conv_blocks_train(i, level, lvl)
         lvl["kind"] = "conv"
+        lvl["level_index"] = i
+        self._level_of[i] = lvl
         self.conv_lv.append(lvl)
         prev = lvl
     self.conv_out = prev
@@ -134,7 +143,7 @@ def _emit_conv_blocks_train(self, i: int, level, lv: dict) -> None:
         if hasattr(blk, "gamma"):
             raise L.FvitError("layer_scale_conv is not supported by the training kernels (unused by every shipped config)")
         nm = f"l{i}.b{j}"
-        rate = self.model.drop_path_rates[self._block_counter]
+        rate = self._drop_rate(i)
         self._block_counter += 1
         rs = self._drop_buf(f"levels.{i}.blocks.{j}", rate, B, (lv["H"] + 2) * (lv["W"] + 2))
         w1, ld1 = self._pack_conv(nm + ".conv1", blk.conv1)
@@ -261,7 +270,9 @@ def _emit_downsample_bwd(self, ds: dict, src: dict, dst: dict) -> None:
              ("scal", 1), self.G(mod.norm.weight), self.G(mod.norm.bias))
 
 
-def _emit_conv_blocks_bwd(self, lv: dict) -> None:
+def _emit_conv_blocks_bwd(self, lv: dict, input_grad: bool = True) -> None:
+    """input_grad=False: nothing below reads the gradient of the level's input (the frozen prefix ends here), so the
+    first block's conv1 data-gradient GEMM is not emitted"""
     ops = self.bwd_ops
     Cc, rows, ld, npix = lv["C"], lv["rows"], lv["ld"], lv["npix"]
     g = lv["g"].data_ptr()
@@ -293,6 +304,8 @@ def _emit_conv_blocks_bwd(self, lv: dict) -> None:
                  self.G(blk.norm1.weight), self.G(blk.norm1.bias), None)
         _conv_wgrad(self, dz=lv["dzA"].data_ptr(), lddz=ld, x=sv["xin"].data_ptr(), ldx=ld, x_rows=rows, rows=rows, cout=Cc,
                     cin=Cc, shifts=shifts, conv_weight=blk.conv1.weight, name="convA")
+        if sv is lv["blocks_sv"][0] and not input_grad:
+            continue
         # g += conv1 data gradient
         self._bgemm(a=lv["dzA"].data_ptr(), a_rows=rows, lda=ld, b=sv["wT1"].data_ptr(), b_rows=Cc, ldb=9 * _ru(Cc, 64),
                     m=rows, n=Cc, kc=Cc, taps=lv["taps"], row_map=interior, resid=g, ld_resid=Cc, out_f32=g, ld_o32=Cc,
@@ -304,9 +317,18 @@ def _emit_conv_part_bwd(self) -> None:
     m, B = self.model, self.B
     for idx in range(len(self.conv_lv) - 1, -1, -1):
         lv = self.conv_lv[idx]
-        _emit_conv_blocks_bwd(self, lv)
+        if idx < self.n_frozen_lv:    # frozen prefix: no dgrad / wgrad / BatchNorm backward below this point
+            return
+        if lv is self.feat:           # levels mode with a conv top level: its output gradient enters here
+            self._inject(idx)
+        _emit_conv_blocks_bwd(self, lv, input_grad=(idx - 1 >= self.n_frozen_lv) if idx > 0 else not self.stem_frozen)
         if idx > 0:
+            if idx - 1 < self.n_frozen_lv:
+                return
             _emit_downsample_bwd(self, lv["ds"], self.conv_lv[idx - 1], lv)
+            self._inject(idx - 1)
+    if self.stem_frozen:
+        return
     # PatchEmbed
     st, lv0 = self.stem_sv, self.conv_lv[0]
     pe = m.patch_embed.conv_down

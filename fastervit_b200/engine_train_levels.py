@@ -44,13 +44,17 @@ def _build_forward(self) -> None:
     self.drop_specs: list[dict] = []
     self._block_counter = 0
     self._bn_modules = [mod for mod in m.modules() if isinstance(mod, nn.BatchNorm2d)]
+    self._bn_batch_stats: list = []   # BatchNorms this forward normalises with batch statistics (_bn_finalize)
     self.lv: list[dict] = []          # per-level geometry/buffers (+ "sv": saved activations)
     self.ds: list[dict] = []          # per-downsample saved state
+    self._level_of: dict[int, dict] = {}
     prev = self._emit_conv_part_train()
     Hc, Wc, Cc = prev["H"], prev["W"], prev["C"]
     for i, level in enumerate(m.levels):
         if level.conv:
             continue
+        if i > self.stop_level:   # levels mode: the forward ends at the highest requested level
+            break
         Hc, Wc, Cc = (Hc + 1) // 2, (Wc + 1) // 2, Cc * 2
         tl = self._token_level_buffers(i, level, Cc, Hc, Wc)
         # gradient buffer mirroring xs, plus one guaranteed-zero row at the end
@@ -62,10 +66,96 @@ def _build_forward(self) -> None:
         self._emit_downsample_train(i - 1, prev, tl)
         self._emit_token_level_train(i, level, tl)
         tl["kind"] = "tok"
+        self._level_of[i] = tl
         self.lv.append(tl)
         prev = tl
     self.feat = prev
-    self._emit_head_train(prev)
+    if self.kind == "levels":
+        self._emit_dense_outputs()
+        # num_batches_tracked counts the BatchNorms that ran on batch statistics (not the frozen prefix's, not the
+        # levels above the last requested one)
+        self._bn_modules = self._bn_batch_stats
+    else:
+        self._emit_head_train(prev)
+
+
+def _level_rows(lv: dict) -> tuple:
+    """(fp32 activation, row map of the B*H*W pixels) of a level's output: the zero-bordered conv map or the
+    window-major token buffer through its crop map (any-res window padding and carrier rows excluded)"""
+    if lv["kind"] == "conv":
+        return lv["x32"], lv["pix"]
+    return lv["xs"], lv["crop_map"]
+
+
+def _const_vec(self, value: float, n: int) -> torch.Tensor:
+    cache = self.__dict__.setdefault("_const_vecs", {})
+    if (value, n) not in cache:
+        cache[(value, n)] = self.bufs.new(f"const.{value}.{n}", (n,), torch.float32).fill_(value)
+    return cache[(value, n)]
+
+
+def _emit_dense_outputs(self) -> None:
+    """Levels mode forward tail: every requested level output (x before its Downsample, live in the level's buffer
+    until the plan's next forward: the backward never writes it) as an NCHW fp32 map in a static buffer, through its
+    BatchNorm2d with batch statistics (fvit_colstats_f32 -> fvit_bn_finalize, which also updates the running
+    statistics -> fvit_feature_map_fwd), or raw."""
+    B, nb = self.B, self.bufs
+    self.dense, self.outputs = [], []
+    tot = 1
+    for k, (i, bn) in enumerate(self.spec["outs"]):
+        lv = self._level_of[i]
+        x, rows = _level_rows(lv)
+        C, H, W = lv["C"], lv["H"], lv["W"]
+        T = H * W
+        out = nb.new(f"dense.out{k}", (B, C, H, W), torch.float32)
+        d = dict(level=i, lv=lv, x=x, rows=rows, C=C, T=T, bn=bn, out=out,
+                 dy=nb.new(f"dense.dy{k}", (B, C, H, W), torch.float32), acc=tot)
+        tot += 2 * _ru(C, 4)
+        if bn is not None:
+            if bn.num_features != C:
+                raise L.FvitError(f"the norm of level {i} has {bn.num_features} features, the level has {C} channels")
+            st = self._bn_train(f"dense.norm{k}", bn, B * T)
+            self._op(self.ops, "fvit_colstats_f32", x.data_ptr(), C, rows.data_ptr(), B * T, C, st["st"][0].data_ptr(),
+                     st["st"][1].data_ptr())
+            self._bn_finalize(st)
+            d.update(sc=st["sc"], sh=st["sh"], mu=st["mu"], rs=st["rs"])
+        else:
+            d.update(sc=_const_vec(self, 1.0, C), sh=_const_vec(self, 0.0, C), mu=None, rs=None)
+        self._op(self.ops, "fvit_feature_map_fwd", x.data_ptr(), C, rows.data_ptr(), B, T, C, d["sc"].data_ptr(),
+                 d["sh"].data_ptr(), out.data_ptr())
+        self.dense.append(d)
+        self.outputs.append(out)
+    # backward-side accumulators, cleared by every backward's prologue: [0] = max |dy| over all outputs, then per
+    # output the per-channel sums s1 = sum dy, s2 = sum dy * xhat of the statistics pass
+    self._dense_acc = nb.new("dense.acc", (tot,), torch.float32)
+    acc = self._dense_acc.data_ptr()
+    for d in self.dense:
+        d["s1"], d["s2"] = acc + 4 * d["acc"], acc + 4 * (d["acc"] + _ru(d["C"], 4))
+        bn = d["bn"]
+        self._op(self._scale_ops, "fvit_feature_map_bwd_stats", d["dy"].data_ptr(), d["x"].data_ptr(), d["C"],
+                 d["rows"].data_ptr(), B, d["T"], d["C"], P(d["mu"]), P(d["rs"]), d["s1"] if bn is not None else None,
+                 d["s2"] if bn is not None else None, acc)
+    self._op(self._scale_ops, "fvit_grad_scale_finalize", acc, 64.0, ("scal", 0))
+
+
+def _inject(self, level: int, g=True) -> None:
+    """Backward: add the gradients of the requested outputs of `level` to the level's residual-stream gradient g
+    (scaled by S). Called right after g is complete from above (the Downsample backward wrote it; for the top level:
+    the cleared buffer), before the level's own blocks read it. g=False: only the norm's weight / bias gradients
+    (an output inside the frozen prefix)."""
+    if self.kind != "levels":
+        return
+    for d in self.dense:
+        if d["level"] != level:
+            continue
+        bn, lv = d["bn"], d["lv"]
+        if bn is None and not g:
+            continue
+        self._op(self.bwd_ops, "fvit_feature_map_bwd", d["dy"].data_ptr(), d["x"].data_ptr(), d["C"],
+                 d["rows"].data_ptr(), self.B, d["T"], d["C"], P(d["mu"]), P(d["rs"]),
+                 bn.weight.data_ptr() if bn is not None else None, d["s1"] if bn is not None else None,
+                 d["s2"] if bn is not None else None, ("scal", 0), None, lv["g"].data_ptr() if g else None, d["C"],
+                 self.G(bn.weight) if bn is not None else None, self.G(bn.bias) if bn is not None else None)
 
 
 def _posemb_train(self, nm: str, tpe, n_side: int, Cc: int) -> dict:
@@ -213,7 +303,7 @@ def _emit_token_level_train(self, i: int, level, tl: dict) -> None:
     for j, blk in enumerate(level.blocks):
         nm = f"l{i}.b{j}"
         key = f"levels.{i}.blocks.{j}"
-        rate = self.model.drop_path_rates[self._block_counter]
+        rate = self._drop_rate(i)
         self._block_counter += 1
         sv: dict = dict(blk=blk)
         sv["rs_attn"] = self._drop_buf(key + ".attn", rate, nW, S)
@@ -324,6 +414,16 @@ def _emit_head_train(self, prev: dict) -> None:
     pooled = nb.new("head.pooled", (B, _ru(nf, 8)), torch.float16)
     self._op(self.ops, "fvit_pool_affine_fwd", prev["xs"].data_ptr(), nf, prev["crop_map"].data_ptr(), B, T, nf,
              sN.data_ptr(), tN.data_ptr(), pooled.data_ptr(), pooled.stride(0))
+    if self.kind == "pooled":
+        # num_classes = 0: the head is nn.Identity and the pooled features are the output (fv.py:955-958); the fp16
+        # classifier operand is widened to a fp32 output buffer (the eval plan returns the same fp16 values)
+        pooled32 = nb.new("head.pooled32", (B, nf), torch.float32)
+        self._op(self.ops, "fvit_affine_rows", pooled.data_ptr(), pooled.stride(0), None, B, nf,
+                 _const_vec(self, 1.0, nf).data_ptr(), _const_vec(self, 0.0, nf).data_ptr(), L.ACT_NONE, None, 0,
+                 pooled32.data_ptr(), nf, None, 0, None)
+        self.outputs = [pooled32]
+        self.head_sv = dict(pooled=pooled, mu=mu, rs=rs, T=T, nf=nf)
+        return
     hw16, ldh = self._pack_linear("head", m.head)
     self.logits = nb.new("logits", (B, m.num_classes), torch.float32)
     self._gemm(a=pooled.data_ptr(), a_rows=B, lda=pooled.stride(0), b=hw16.data_ptr(), ldb=ldh, m=B, n=m.num_classes,
@@ -346,7 +446,9 @@ def _build_backward(self) -> None:
     for name, p in m.named_parameters():
         if name.startswith("levels."):
             first.setdefault(int(name.split(".")[1]), self._goff[id(p)])
-    total = self.gflat.numel()
+    # (level norms outside the model have slices after [0, total): they are final once every injection ran, a bucket
+    # point of their own at the end)
+    total = self._n_model_flat
     group_floats = int(float(os.environ.get("FVIT_BUCKET_MB", "100")) * 1e6 / 4)
     self.grad_buckets = []
 
@@ -355,13 +457,23 @@ def _build_backward(self) -> None:
             self.grad_buckets.append((lo, hi))
             self.bwd_ops.append(("bucket", (lo, hi), "grad_bucket"))
 
-    self._emit_head_bwd(self.feat)
+    if self.kind is None:
+        self._emit_head_bwd(self.feat)
+    elif self.kind == "pooled":
+        self._emit_pooled_bwd(self.feat)
+    else:
+        for d in self.dense:      # outputs inside the frozen prefix: their norm's weight / bias gradients only
+            if d["level"] < self.n_frozen_lv:
+                self._inject(d["level"], g=False)
+        if self.feat["kind"] == "tok" and self.feat["level_index"] >= self.n_frozen_lv:
+            self._inject(self.feat["level_index"])   # (a conv top level: _emit_conv_part_bwd)
     toks = [lv for lv in self.lv]
-    n_conv = len(m.levels) - len(toks)
     hi = total
     for idx in range(len(toks) - 1, -1, -1):
         tl = toks[idx]
-        lo = first.get(n_conv + idx, hi)
+        if tl["level_index"] < self.n_frozen_lv:
+            break
+        lo = first.get(tl["level_index"], hi)
         # offsets of the level's blocks in the flat buffer (module order = offset order, contiguous)
         spans = []
         for blk in m.levels[tl["level_index"]].blocks:
@@ -382,9 +494,31 @@ def _build_backward(self) -> None:
             point(lo, hi)
         hi = lo
         src = toks[idx - 1] if idx > 0 else self.conv_out
+        if tl["level_index"] - 1 < self.n_frozen_lv:
+            break     # the Downsample in front of this level belongs to the frozen prefix: the backward ends here
         self._emit_downsample_bwd(tl["ds"], src, tl)
-    self._emit_conv_part_bwd()
+        self._inject(tl["level_index"] - 1)
+    else:
+        self._emit_conv_part_bwd()
     point(0, hi)
+    point(total, self.gflat.numel())
+
+
+def _emit_pooled_bwd(self, feat: dict) -> None:
+    """Backward of the pooled features of a num_classes = 0 model: BatchNorm (batch statistics) + average pool, from
+    the autograd gradient scaled by S on the device (fvit_vec_mul), as _emit_head_bwd does from the head GEMM."""
+    B, nb, nf = self.B, self.bufs, self.head_sv["nf"]
+    hs = self.head_sv
+    m = self.model
+    self._dpool_in = nb.new("grad.dpool_in", (B, nf), torch.float32)
+    self.dense = [dict(dy=self._dpool_in)]
+    dpool = nb.new("grad.dpool", (B, nf), torch.float32)
+    self._op(self.bwd_ops, "fvit_vec_mul", self._dpool_in.data_ptr(), 1, ("scal", 0), 0, dpool.data_ptr(), B * nf)
+    s12 = nb.new("grad.head_s12", (2, nf), torch.float32)
+    self._op(self.bwd_ops, "fvit_pool_bn_bwd", feat["xs"].data_ptr(), nf, feat["crop_map"].data_ptr(), B, hs["T"], nf,
+             hs["mu"].data_ptr(), hs["rs"].data_ptr(), m.norm.weight.data_ptr(), dpool.data_ptr(), nf,
+             s12[0].data_ptr(), s12[1].data_ptr(), ("scal", 1), feat["g"].data_ptr(), nf, self.G(m.norm.weight),
+             self.G(m.norm.bias))
 
 
 def _emit_head_bwd(self, feat: dict) -> None:
@@ -686,6 +820,9 @@ class TokenLevelEmitters:
     _emit_token_level_train = _emit_token_level_train
     _mlp_fwd_train = _mlp_fwd_train
     _emit_head_train = _emit_head_train
+    _emit_dense_outputs = _emit_dense_outputs
+    _inject = _inject
+    _emit_pooled_bwd = _emit_pooled_bwd
     _build_backward = _build_backward
     _emit_head_bwd = _emit_head_bwd
     _emit_attn_core_bwd = _emit_attn_core_bwd

@@ -133,6 +133,10 @@ _OP_SIGS: dict[str, list] = {
     "fvit_pool_affine_fwd": [_P, _L, _P, _I, _I, _I, _P, _P, _P, _L, _P],
     "fvit_feature_map_fwd": [_P, _L, _P, _I, _I, _I, _P, _P, _P, _P],
     "fvit_nchw_pool_f16": [_P, _I, _I, _I, _P, _L, _P],
+    # dense-prediction outputs in training (include/fvit.h "Backward of fvit_feature_map_fwd")
+    "fvit_feature_map_bwd_stats": [_P, _P, _L, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P],
+    "fvit_feature_map_bwd": [_P, _P, _L, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _L, _P, _P, _P],
+    "fvit_grad_scale_finalize": [_P, _F, _P, _P],
     # optimizer step (include/fvit.h "optimizer step on the flat gradient buffer")
     "fvit_optim_gather_f32": [_P, _I, _P, _P, _P, _P],
     "fvit_optim_sqnorm": [_P, _I, _P, _P, _P, _P],

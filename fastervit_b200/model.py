@@ -302,10 +302,14 @@ class FasterViT(nn.Module):
 
     def forward_levels(self, x, out_indices=(0, 1, 2, 3)):
         """Per-level feature maps [B, C_i, H_i, W_i] (each level's output before its Downsample), the `xo` a dense-
-        prediction backbone taps (downstream/object_detection/dino/models/dino/fastervit.py:686-709, 816-827)."""
+        prediction backbone taps (downstream/object_detection/dino/models/dino/fastervit.py:686-709, 816-827).
+        Under .train() the maps are differentiable (the forward stops after the highest requested level; parameters
+        above it, `norm` and `head` get no gradient)."""
         return self._get_engine().forward_levels(x, tuple(out_indices))
 
     def forward_features(self, x):
+        """The `norm`-ed last-level map [B, C, H, W] (fv.py:949-953); under .train() with batch statistics (running
+        statistics updated) and differentiable."""
         return self._get_engine().forward(x, features_only=True)
 
     def forward_head(self, x):

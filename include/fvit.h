@@ -273,6 +273,27 @@ int fvit_pool_affine_fwd(const float* xs, int64_t ldx, const int32_t* row_map, i
 int fvit_feature_map_fwd(const float* xs, int64_t ldx, const int32_t* row_map, int32_t B, int32_t T, int32_t C,
                          const float* scale, const float* shift, float* out_nchw, void* stream);
 
+/* Backward of fvit_feature_map_fwd with a batch-statistics BatchNorm2d folded in: autograd of the level norms
+ * (downstream/object_detection/dino/models/dino/fastervit.py:816-827 `norm_layer(xo)` under .train()) and of the
+ * final `norm` (faster_vit.py:953) in forward_features. dy is the NCHW fp32 gradient [B, C, T] of the map; xs / row_map
+ * address the token-major level activation as in the forward. Two passes:
+ * fvit_feature_map_bwd_stats: s1[c] += sum_{b,t} dy, s2[c] += sum dy * xhat (xhat = (xs[row][c] - mean[c]) * rstd[c]),
+ *   *amax = max(*amax, max |dy|) (fp32 bits compared as integers; zero it before the first output). mean == NULL is
+ *   the mode without a BatchNorm (raw forward_levels maps): only amax; xs, rstd, s1, s2 may be NULL.
+ * fvit_feature_map_bwd: g[row_map[b*T+t]][c] += S * dx with S = gs[0] and, BatchNorm mode, dx = w*rstd*(dy - s1/N -
+ *   xhat*s2/N) (N = B*T), else dx = dy; rows outside row_map are untouched. dw[c] += s2*(*scalar), dbeta[c] +=
+ *   s1*(*scalar) (BatchNorm mode, optional, scalar NULL = 1). g NULL: only dw / dbeta.
+ * fvit_grad_scale_finalize: gs = {S, 1/S}, S = 2^floor(log2(target / *amax)) (the fvit_grad_scale_init rule over the
+ *   maximum the stats passes of every requested output gathered). */
+int fvit_feature_map_bwd_stats(const float* dy, const float* xs, int64_t ldx, const int32_t* row_map, int32_t B,
+                               int32_t T, int32_t C, const float* mean, const float* rstd, float* s1, float* s2,
+                               float* amax, void* stream);
+int fvit_feature_map_bwd(const float* dy, const float* xs, int64_t ldx, const int32_t* row_map, int32_t B, int32_t T,
+                         int32_t C, const float* mean, const float* rstd, const float* w, const float* s1,
+                         const float* s2, const float* gs, const float* scalar, float* g, int64_t ldg, float* dw,
+                         float* dbeta, void* stream);
+int fvit_grad_scale_finalize(const float* amax, float target, float* gs, void* stream);
+
 /* forward_head (faster_vit.py:955-958): AdaptiveAvgPool2d(1) + flatten of an NCHW fp32 map into the fp16 operand
  * [B, ldo] of the classifier GEMM. */
 int fvit_nchw_pool_f16(const float* x, int32_t B, int32_t C, int32_t T, void* out16, int64_t ldo, void* stream);
