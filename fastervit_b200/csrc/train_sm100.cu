@@ -17,18 +17,24 @@ __device__ __forceinline__ float warp_sum_t(float v) {
 }
 
 // ---------------------------------------------------------------------------------- column statistics
-// sum[c] += sum_r x[rows[r]][c], sumsq[c] += sum_r x[..]^2 over a row list (fp32 input).
+// sum[c] += sum_r d, sumsq[c] += sum_r d^2 with d = x[rows[r]][c] - K[c] over a row list (fp32 input). K = 0, or
+// with `pivot` the column's first listed value (written to pivot[c]): one-pass fp32 moments about K lose
+// ~ 2^-24 * (mean - K)^2 / var of the variance per term, so a pivot inside the data keeps them exact whatever
+// per-channel offset the residual stream carries.
 // Block = 256 threads handles a slab of rows for 64 columns: threadIdx.x & 63 = column, >> 6 = row lane.
 __global__ void colstats_f32_kernel(const float* __restrict__ x, long long ldx, const int* __restrict__ rows,
-                                    int nrows, int C, float* __restrict__ sum, float* __restrict__ sumsq) {
+                                    int nrows, int C, float* __restrict__ sum, float* __restrict__ sumsq,
+                                    float* __restrict__ pivot) {
   __shared__ float red[2][4][64];
   const int c = blockIdx.y * 64 + (threadIdx.x & 63);
   const int rl = threadIdx.x >> 6;
   float s = 0.f, q = 0.f;
   if (c < C) {
+    const float k = pivot ? x[(rows ? (long long)rows[0] : 0LL) * ldx + c] : 0.f;
+    if (pivot && blockIdx.x == 0 && rl == 0) pivot[c] = k;
     for (int r = blockIdx.x * 4 + rl; r < nrows; r += gridDim.x * 4) {
       const long long row = rows ? rows[r] : r;
-      const float v = x[row * ldx + c];
+      const float v = x[row * ldx + c] - k;
       s += v;
       q += v * v;
     }
@@ -43,11 +49,14 @@ __global__ void colstats_f32_kernel(const float* __restrict__ x, long long ldx, 
   }
 }
 
-// BatchNorm2d training-mode finalize (fv.py:459-462, 490-493, 925 with module.training):
-//   mean = sum/n, var = sumsq/n - mean^2 (biased, used to normalise);
-//   running_mean = (1-m) running_mean + m mean ; running_var = (1-m) running_var + m var n/(n-1);
-//   scale = w * rsqrt(var+eps) [* ls] ; shift = (b - mean*scale_raw) [* ls]  -> y = x*scale + shift
-__global__ void bn_finalize_kernel(const float* __restrict__ sum, const float* __restrict__ sumsq, float count,
+// BatchNorm2d training-mode finalize (fv.py:459-462, 490-493, 925 with module.training), from moments of
+// d = x - K (K = pivot[c], or 0):
+//   md = sum/n, var = sumsq/n - md^2 (biased, used to normalise), batch mean = K + md;
+//   running_mean = (1-m) running_mean + m (K + md) ; running_var = (1-m) running_var + m var n/(n-1);
+//   mean = md if the normalised data is d itself (`shifted`), else K + md;
+//   scale = w * rsqrt(var+eps) [* ls] ; shift = (b - mean*scale_raw) [* ls]  -> y = data*scale + shift
+__global__ void bn_finalize_kernel(const float* __restrict__ sum, const float* __restrict__ sumsq,
+                                   const float* __restrict__ pivot, int shifted, float count,
                                    const float* __restrict__ w, const float* __restrict__ b, float eps,
                                    float momentum, float* __restrict__ running_mean,
                                    float* __restrict__ running_var, const float* __restrict__ ls,
@@ -55,12 +64,14 @@ __global__ void bn_finalize_kernel(const float* __restrict__ sum, const float* _
                                    float* __restrict__ mean_out, float* __restrict__ rstd_out, int C) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const float mean = sum[c] / count;
-  float var = sumsq[c] / count - mean * mean;
+  const float md = sum[c] / count;
+  float var = sumsq[c] / count - md * md;
   var = fmaxf(var, 0.f);
   const float rstd = rsqrtf(var + eps);
+  const float batch_mean = pivot ? pivot[c] + md : md;
+  const float mean = shifted ? md : batch_mean;
   if (running_mean) {
-    running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * mean;
+    running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * batch_mean;
     const float unbiased = count > 1.f ? var * count / (count - 1.f) : var;
     running_var[c] = (1.f - momentum) * running_var[c] + momentum * unbiased;
   }
@@ -75,6 +86,14 @@ __global__ void bn_finalize_kernel(const float* __restrict__ sum, const float* _
     mean_out[c] = mean;
     rstd_out[c] = rstd;
   }
+}
+
+// col_shift = bias - pivot (bias NULL = 0): the epilogue vector that centres a convolution GEMM's output and its
+// statistics on the BatchNorm's pivot; recomputed every step because the bias is a trained parameter.
+__global__ void bn_col_shift_kernel(const float* __restrict__ bias, const float* __restrict__ pivot, int C,
+                                    float* __restrict__ col_shift) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c < C) col_shift[c] = (bias ? bias[c] : 0.f) - pivot[c];
 }
 
 // y = act(x16[row]*scale + shift) * row_scale (+ resid32[row]) for the listed rows; writes fp32 and/or fp16.
@@ -1465,20 +1484,51 @@ int fvit_colstats_f32(const float* x, int64_t ldx, const int32_t* rows, int32_t 
                       float* sumsq, void* stream) {
   FVIT_CHECK(x && sum && sumsq && nrows > 0 && C > 0, "fvit_colstats_f32: bad arguments");
   dim3 grid((unsigned)grid_cap(((long long)nrows + 15) / 16, 1, 24), (unsigned)((C + 63) / 64));
-  colstats_f32_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, rows, nrows, C, sum, sumsq);
+  colstats_f32_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, rows, nrows, C, sum, sumsq, nullptr);
   return post_launch("colstats_f32_kernel");
+}
+
+int fvit_colstats_pivot_f32(const float* x, int64_t ldx, const int32_t* rows, int32_t nrows, int32_t C, float* pivot,
+                            float* sum, float* sumsq, void* stream) {
+  FVIT_CHECK(x && pivot && sum && sumsq && nrows > 0 && C > 0, "fvit_colstats_pivot_f32: bad arguments");
+  dim3 grid((unsigned)grid_cap(((long long)nrows + 15) / 16, 1, 24), (unsigned)((C + 63) / 64));
+  colstats_f32_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, rows, nrows, C, sum, sumsq, pivot);
+  return post_launch("colstats_f32_kernel");
+}
+
+static int bn_finalize_launch(const float* sum, const float* sumsq, const float* pivot, int32_t shifted, float count,
+                              const float* w, const float* b, float eps, float momentum, float* running_mean,
+                              float* running_var, const float* layer_scale, float* scale, float* shift, float* mean_out,
+                              float* rstd_out, int32_t C, void* stream) {
+  FVIT_CHECK(sum && sumsq && w && b && scale && shift && C > 0 && count > 0, "fvit_bn_finalize: bad arguments");
+  FVIT_CHECK((running_mean == nullptr) == (running_var == nullptr), "fvit_bn_finalize: running stats come in pairs");
+  FVIT_CHECK((mean_out == nullptr) == (rstd_out == nullptr), "fvit_bn_finalize: mean/rstd outputs come in pairs");
+  bn_finalize_kernel<<<ceil_div(C, 128), 128, 0, (cudaStream_t)stream>>>(
+      sum, sumsq, pivot, shifted, count, w, b, eps, momentum, running_mean, running_var, layer_scale, scale, shift,
+      mean_out, rstd_out, C);
+  return post_launch("bn_finalize_kernel");
 }
 
 int fvit_bn_finalize(const float* sum, const float* sumsq, float count, const float* w, const float* b, float eps,
                      float momentum, float* running_mean, float* running_var, const float* layer_scale,
                      float* scale, float* shift, float* mean_out, float* rstd_out, int32_t C, void* stream) {
-  FVIT_CHECK(sum && sumsq && w && b && scale && shift && C > 0 && count > 0, "fvit_bn_finalize: bad arguments");
-  FVIT_CHECK((running_mean == nullptr) == (running_var == nullptr), "fvit_bn_finalize: running stats come in pairs");
-  FVIT_CHECK((mean_out == nullptr) == (rstd_out == nullptr), "fvit_bn_finalize: mean/rstd outputs come in pairs");
-  bn_finalize_kernel<<<ceil_div(C, 128), 128, 0, (cudaStream_t)stream>>>(
-      sum, sumsq, count, w, b, eps, momentum, running_mean, running_var, layer_scale, scale, shift, mean_out,
-      rstd_out, C);
-  return post_launch("bn_finalize_kernel");
+  return bn_finalize_launch(sum, sumsq, nullptr, 0, count, w, b, eps, momentum, running_mean, running_var, layer_scale,
+                            scale, shift, mean_out, rstd_out, C, stream);
+}
+
+int fvit_bn_finalize_pivot(const float* sum, const float* sumsq, const float* pivot, int32_t shifted, float count,
+                           const float* w, const float* b, float eps, float momentum, float* running_mean,
+                           float* running_var, const float* layer_scale, float* scale, float* shift, float* mean_out,
+                           float* rstd_out, int32_t C, void* stream) {
+  FVIT_CHECK(pivot != nullptr, "fvit_bn_finalize_pivot: pivot is required");
+  return bn_finalize_launch(sum, sumsq, pivot, shifted, count, w, b, eps, momentum, running_mean, running_var,
+                            layer_scale, scale, shift, mean_out, rstd_out, C, stream);
+}
+
+int fvit_bn_col_shift(const float* bias, const float* pivot, int32_t C, float* col_shift, void* stream) {
+  FVIT_CHECK(pivot && col_shift && C > 0, "fvit_bn_col_shift: bad arguments");
+  bn_col_shift_kernel<<<ceil_div(C, 128), 128, 0, (cudaStream_t)stream>>>(bias, pivot, C, col_shift);
+  return post_launch("bn_col_shift_kernel");
 }
 
 int fvit_affine_rows(const void* x16, int64_t ldx, const int32_t* rows, int32_t nrows, int32_t C,

@@ -1,8 +1,9 @@
 """Train-mode forward and backward emitters for the convolutional part of FasterViT (PatchEmbed,
 ConvBlock levels, Downsample) — methods of TrainPlan.
 
-BatchNorm2d runs with batch statistics: the convolution GEMM stores the raw output (fp16) and per-channel
-sum / sum-of-squares, `fvit_bn_finalize` turns them into scale/shift (and updates the running statistics),
+BatchNorm2d runs with batch statistics: the convolution GEMM stores the raw output (fp16) centred on a per-channel
+pivot (the running mean when the plan was built) and its sum / sum-of-squares, `fvit_bn_finalize_pivot` turns them
+into scale/shift (and updates the running statistics),
 `fvit_affine_rows` normalises + activates (+ residual). The backward is the mirror image: `fvit_bn_bwd`,
 the data-gradient convolution as a 9-tap GEMM over the flipped-transposed packed weights, and the
 weight gradient as nine MN-major GEMMs (one per tap: dW_t = dZ^T X shifted by the tap) with split-K.
@@ -26,10 +27,29 @@ def _bn_train(self, name: str, bn: nn.BatchNorm2d, count: int, ls=None) -> dict:
     nb = self.bufs
     st = nb.new(name + ".stats", (2, C), torch.float32)
     self.fwd_zero.append(st)
+    # moments about `pivot` (include/fvit.h "Pivoted statistics"): fvit_colstats_pivot_f32 fills it, or _bn_col_shift
+    # (convolution GEMMs) sets it once; shifted: the normalised rows are the GEMM output centred on it
     d = dict(bn=bn, st=st, sc=nb.new(name + ".scale", (C,), torch.float32), sh=nb.new(name + ".shift", (C,), torch.float32),
              mu=nb.new(name + ".mean", (C,), torch.float32), rs=nb.new(name + ".rstd", (C,), torch.float32),
-             s12=nb.new(name + ".s12", (2, C), torch.float32), count=count)
+             s12=nb.new(name + ".s12", (2, C), torch.float32), pivot=nb.new(name + ".pivot", (C,), torch.float32),
+             shifted=False, count=count, name=name)
     return d
+
+
+def _bn_col_shift(self, d: dict, bias) -> int | None:
+    """col_shift of the convolution GEMM feeding BatchNorm d. The GEMM writes and sums conv + bias - K with K the
+    running mean when the plan is built (a pretrained or fine-tuned model: within a few std of the batch mean; 0 for
+    a fresh one, which is the plain one-pass sum). K stays fixed for the plan's life, so steps on the same input
+    round the same way. The frozen prefix normalises with running statistics and keeps the plain bias."""
+    bn = d["bn"]
+    if id(bn) in self._frozen_bn:
+        return P(bias)
+    with torch.no_grad():
+        d["pivot"].copy_(bn.running_mean.to(d["pivot"].device))
+    cs = self.bufs.new(d["name"] + ".col_shift", (bn.num_features,), torch.float32)
+    self._op(self.prep_ops, "fvit_bn_col_shift", P(bias), d["pivot"].data_ptr(), bn.num_features, cs.data_ptr())
+    d["shifted"] = True
+    return cs.data_ptr()
 
 
 def _bn_finalize(self, d: dict, ls=None) -> None:
@@ -41,10 +61,10 @@ def _bn_finalize(self, d: dict, ls=None) -> None:
                  float(bn.eps), None, P(ls))
         return
     self._bn_batch_stats.append(bn)
-    self._op(self.ops, "fvit_bn_finalize", d["st"][0].data_ptr(), d["st"][1].data_ptr(), float(d["count"]),
-             bn.weight.data_ptr(), bn.bias.data_ptr(), float(bn.eps), float(bn.momentum), bn.running_mean.data_ptr(),
-             bn.running_var.data_ptr(), P(ls), d["sc"].data_ptr(), d["sh"].data_ptr(), d["mu"].data_ptr(),
-             d["rs"].data_ptr(), bn.num_features)
+    self._op(self.ops, "fvit_bn_finalize_pivot", d["st"][0].data_ptr(), d["st"][1].data_ptr(), d["pivot"].data_ptr(),
+             int(d["shifted"]), float(d["count"]), bn.weight.data_ptr(), bn.bias.data_ptr(), float(bn.eps),
+             float(bn.momentum), bn.running_mean.data_ptr(), bn.running_var.data_ptr(), P(ls), d["sc"].data_ptr(),
+             d["sh"].data_ptr(), d["mu"].data_ptr(), d["rs"].data_ptr(), bn.num_features)
 
 
 def _emit_conv_part_train(self) -> dict:
@@ -72,7 +92,8 @@ def _emit_conv_part_train(self) -> dict:
     planes = nb.new("stem.planes", (4 * pl_rows, ld_in), torch.float16)
     bn1 = _bn_train(self, "stem.bn1", pe[1], npix1)
     self._gemm(a=col16.data_ptr(), a_rows=npix1, lda=self.STEM_LD, b=w1.data_ptr(), ldb=self.STEM_LD, m=npix1, n=in_dim,
-               kc=32, row_map=stem_map.data_ptr(), out_f16=raw1.data_ptr(), ld_o16=ld_in, col_sum=bn1["st"][0].data_ptr(),
+               kc=32, col_shift=_bn_col_shift(self, bn1, None), row_map=stem_map.data_ptr(), out_f16=raw1.data_ptr(),
+               ld_o16=ld_in, col_sum=bn1["st"][0].data_ptr(),
                col_sumsq=bn1["st"][1].data_ptr())
     self.op_flops[len(self.ops) - 1] = 2.0 * npix1 * in_dim * 27
     _bn_finalize(self, bn1)
@@ -85,7 +106,8 @@ def _emit_conv_part_train(self) -> dict:
     bn2 = _bn_train(self, "stem.bn2", pe[4], B * H0 * W0)
     to_l0 = self._plane_to_padded_map("stem.to_l0", B, H0, W0)
     self._gemm(a=planes.data_ptr(), a_rows=pl_rows, lda=ld_in, a_planes=4, a_plane_stride=pl_rows * ld_in, b=w2.data_ptr(),
-               ldb=ldw2, m=pl_rows, n=dim, kc=in_dim, taps=self._s2_taps(W0), m_alg=B * H0 * W0, row_map=to_l0.data_ptr(),
+               ldb=ldw2, m=pl_rows, n=dim, kc=in_dim, taps=self._s2_taps(W0), m_alg=B * H0 * W0,
+               col_shift=_bn_col_shift(self, bn2, None), row_map=to_l0.data_ptr(),
                out_f16=raw2.data_ptr(), ld_o16=lvl["ld"], col_sum=bn2["st"][0].data_ptr(), col_sumsq=bn2["st"][1].data_ptr())
     _bn_finalize(self, bn2)
     self._op(self.ops, "fvit_affine_rows", raw2.data_ptr(), lvl["ld"], lvl["pix"].data_ptr(), B * H0 * W0, dim,
@@ -155,13 +177,13 @@ def _emit_conv_blocks_train(self, i: int, level, lv: dict) -> None:
         bnB = _bn_train(self, nm + ".bn2", blk.norm2, npix)
         xin, xout = lv["x16s"][j], lv["x16s"][j + 1]
         self._gemm(a=xin.data_ptr(), a_rows=rows, lda=ld, b=w1.data_ptr(), ldb=ld1, m=rows, n=Cc, kc=Cc, taps=taps,
-                   m_alg=npix, col_shift=blk.conv1.bias.data_ptr(), row_map=lv["interior"].data_ptr(),
+                   m_alg=npix, col_shift=_bn_col_shift(self, bnA, blk.conv1.bias), row_map=lv["interior"].data_ptr(),
                    out_f16=rawA.data_ptr(), ld_o16=ld, col_sum=bnA["st"][0].data_ptr(), col_sumsq=bnA["st"][1].data_ptr())
         _bn_finalize(self, bnA)
         self._op(self.ops, "fvit_affine_rows", rawA.data_ptr(), ld, lv["pix"].data_ptr(), npix, Cc, bnA["sc"].data_ptr(),
                  bnA["sh"].data_ptr(), L.ACT_GELU, None, 0, None, 0, h16.data_ptr(), ld, None)
         self._gemm(a=h16.data_ptr(), a_rows=rows, lda=ld, b=w2.data_ptr(), ldb=ld2, m=rows, n=Cc, kc=Cc, taps=taps,
-                   m_alg=npix, col_shift=blk.conv2.bias.data_ptr(), row_map=lv["interior"].data_ptr(),
+                   m_alg=npix, col_shift=_bn_col_shift(self, bnB, blk.conv2.bias), row_map=lv["interior"].data_ptr(),
                    out_f16=rawB.data_ptr(), ld_o16=ld, col_sum=bnB["st"][0].data_ptr(), col_sumsq=bnB["st"][1].data_ptr())
         _bn_finalize(self, bnB)
         self._op(self.ops, "fvit_affine_rows", rawB.data_ptr(), ld, lv["pix"].data_ptr(), npix, Cc, bnB["sc"].data_ptr(),

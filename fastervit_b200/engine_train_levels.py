@@ -97,7 +97,7 @@ def _const_vec(self, value: float, n: int) -> torch.Tensor:
 def _emit_dense_outputs(self) -> None:
     """Levels mode forward tail: every requested level output (x before its Downsample, live in the level's buffer
     until the plan's next forward: the backward never writes it) as an NCHW fp32 map in a static buffer, through its
-    BatchNorm2d with batch statistics (fvit_colstats_f32 -> fvit_bn_finalize, which also updates the running
+    BatchNorm2d with batch statistics (fvit_colstats_pivot_f32 -> fvit_bn_finalize_pivot, which also updates the running
     statistics -> fvit_feature_map_fwd), or raw."""
     B, nb = self.B, self.bufs
     self.dense, self.outputs = [], []
@@ -115,8 +115,8 @@ def _emit_dense_outputs(self) -> None:
             if bn.num_features != C:
                 raise L.FvitError(f"the norm of level {i} has {bn.num_features} features, the level has {C} channels")
             st = self._bn_train(f"dense.norm{k}", bn, B * T)
-            self._op(self.ops, "fvit_colstats_f32", x.data_ptr(), C, rows.data_ptr(), B * T, C, st["st"][0].data_ptr(),
-                     st["st"][1].data_ptr())
+            self._op(self.ops, "fvit_colstats_pivot_f32", x.data_ptr(), C, rows.data_ptr(), B * T, C, st["pivot"].data_ptr(),
+                     st["st"][0].data_ptr(), st["st"][1].data_ptr())
             self._bn_finalize(st)
             d.update(sc=st["sc"], sh=st["sh"], mu=st["mu"], rs=st["rs"])
         else:
@@ -406,10 +406,13 @@ def _emit_head_train(self, prev: dict) -> None:
     tN = nb.new("norm.shift", (nf,), torch.float32)
     mu = nb.new("norm.mean", (nf,), torch.float32)
     rs = nb.new("norm.rstd", (nf,), torch.float32)
-    self._op(self.ops, "fvit_colstats_f32", prev["xs"].data_ptr(), nf, prev["crop_map"].data_ptr(), B * T, nf,
-             st[0].data_ptr(), st[1].data_ptr())
-    self._op(self.ops, "fvit_bn_finalize", st[0].data_ptr(), st[1].data_ptr(), float(B * T), m.norm.weight.data_ptr(),
-             m.norm.bias.data_ptr(), float(m.norm.eps), float(m.norm.momentum), m.norm.running_mean.data_ptr(),
+    pv = nb.new("norm.pivot", (nf,), torch.float32)
+    # the fp32 residual stream carries per-channel offsets: moments about each channel's first value
+    self._op(self.ops, "fvit_colstats_pivot_f32", prev["xs"].data_ptr(), nf, prev["crop_map"].data_ptr(), B * T, nf,
+             pv.data_ptr(), st[0].data_ptr(), st[1].data_ptr())
+    self._op(self.ops, "fvit_bn_finalize_pivot", st[0].data_ptr(), st[1].data_ptr(), pv.data_ptr(), 0, float(B * T),
+             m.norm.weight.data_ptr(), m.norm.bias.data_ptr(), float(m.norm.eps), float(m.norm.momentum),
+             m.norm.running_mean.data_ptr(),
              m.norm.running_var.data_ptr(), None, sN.data_ptr(), tN.data_ptr(), mu.data_ptr(), rs.data_ptr(), nf)
     pooled = nb.new("head.pooled", (B, _ru(nf, 8)), torch.float16)
     self._op(self.ops, "fvit_pool_affine_fwd", prev["xs"].data_ptr(), nf, prev["crop_map"].data_ptr(), B, T, nf,

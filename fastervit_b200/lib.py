@@ -106,6 +106,9 @@ _OP_SIGS: dict[str, list] = {
     "fvit_vec_headpad_f32": [_P, _P, _I, _I, _I, _P],
     "fvit_colstats_f32": [_P, _L, _P, _I, _I, _P, _P, _P],
     "fvit_bn_finalize": [_P, _P, _F, _P, _P, _F, _F, _P, _P, _P, _P, _P, _P, _P, _I, _P],
+    "fvit_colstats_pivot_f32": [_P, _L, _P, _I, _I, _P, _P, _P, _P],
+    "fvit_bn_col_shift": [_P, _P, _I, _P, _P],
+    "fvit_bn_finalize_pivot": [_P, _P, _P, _I, _F, _P, _P, _F, _F, _P, _P, _P, _P, _P, _P, _P, _I, _P],
     "fvit_affine_rows": [_P, _L, _P, _I, _I, _P, _P, _I, _P, _L, _P, _L, _P, _L, _P, _P],
     "fvit_grad_scale_init": [_P, _I, _F, _P, _P],
     "fvit_vec_mul": [_P, _I, _P, _I, _P, _I, _P],

@@ -239,6 +239,23 @@ int fvit_bn_finalize(const float* sum, const float* sumsq, float count, const fl
 int fvit_affine_rows(const void* x16, int64_t ldx, const int32_t* rows, int32_t nrows, int32_t C,
                      const float* scale, const float* shift, int32_t act, const float* resid, int64_t ldr,
                      float* out32, int64_t ldo32, void* out16, int64_t ldo16, const float* row_scale, void* stream);
+/* Pivoted statistics. One-pass fp32 sums of x and x^2 lose about 2^-24 * (mean/std)^2 of the variance per summed
+ * term, which is percents once a channel's offset is ~100 std. Summing d = x - K with K near the batch mean removes
+ * that loss:
+ * fvit_colstats_pivot_f32: as fvit_colstats_f32 over d = x - K with K[c] = x[rows[0]][c], written to pivot[c].
+ * fvit_bn_col_shift      : col_shift = (bias ? bias : 0) - pivot, the GEMM epilogue vector that makes a convolution
+ *   GEMM write and sum d = conv + bias - pivot.
+ * fvit_bn_finalize_pivot : fvit_bn_finalize from moments of d: batch mean = pivot + sum/n, var = sumsq/n - (sum/n)^2;
+ *   the running statistics use the batch mean. shifted != 0: the rows later normalised are d themselves (a GEMM
+ *   output whose col_shift subtracted the pivot), so shift and mean_out use sum/n; shifted == 0: they use the batch
+ *   mean. */
+int fvit_colstats_pivot_f32(const float* x, int64_t ldx, const int32_t* rows, int32_t nrows, int32_t C, float* pivot,
+                            float* sum, float* sumsq, void* stream);
+int fvit_bn_col_shift(const float* bias, const float* pivot, int32_t C, float* col_shift, void* stream);
+int fvit_bn_finalize_pivot(const float* sum, const float* sumsq, const float* pivot, int32_t shifted, float count,
+                           const float* w, const float* b, float eps, float momentum, float* running_mean,
+                           float* running_var, const float* layer_scale, float* scale, float* shift, float* mean_out,
+                           float* rstd_out, int32_t C, void* stream);
 
 /* ---- positional MLPs (cpb_mlp: Linear(2,512)+ReLU+Linear(512,D, no bias); fv.py:223-225, 322-324) --
  * out[p][d] for P coordinate pairs; hidden_out (optional, [P,512]) saves the ReLU output. */
@@ -302,7 +319,9 @@ int fvit_nchw_pool_f16(const float* x, int32_t B, int32_t C, int32_t T, void* ou
  * Activation gradients are fp16 tensors (or the fp32 residual-stream gradient) multiplied by a
  * power-of-two scale S kept in device memory, gs = {S, 1/S}; parameter gradients are fp32, un-scaled by
  * the `scalar` / alpha_ptr device scalars. Nothing synchronises with the host. */
-/* gs[0] = 2^floor(log2(target / max|x|)), gs[1] = 1/gs[0] (x = d loss / d logits, n elements). */
+/* gs[0] = 2^floor(log2(target / max|x|)), gs[1] = 1/gs[0] (x = d loss / d logits, n elements), clamped to
+ * [2^-24, 2^40]; S = 1 when the maximum is 0 or inf. NaN elements are skipped (the maximum is that of the others):
+ * a NaN loss gradient is left to the optimizer's non-finite check. */
 int fvit_grad_scale_init(const float* x, int32_t n, float target, float* gs, void* stream);
 /* out[i] = a[i*a_stride] * b[i*b_stride] (vectors of device scalars). */
 int fvit_vec_mul(const float* a, int32_t a_stride, const float* b, int32_t b_stride, float* out, int32_t n,
@@ -380,7 +399,8 @@ int fvit_pool_bn_bwd(const float* xs, int64_t ldx, const int32_t* rows, int32_t 
                      const float* mean, const float* rstd, const float* w, const float* dpool, int64_t lddp,
                      float* s1, float* s2, const float* scalar, float* g, int64_t ldg, float* dw, float* dbeta,
                      void* stream);
-/* dst[map[r]] += src[r] (fp32 rows; ct_dewindow backward, fv.py:96-101). */
+/* dst[map[r]] += src[r] (fp32 rows; ct_dewindow backward, fv.py:96-101); rows with map[r] < 0 are skipped. The add is
+ * a plain read-modify-write (no atomics): `map` must be injective on its non-negative entries. */
 int fvit_scatter_add_rows(const float* src, int64_t lds, float* dst, int64_t ldd, const int32_t* map, int32_t rows,
                           int32_t C, void* stream);
 /* BatchNorm2d (batch statistics) backward over row lists: dy = gin (fp32 or fp16) * colmul, masked by the
