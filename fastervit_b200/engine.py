@@ -859,7 +859,9 @@ class Engine:
         weights is irrelevant to these kernels; channels_last *inputs* are consumed through their strides).
         Returns the pointer signature the cached plans were built against."""
         ptrs = []
-        for name, t in list(self.model.named_parameters()) + list(self.model.named_buffers()):
+        named = list(self.model.named_parameters())
+        self._params = [p for _, p in named]   # (for Engine.forward: one module walk per call is enough)
+        for name, t in named + list(self.model.named_buffers()):
             if t.is_floating_point() and t.dtype != torch.float32:
                 raise L.FvitError(f"{name} is {t.dtype}: fastervit_b200 keeps parameters and buffers in float32 (the "
                                   "kernels form their own fp16 tensor-core operands); drop .half() / .bfloat16()")
@@ -890,7 +892,7 @@ class Engine:
         if spec is not None:
             # dense train plans: one per (requested outputs, norms present, frozen prefix) besides the input shape
             key += (spec["kind"], tuple((i, None if bn is None else id(bn)) for i, bn in spec.get("outs", ())),
-                    spec.get("frozen", -1))
+                    spec.get("frozen", -1), bool(spec.get("eval")))
             # the level norms are not the model's own tensors (the backbone's norm{i}): the plan reads them through raw
             # pointers too, so a reallocation of one of them (`bn.weight.data = ...`) rebuilds it
             norm_sig = self._norm_sig(spec)
@@ -900,7 +902,7 @@ class Engine:
             plan = None
         if plan is None:
             with torch.cuda.device(x.device):
-                if training:
+                if training or (spec is not None and spec.get("eval")):
                     from .engine_train import TrainPlan
                     plan = TrainPlan(self.model, x.shape[0], x.shape[2], x.shape[3], x.device, spec=spec)
                 else:
@@ -951,6 +953,32 @@ class Engine:
                 if torch.is_grad_enabled() and any(p.requires_grad for p in plan.params):
                     return _FasterViTFunction.apply(plan, x, *plan.params)
                 return plan.run_forward(x).clone()
+        params = self._params
+        if not features_only and torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params)):
+            # differentiable eval forward: the inference launch list as below, the backward recomputes it
+            # (engine_train._EvalGradFunction)
+            from .engine_train import _EvalGradFunction
+            return _EvalGradFunction.apply_fast(self, plan, x, *params)
+        return self._run_eval(plan, x, features_only)
+
+    def eval_grad_plan(self, x: torch.Tensor) -> Plan:
+        """The plan the backward of a differentiable eval forward runs (built at the first such backward): a TrainPlan
+        whose BatchNorms use their running statistics and whose backward also writes the image gradient."""
+        kind = None if isinstance(self.model.head, nn.Linear) else "pooled"
+        return self._plan(x, dict(kind=kind, eval=True))
+
+    def eval_grad_plans(self) -> list:
+        """the eval-grad plans built so far (one per input shape)"""
+        return [p for p in self.plans.values() if getattr(p, "eval_grad", False)]
+
+    def release_eval_grad_plans(self) -> None:
+        """Drop the eval-grad plans: each holds a training step's saved activations on the device for the model's
+        lifetime otherwise. The next eval-mode backward builds its plan again."""
+        for k in [k for k, p in self.plans.items() if getattr(p, "eval_grad", False)]:
+            del self.plans[k]
+
+    def _run_eval(self, plan: Plan, x: torch.Tensor, features_only: bool = False) -> torch.Tensor:
+        """the inference launch list (re-packing the fp16 weights first when they changed); returns a new tensor"""
         with torch.cuda.device(x.device):
             wk = plan.weights_key()
             if self._prepped.get(id(plan)) != wk:

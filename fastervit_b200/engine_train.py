@@ -39,7 +39,10 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
     num_classes = 0 model (fv.py:955-958); {"kind": "levels", "outs": ((level, BatchNorm2d or None), ...),
     "frozen": frozen_stages} = NCHW level outputs taken before each level's Downsample, each optionally through a
     batch-statistics BatchNorm2d (forward_levels, forward_features, FasterViTBackbone; the backbone's frozen prefix,
-    downstream/.../dino/fastervit.py:801-812, runs its BatchNorms on running statistics and gets no backward)."""
+    downstream/.../dino/fastervit.py:801-812, runs its BatchNorms on running statistics and gets no backward).
+    {"kind": None | "pooled", "eval": True} = the eval-grad plan, the backward of an eval()-mode forward: every BatchNorm
+    on its running statistics (not updated), no stochastic depth, and a backward that also yields the image gradient
+    `dx` (engine.Engine.forward)."""
 
     def __init__(self, model, B: int, H: int, W: int, device, spec: dict | None = None):
         self.bwd_ops: list[tuple] = []
@@ -47,6 +50,7 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         self.saved_levels: list[dict] = []
         self.spec = spec
         self.kind = None if spec is None else spec["kind"]
+        self.eval_grad = bool(spec is not None and spec.get("eval"))
         nlev = len(model.levels)
         outs = tuple(spec.get("outs", ())) if spec is not None else ()
         for i, bn in outs:
@@ -60,7 +64,8 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         self.stem_frozen = fs >= 0                       # fastervit.py:801-812
         self.n_frozen_lv = fs - 1 if fs >= 2 else 0      # levels[0 .. fs-2]
         frozen_mods = ([model.patch_embed] if self.stem_frozen else []) + [model.levels[i] for i in range(self.n_frozen_lv)]
-        self._frozen_bn = {id(b) for fm in frozen_mods for b in fm.modules() if isinstance(b, torch.nn.BatchNorm2d)}
+        self._frozen_bn = {id(b) for fm in ([model] if self.eval_grad else frozen_mods) for b in fm.modules()
+                           if isinstance(b, torch.nn.BatchNorm2d)}
         self._frozen_params = {id(p) for fm in frozen_mods for p in fm.parameters()}
         super().__init__(model, B, H, W, True, device)
 
@@ -106,7 +111,7 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         prefix run without it: the reference eval()s that prefix (fastervit.py:801-812), where DropPath is the
         identity."""
         rate = self.model.drop_path_rates[self._block_counter]
-        return 0.0 if level < self.n_frozen_lv else rate
+        return 0.0 if level < self.n_frozen_lv or self.eval_grad else rate
 
     def _params_on_path(self) -> set[int]:
         """ids of the parameters the requested outputs depend on (the rest get no gradient: .grad stays None, as under
@@ -323,7 +328,8 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         # saved activations / batch statistics / drop masks live in this plan's persistent buffers: a new forward
         # invalidates the state an earlier, not yet differentiated forward left behind (checked in backward)
         self.fwd_generation = getattr(self, "fwd_generation", 0) + 1
-        L.bump_weights_epoch()   # BatchNorm running statistics are updated through raw pointers
+        if not self.eval_grad:   # (the eval-grad forward writes no parameter or buffer)
+            L.bump_weights_epoch()   # BatchNorm running statistics are updated through raw pointers
         def body(xin):
             for t in self.fwd_zero:
                 t.zero_()
@@ -593,3 +599,56 @@ class _DenseFunction(torch.autograd.Function):
                 "between and overwrote the saved activations of this one (call backward before the next forward)")
         plan.run_backward([None if g is None else g.contiguous().float() for g in grads])
         return (None, None, *plan.grad_views_on_path())
+
+
+class _EvalGradFunction(torch.autograd.Function):
+    """Autograd node of a grad-enabled eval()-mode forward (logits, or the pooled features of a num_classes = 0 model).
+    forward runs the inference launch list unchanged -- bitwise the output of the same call under no_grad, at its speed
+    and memory -- and keeps x. backward recomputes: the eval-grad plan (Engine.eval_grad_plan) runs a saving forward on
+    x with every BatchNorm on its running statistics, then its backward from the output gradient, which yields the
+    parameter gradients and the image gradient. Each node recomputes on its own, so several forwards may feed one
+    backward; nothing is built until the first backward. First order only: the gradients come from raw kernel buffers
+    and carry no graph, so a backward through them (create_graph=True, then differentiating dx) raises."""
+
+    @classmethod
+    def apply_fast(cls, *args):
+        """Function.apply without its functorch dead-wrapper pass: that pass walks every argument in Python (about
+        150 us for a model's few hundred parameters, a third of the node's host cost). It only matters while functorch
+        transforms are active, and then the ordinary apply runs."""
+        if torch._C._are_functorch_transforms_active():
+            return cls.apply(*args)
+        return super(torch.autograd.Function, cls).apply(*args)   # (the C implementation underneath)
+
+    @staticmethod
+    def forward(ctx, engine, plan, x: torch.Tensor, *params):
+        ctx.engine, ctx.plan = engine, plan
+        out = engine._run_eval(plan, x)
+        ctx.weights_key = engine._prepped[id(plan)]    # (what _run_eval just checked the packed weights against)
+        ctx.save_for_backward(x)    # (autograd then rejects a backward after an in-place change of x)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gout):
+        (x,) = ctx.saved_tensors
+        engine, plan = ctx.engine, ctx.plan
+        m = engine.model
+        if plan.weights_key() != ctx.weights_key:
+            raise L.FvitError(
+                "backward of an eval-mode forward after a weight change: this model's parameters or buffers changed, "
+                "or any model's fused optimizer step, EMA update or train-mode forward ran in between (those write "
+                "through raw pointers and advance one library-wide epoch, so they count even for another model); the "
+                "recomputed forward might not be the one that ran: call backward before them")
+        if getattr(m, "_grad_allreduce", None) is not None:
+            raise L.FvitError("eval-mode gradients are not all-reduced across ranks: the gradient all-reduce "
+                              "(enable_grad_allreduce) only covers train-mode steps")
+        if any(getattr(mod, "deploy", False) for mod in m.modules()):
+            raise L.FvitError("eval-mode gradients need the relative-position-bias MLPs: a module was switched to "
+                              "deploy mode (switch_to_deploy caches their output), so they have no gradient path")
+        with torch.cuda.device(x.device):
+            gp = engine.eval_grad_plan(x)
+            gp.run_forward(x)
+            g = gout.contiguous().float()
+            gp.run_backward(g if gp.kind is None else [g])
+            dx = gp.dx.clone() if ctx.needs_input_grad[2] else None
+            return (None, None, dx, *gp.grad_views())

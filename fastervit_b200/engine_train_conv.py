@@ -22,17 +22,21 @@ def P(t):
 
 
 def _bn_train(self, name: str, bn: nn.BatchNorm2d, count: int, ls=None) -> dict:
-    """statistics accumulators + finalize launch; returns the saved vectors"""
+    """statistics accumulators + finalize launch; returns the saved vectors. A BatchNorm on running statistics (the
+    frozen prefix, an eval-mode plan) has no accumulators: its GEMM gets col_sum = col_sumsq = None."""
     C = bn.num_features
     nb = self.bufs
     st = nb.new(name + ".stats", (2, C), torch.float32)
-    self.fwd_zero.append(st)
+    frozen = id(bn) in self._frozen_bn
+    if not frozen:
+        self.fwd_zero.append(st)
     # moments about `pivot` (include/fvit.h "Pivoted statistics"): fvit_colstats_pivot_f32 fills it, or _bn_col_shift
     # (convolution GEMMs) sets it once; shifted: the normalised rows are the GEMM output centred on it
     d = dict(bn=bn, st=st, sc=nb.new(name + ".scale", (C,), torch.float32), sh=nb.new(name + ".shift", (C,), torch.float32),
              mu=nb.new(name + ".mean", (C,), torch.float32), rs=nb.new(name + ".rstd", (C,), torch.float32),
              s12=nb.new(name + ".s12", (2, C), torch.float32), pivot=nb.new(name + ".pivot", (C,), torch.float32),
-             shifted=False, count=count, name=name)
+             shifted=False, count=count, name=name,
+             col_sum=None if frozen else st[0].data_ptr(), col_sumsq=None if frozen else st[1].data_ptr())
     return d
 
 
@@ -93,8 +97,8 @@ def _emit_conv_part_train(self) -> dict:
     bn1 = _bn_train(self, "stem.bn1", pe[1], npix1)
     self._gemm(a=col16.data_ptr(), a_rows=npix1, lda=self.STEM_LD, b=w1.data_ptr(), ldb=self.STEM_LD, m=npix1, n=in_dim,
                kc=32, col_shift=_bn_col_shift(self, bn1, None), row_map=stem_map.data_ptr(), out_f16=raw1.data_ptr(),
-               ld_o16=ld_in, col_sum=bn1["st"][0].data_ptr(),
-               col_sumsq=bn1["st"][1].data_ptr())
+               ld_o16=ld_in, col_sum=bn1["col_sum"],
+               col_sumsq=bn1["col_sumsq"])
     self.op_flops[len(self.ops) - 1] = 2.0 * npix1 * in_dim * 27
     _bn_finalize(self, bn1)
     self._op(self.ops, "fvit_affine_rows", raw1.data_ptr(), ld_in, stem_map.data_ptr(), npix1, in_dim, bn1["sc"].data_ptr(),
@@ -108,7 +112,7 @@ def _emit_conv_part_train(self) -> dict:
     self._gemm(a=planes.data_ptr(), a_rows=pl_rows, lda=ld_in, a_planes=4, a_plane_stride=pl_rows * ld_in, b=w2.data_ptr(),
                ldb=ldw2, m=pl_rows, n=dim, kc=in_dim, taps=self._s2_taps(W0), m_alg=B * H0 * W0,
                col_shift=_bn_col_shift(self, bn2, None), row_map=to_l0.data_ptr(),
-               out_f16=raw2.data_ptr(), ld_o16=lvl["ld"], col_sum=bn2["st"][0].data_ptr(), col_sumsq=bn2["st"][1].data_ptr())
+               out_f16=raw2.data_ptr(), ld_o16=lvl["ld"], col_sum=bn2["col_sum"], col_sumsq=bn2["col_sumsq"])
     _bn_finalize(self, bn2)
     self._op(self.ops, "fvit_affine_rows", raw2.data_ptr(), lvl["ld"], lvl["pix"].data_ptr(), B * H0 * W0, dim,
              bn2["sc"].data_ptr(), bn2["sh"].data_ptr(), L.ACT_RELU, None, 0, lvl["x32"].data_ptr(), dim,
@@ -178,13 +182,13 @@ def _emit_conv_blocks_train(self, i: int, level, lv: dict) -> None:
         xin, xout = lv["x16s"][j], lv["x16s"][j + 1]
         self._gemm(a=xin.data_ptr(), a_rows=rows, lda=ld, b=w1.data_ptr(), ldb=ld1, m=rows, n=Cc, kc=Cc, taps=taps,
                    m_alg=npix, col_shift=_bn_col_shift(self, bnA, blk.conv1.bias), row_map=lv["interior"].data_ptr(),
-                   out_f16=rawA.data_ptr(), ld_o16=ld, col_sum=bnA["st"][0].data_ptr(), col_sumsq=bnA["st"][1].data_ptr())
+                   out_f16=rawA.data_ptr(), ld_o16=ld, col_sum=bnA["col_sum"], col_sumsq=bnA["col_sumsq"])
         _bn_finalize(self, bnA)
         self._op(self.ops, "fvit_affine_rows", rawA.data_ptr(), ld, lv["pix"].data_ptr(), npix, Cc, bnA["sc"].data_ptr(),
                  bnA["sh"].data_ptr(), L.ACT_GELU, None, 0, None, 0, h16.data_ptr(), ld, None)
         self._gemm(a=h16.data_ptr(), a_rows=rows, lda=ld, b=w2.data_ptr(), ldb=ld2, m=rows, n=Cc, kc=Cc, taps=taps,
                    m_alg=npix, col_shift=_bn_col_shift(self, bnB, blk.conv2.bias), row_map=lv["interior"].data_ptr(),
-                   out_f16=rawB.data_ptr(), ld_o16=ld, col_sum=bnB["st"][0].data_ptr(), col_sumsq=bnB["st"][1].data_ptr())
+                   out_f16=rawB.data_ptr(), ld_o16=ld, col_sum=bnB["col_sum"], col_sumsq=bnB["col_sumsq"])
         _bn_finalize(self, bnB)
         self._op(self.ops, "fvit_affine_rows", rawB.data_ptr(), ld, lv["pix"].data_ptr(), npix, Cc, bnB["sc"].data_ptr(),
                  bnB["sh"].data_ptr(), L.ACT_NONE, lv["x32"].data_ptr(), Cc, lv["x32"].data_ptr(), Cc, xout.data_ptr(), ld, rs)
@@ -257,9 +261,27 @@ def _emit_downsample_train(self, i: int, src: dict, dst: dict) -> None:
 
 
 # ====================================================================================== backward
-def _conv_wgrad(self, *, dz, lddz, x, ldx, x_rows, rows, cout, cin, shifts, conv_weight, name: str) -> None:
+def _bn_bwd(self, d: dict, gin, g_is_f16: int, ldg: int, g_rows, raw, ldr: int, r_rows, nrows: int, act: int, out,
+            ldo: int, o_rows, row_scale=None) -> None:
+    """BatchNorm2d backward of d (_bn_train) into fp16 rows `out`: batch statistics (fvit_bn_bwd), or the running
+    statistics of an eval-mode plan (fvit_bn_eval_bwd: no mean(dy) terms, one pass)"""
+    bn = d["bn"]
+    if self.eval_grad:
+        self._op(self.bwd_ops, "fvit_bn_eval_bwd", gin, g_is_f16, ldg, g_rows, raw, ldr, r_rows, nrows, bn.num_features,
+                 bn.running_mean.data_ptr(), bn.running_var.data_ptr(), float(bn.eps), bn.weight.data_ptr(),
+                 bn.bias.data_ptr(), act, None, ("scal", 1), out, ldo, o_rows, self.G(bn.weight), self.G(bn.bias))
+        return
+    self._op(self.bwd_ops, "fvit_bn_bwd", gin, g_is_f16, ldg, g_rows, raw, ldr, r_rows, nrows, bn.num_features,
+             d["mu"].data_ptr(), d["rs"].data_ptr(), bn.weight.data_ptr(), bn.bias.data_ptr(), act, None,
+             d["s12"][0].data_ptr(), d["s12"][1].data_ptr(), ("scal", 1), out, ldo, o_rows, self.G(bn.weight),
+             self.G(bn.bias), row_scale)
+
+
+def _conv_wgrad(self, *, dz, lddz, x, ldx, x_rows, rows, cout, cin, shifts, conv_weight, name: str, bias=None,
+                bias_rows=None, bias_nrows=0) -> None:
     """dW[co][ci][t] = sum_q dz[q][co] * x[q + shift_t][ci]: ONE MN-major split-K GEMM whose N dimension
-    enumerates (tap, ci) -- every dz tile is fetched once for the nine shifted views of x -- plus a repack."""
+    enumerates (tap, ci) -- every dz tile is fetched once for the nine shifted views of x -- plus a repack.
+    bias: db[co] += sum over the rows `bias_rows` of dz (scaled by 1/S), a column sum beside the GEMM."""
     nt = len(shifts)
     scr = ("scr", self._scratch(name + ".dWtaps", nt * cout * cin))
     sk = self._split_k(cout, cin, rows, nt)
@@ -268,6 +290,9 @@ def _conv_wgrad(self, *, dz, lddz, x, ldx, x_rows, rows, cout, cin, shifts, conv
                 n=cin, kc=rows, split_k=sk, alpha_ptr=("scal", 1), out_f32=scr, ld_o32=nt * cin,
                 flops=2.0 * rows * cout * cin * nt)
     self._op(self.bwd_ops, "fvit_unpack_conv_grad", scr, nt * cin, self.G(conv_weight), cout, cin)
+    if bias is not None:
+        self._op(self.bwd_ops, "fvit_colsum", dz, 1, lddz, bias_rows, None, 0, bias_nrows, cout, None, ("scal", 1),
+                 self.G(bias), None)
     self._side_from(n0, dz)   # (its own zeroed scratch slice in, a parameter gradient out: a leaf pair)
 
 
@@ -295,37 +320,36 @@ def _emit_downsample_bwd(self, ds: dict, src: dict, dst: dict) -> None:
 def _emit_conv_blocks_bwd(self, lv: dict, input_grad: bool = True) -> None:
     """input_grad=False: nothing below reads the gradient of the level's input (the frozen prefix ends here), so the
     first block's conv1 data-gradient GEMM is not emitted"""
-    ops = self.bwd_ops
     Cc, rows, ld, npix = lv["C"], lv["rows"], lv["ld"], lv["npix"]
     g = lv["g"].data_ptr()
     pix, interior = lv["pix"].data_ptr(), lv["interior"].data_ptr()
     shifts = [s for (s, _) in lv["taps"]]
-    inv = ("scal", 1)
     for sv in reversed(lv["blocks_sv"]):
         blk, bnA, bnB = sv["blk"], sv["bnA"], sv["bnB"]
         # x_out = x_in + BN2(conv2(h)); h = GELU(BN1(conv1(x_in)))
         self._before_write(lv["dzB"].data_ptr())
-        self._op(ops, "fvit_bn_bwd", g, 0, Cc, pix, sv["rawB"].data_ptr(), ld, pix, npix, Cc, bnB["mu"].data_ptr(),
-                 bnB["rs"].data_ptr(), blk.norm2.weight.data_ptr(), blk.norm2.bias.data_ptr(), L.ACT_NONE, None,
-                 bnB["s12"][0].data_ptr(), bnB["s12"][1].data_ptr(), inv, lv["dzB"].data_ptr(), ld, pix,
-                 self.G(blk.norm2.weight), self.G(blk.norm2.bias), sv["rs"])
+        _bn_bwd(self, bnB, g, 0, Cc, pix, sv["rawB"].data_ptr(), ld, pix, npix, L.ACT_NONE, lv["dzB"].data_ptr(), ld, pix,
+                sv["rs"])
         # h = GELU(BN1(rawA)) was kept by the forward; the pre-activation BN1(rawA) is re-derived inside the dgrad
-        # epilogue from rawA and the batch-statistics affine (aux_scale / aux_shift).
+        # epilogue from rawA and the BatchNorm affine (aux_scale / aux_shift).
         # conv biases sit in front of a batch-statistics BatchNorm: their gradient sum_rows(dz) is identically zero
-        # (BN backward removes the per-channel mean), so it is left at the zero the buffer was cleared to.
+        # (BN backward removes the per-channel mean), so it is left at the zero the buffer was cleared to. Running
+        # statistics (eval-mode plan) remove nothing: there it is a column sum of dz.
+        bias_b = blk.conv2.bias if self.eval_grad else None
+        bias_a = blk.conv1.bias if self.eval_grad else None
         _conv_wgrad(self, dz=lv["dzB"].data_ptr(), lddz=ld, x=sv["h16"].data_ptr(), ldx=ld, x_rows=rows, rows=rows, cout=Cc,
-                    cin=Cc, shifts=shifts, conv_weight=blk.conv2.weight, name="convB")
+                    cin=Cc, shifts=shifts, conv_weight=blk.conv2.weight, name="convB", bias=bias_b, bias_rows=pix,
+                    bias_nrows=npix)
         self._bgemm(a=lv["dzB"].data_ptr(), a_rows=rows, lda=ld, b=sv["wT2"].data_ptr(), b_rows=Cc, ldb=9 * _ru(Cc, 64),
                     m=rows, n=Cc, kc=Cc, taps=lv["taps"], act=L.ACT_GELU_BWD, aux=sv["rawA"].data_ptr(), ld_aux=ld,
                     aux_scale=bnA["sc"].data_ptr(), aux_shift=bnA["sh"].data_ptr(),
                     row_map=interior, out_f16=lv["dyA"].data_ptr(), ld_o16=ld, flops=2.0 * npix * Cc * Cc * 9)
         self._before_write(lv["dzA"].data_ptr())
-        self._op(ops, "fvit_bn_bwd", lv["dyA"].data_ptr(), 1, ld, pix, sv["rawA"].data_ptr(), ld, pix, npix, Cc,
-                 bnA["mu"].data_ptr(), bnA["rs"].data_ptr(), blk.norm1.weight.data_ptr(), blk.norm1.bias.data_ptr(), L.ACT_NONE,
-                 None, bnA["s12"][0].data_ptr(), bnA["s12"][1].data_ptr(), inv, lv["dzA"].data_ptr(), ld, pix,
-                 self.G(blk.norm1.weight), self.G(blk.norm1.bias), None)
+        _bn_bwd(self, bnA, lv["dyA"].data_ptr(), 1, ld, pix, sv["rawA"].data_ptr(), ld, pix, npix, L.ACT_NONE,
+                lv["dzA"].data_ptr(), ld, pix)
         _conv_wgrad(self, dz=lv["dzA"].data_ptr(), lddz=ld, x=sv["xin"].data_ptr(), ldx=ld, x_rows=rows, rows=rows, cout=Cc,
-                    cin=Cc, shifts=shifts, conv_weight=blk.conv1.weight, name="convA")
+                    cin=Cc, shifts=shifts, conv_weight=blk.conv1.weight, name="convA", bias=bias_a, bias_rows=pix,
+                    bias_nrows=npix)
         if sv is lv["blocks_sv"][0] and not input_grad:
             continue
         # g += conv1 data gradient
@@ -362,10 +386,8 @@ def _emit_conv_part_bwd(self) -> None:
     q_of_pix = nb.i32("stem.q_of_pix", (bb * (H0 + 1) * (W0 + 1) + (aa + 1) * (W0 + 1) + cc + 1).reshape(-1))
     dY2 = nb.new("stem.dY2", (pl_rows, lv0["ld"]), torch.float16)
     bn2, bn1 = st["bn2"], st["bn1"]
-    self._op(ops, "fvit_bn_bwd", lv0["g"].data_ptr(), 0, dim, lv0["pix"].data_ptr(), st["raw2"].data_ptr(), lv0["ld"],
-             lv0["pix"].data_ptr(), B * H0 * W0, dim, bn2["mu"].data_ptr(), bn2["rs"].data_ptr(), pe[4].weight.data_ptr(),
-             pe[4].bias.data_ptr(), L.ACT_RELU, None, bn2["s12"][0].data_ptr(), bn2["s12"][1].data_ptr(), inv,
-             dY2.data_ptr(), lv0["ld"], q_of_pix.data_ptr(), self.G(pe[4].weight), self.G(pe[4].bias), None)
+    _bn_bwd(self, bn2, lv0["g"].data_ptr(), 0, dim, lv0["pix"].data_ptr(), st["raw2"].data_ptr(), lv0["ld"],
+            lv0["pix"].data_ptr(), B * H0 * W0, L.ACT_RELU, dY2.data_ptr(), lv0["ld"], q_of_pix.data_ptr())
     taps = self._s2_taps(W0)
     shifts = [p * pl_rows + s for (s, p) in taps]
     _conv_wgrad(self, dz=dY2.data_ptr(), lddz=lv0["ld"], x=st["planes"].data_ptr(), ldx=ld_in, x_rows=4 * pl_rows,
@@ -383,13 +405,16 @@ def _emit_conv_part_bwd(self) -> None:
                     out_f16=dplanes.data_ptr() + 2 * p * pl_rows * ld_in, ld_o16=ld_in,
                     flops=2.0 * B * H0 * W0 * in_dim * dim * len(tl_))
     dz1 = nb.new("stem.dz1", (npix1, ld_in), torch.float16)
-    self._op(ops, "fvit_bn_bwd", dplanes.data_ptr(), 1, ld_in, st["stem_map"].data_ptr(), st["raw1"].data_ptr(), ld_in,
-             st["stem_map"].data_ptr(), npix1, in_dim, bn1["mu"].data_ptr(), bn1["rs"].data_ptr(), pe[1].weight.data_ptr(),
-             pe[1].bias.data_ptr(), L.ACT_RELU, None, bn1["s12"][0].data_ptr(), bn1["s12"][1].data_ptr(), inv, dz1.data_ptr(),
-             ld_in, None, self.G(pe[1].weight), self.G(pe[1].bias), None)
+    _bn_bwd(self, bn1, dplanes.data_ptr(), 1, ld_in, st["stem_map"].data_ptr(), st["raw1"].data_ptr(), ld_in,
+            st["stem_map"].data_ptr(), npix1, L.ACT_RELU, dz1.data_ptr(), ld_in, None)
     self._bgemm(a=dz1.data_ptr(), a_rows=npix1, lda=ld_in, a_mn=True, b=st["col16"].data_ptr(), b_rows=npix1, ldb=self.STEM_LD,
                 b_mn=True, m=in_dim, n=27, kc=npix1, split_k=self._split_k(in_dim, 27, npix1), alpha_ptr=inv,
                 out_f32=self.G(pe[0].weight), ld_o32=27, flops=2.0 * npix1 * in_dim * 27)
+    if self.eval_grad:
+        # the image gradient (fp32 NCHW, like x): the backward of conv1, 3x3 / stride 2 / pad 1, as a gather
+        self.dx = nb.new("stem.dx", (B, m.cfg["in_chans"], self.H, self.W), torch.float32)
+        self._op(ops, "fvit_stem_conv_dgrad", dz1.data_ptr(), ld_in, B, self.H, self.W, pe[0].weight.data_ptr(), in_dim,
+                 inv, self.dx.data_ptr())
 
 
 class ConvPartEmitters:
@@ -401,6 +426,7 @@ class ConvPartEmitters:
     _conv_level_train_buffers = _conv_level_train_buffers
     _emit_conv_blocks_train = _emit_conv_blocks_train
     _emit_downsample_train = _emit_downsample_train
+    _bn_bwd = _bn_bwd
     _conv_wgrad = _conv_wgrad
     _emit_downsample_bwd = _emit_downsample_bwd
     _emit_conv_blocks_bwd = _emit_conv_blocks_bwd

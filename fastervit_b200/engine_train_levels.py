@@ -77,6 +77,8 @@ def _build_forward(self) -> None:
         self._bn_modules = self._bn_batch_stats
     else:
         self._emit_head_train(prev)
+        if self.eval_grad:
+            self._bn_modules = []     # (running statistics: num_batches_tracked stays)
 
 
 def _level_rows(lv: dict) -> tuple:
@@ -396,24 +398,31 @@ def _mlp_fwd_train(self, nm: str, mlp, gamma, rows: int, y16, p16, h16, stream_b
 
 
 def _emit_head_train(self, prev: dict) -> None:
-    """BatchNorm2d with batch statistics folded into the pool (fv.py:953-958 under .train())."""
+    """BatchNorm2d with batch statistics folded into the pool (fv.py:953-958 under .train()); the eval-grad plan folds
+    the running statistics instead (fvit_pool_bn_eval_bwd reads them directly)."""
     m, B, nb = self.model, self.B, self.bufs
     nf = m.num_features
     T = prev["H"] * prev["W"]
-    st = nb.new("norm.stats", (2, nf), torch.float32)
-    self.fwd_zero.append(st)
     sN = nb.new("norm.scale", (nf,), torch.float32)
     tN = nb.new("norm.shift", (nf,), torch.float32)
-    mu = nb.new("norm.mean", (nf,), torch.float32)
-    rs = nb.new("norm.rstd", (nf,), torch.float32)
-    pv = nb.new("norm.pivot", (nf,), torch.float32)
-    # the fp32 residual stream carries per-channel offsets: moments about each channel's first value
-    self._op(self.ops, "fvit_colstats_pivot_f32", prev["xs"].data_ptr(), nf, prev["crop_map"].data_ptr(), B * T, nf,
-             pv.data_ptr(), st[0].data_ptr(), st[1].data_ptr())
-    self._op(self.ops, "fvit_bn_finalize_pivot", st[0].data_ptr(), st[1].data_ptr(), pv.data_ptr(), 0, float(B * T),
-             m.norm.weight.data_ptr(), m.norm.bias.data_ptr(), float(m.norm.eps), float(m.norm.momentum),
-             m.norm.running_mean.data_ptr(),
-             m.norm.running_var.data_ptr(), None, sN.data_ptr(), tN.data_ptr(), mu.data_ptr(), rs.data_ptr(), nf)
+    mu = rs = None
+    if self.eval_grad:
+        self._op(self.ops, "fvit_affine_fold", sN.data_ptr(), tN.data_ptr(), nf, m.norm.weight.data_ptr(),
+                 m.norm.bias.data_ptr(), m.norm.running_mean.data_ptr(), m.norm.running_var.data_ptr(), float(m.norm.eps),
+                 None, None)
+    else:
+        st = nb.new("norm.stats", (2, nf), torch.float32)
+        self.fwd_zero.append(st)
+        mu = nb.new("norm.mean", (nf,), torch.float32)
+        rs = nb.new("norm.rstd", (nf,), torch.float32)
+        pv = nb.new("norm.pivot", (nf,), torch.float32)
+        # the fp32 residual stream carries per-channel offsets: moments about each channel's first value
+        self._op(self.ops, "fvit_colstats_pivot_f32", prev["xs"].data_ptr(), nf, prev["crop_map"].data_ptr(), B * T, nf,
+                 pv.data_ptr(), st[0].data_ptr(), st[1].data_ptr())
+        self._op(self.ops, "fvit_bn_finalize_pivot", st[0].data_ptr(), st[1].data_ptr(), pv.data_ptr(), 0, float(B * T),
+                 m.norm.weight.data_ptr(), m.norm.bias.data_ptr(), float(m.norm.eps), float(m.norm.momentum),
+                 m.norm.running_mean.data_ptr(),
+                 m.norm.running_var.data_ptr(), None, sN.data_ptr(), tN.data_ptr(), mu.data_ptr(), rs.data_ptr(), nf)
     pooled = nb.new("head.pooled", (B, _ru(nf, 8)), torch.float16)
     self._op(self.ops, "fvit_pool_affine_fwd", prev["xs"].data_ptr(), nf, prev["crop_map"].data_ptr(), B, T, nf,
              sN.data_ptr(), tN.data_ptr(), pooled.data_ptr(), pooled.stride(0))
@@ -511,14 +520,25 @@ def _emit_pooled_bwd(self, feat: dict) -> None:
     """Backward of the pooled features of a num_classes = 0 model: BatchNorm (batch statistics) + average pool, from
     the autograd gradient scaled by S on the device (fvit_vec_mul), as _emit_head_bwd does from the head GEMM."""
     B, nb, nf = self.B, self.bufs, self.head_sv["nf"]
-    hs = self.head_sv
-    m = self.model
     self._dpool_in = nb.new("grad.dpool_in", (B, nf), torch.float32)
     self.dense = [dict(dy=self._dpool_in)]
     dpool = nb.new("grad.dpool", (B, nf), torch.float32)
     self._op(self.bwd_ops, "fvit_vec_mul", self._dpool_in.data_ptr(), 1, ("scal", 0), 0, dpool.data_ptr(), B * nf)
+    _pool_bn_bwd(self, feat, dpool)
+
+
+def _pool_bn_bwd(self, feat: dict, dpool) -> None:
+    """head norm + average pool backward from dpool (scaled by S) into the last level's gradient rows"""
+    B, nb, hs, m = self.B, self.bufs, self.head_sv, self.model
+    nf, T = hs["nf"], hs["T"]
+    if self.eval_grad:
+        self._op(self.bwd_ops, "fvit_pool_bn_eval_bwd", feat["xs"].data_ptr(), nf, feat["crop_map"].data_ptr(), B, T, nf,
+                 m.norm.running_mean.data_ptr(), m.norm.running_var.data_ptr(), float(m.norm.eps),
+                 m.norm.weight.data_ptr(), dpool.data_ptr(), nf, ("scal", 1), feat["g"].data_ptr(), nf,
+                 self.G(m.norm.weight), self.G(m.norm.bias))
+        return
     s12 = nb.new("grad.head_s12", (2, nf), torch.float32)
-    self._op(self.bwd_ops, "fvit_pool_bn_bwd", feat["xs"].data_ptr(), nf, feat["crop_map"].data_ptr(), B, hs["T"], nf,
+    self._op(self.bwd_ops, "fvit_pool_bn_bwd", feat["xs"].data_ptr(), nf, feat["crop_map"].data_ptr(), B, T, nf,
              hs["mu"].data_ptr(), hs["rs"].data_ptr(), m.norm.weight.data_ptr(), dpool.data_ptr(), nf,
              s12[0].data_ptr(), s12[1].data_ptr(), ("scal", 1), feat["g"].data_ptr(), nf, self.G(m.norm.weight),
              self.G(m.norm.bias))
@@ -527,7 +547,7 @@ def _emit_pooled_bwd(self, feat: dict) -> None:
 def _emit_head_bwd(self, feat: dict) -> None:
     m, B, nb = self.model, self.B, self.bufs
     hs = self.head_sv
-    nf, ncls, T = hs["nf"], m.num_classes, hs["T"]
+    nf, ncls = hs["nf"], m.num_classes
     ldl = _ru(ncls, 8)
     ncp = _ru(ncls, 4)   # the loss gradient is kept in rows padded to 16 bytes (any num_classes; padding stays zero)
     self._dlogits = nb.new("grad.dlogits", (B, ncp), torch.float32)
@@ -546,11 +566,7 @@ def _emit_head_bwd(self, feat: dict) -> None:
                 ld_o32=nf)
     self._bgemm(a=dl16.data_ptr(), a_rows=B, lda=ldl, b=hs["hw16"].data_ptr(), b_rows=ncls, ldb=hs["ldh"], b_mn=True,
                 m=B, n=nf, kc=ncls, out_f32=dpool.data_ptr(), ld_o32=nf)
-    s12 = nb.new("grad.head_s12", (2, nf), torch.float32)
-    self._op(ops, "fvit_pool_bn_bwd", feat["xs"].data_ptr(), nf, feat["crop_map"].data_ptr(), B, T, nf,
-             hs["mu"].data_ptr(), hs["rs"].data_ptr(), m.norm.weight.data_ptr(), dpool.data_ptr(), nf,
-             s12[0].data_ptr(), s12[1].data_ptr(), inv, feat["g"].data_ptr(), nf, self.G(m.norm.weight),
-             self.G(m.norm.bias))
+    _pool_bn_bwd(self, feat, dpool)
 
 
 def _emit_attn_core_bwd(self, at: dict, dao, dqkv, groups: int, S: int) -> None:

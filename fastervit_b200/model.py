@@ -300,6 +300,13 @@ class FasterViT(nn.Module):
                 m.switch_to_deploy()
         return self
 
+    def release_eval_grad_plans(self) -> None:
+        """Free the device memory of eval-mode gradients: the first backward of a grad-enabled eval forward builds a
+        plan per input shape that holds a training step's saved activations and keeps it; this drops them (the next
+        such backward builds its plan again)."""
+        if self._engine is not None:
+            self._engine.release_eval_grad_plans()
+
     def forward_levels(self, x, out_indices=(0, 1, 2, 3)):
         """Per-level feature maps [B, C_i, H_i, W_i] (each level's output before its Downsample), the `xo` a dense-
         prediction backbone taps (downstream/object_detection/dino/models/dino/fastervit.py:686-709, 816-827).

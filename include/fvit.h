@@ -410,6 +410,35 @@ int fvit_bn_bwd(const void* gin, int32_t g_is_f16, int64_t ldg, const int32_t* g
                 const int32_t* r_rows, int32_t nrows, int32_t C, const float* mean, const float* rstd, const float* w,
                 const float* b, int32_t act, const float* colmul, float* s1, float* s2, const float* scalar, void* out16,
                 int64_t ldo, const int32_t* o_rows, float* dw, float* db, const float* row_scale, void* stream);
+
+/* ---- Eval-mode gradients: the backward of model(x) under .eval() ----
+ * An eval forward with grad enabled runs the inference launch list unchanged and records the input; its backward
+ * recomputes that forward as a saving train-style forward whose BatchNorms use their running statistics (no drop
+ * path, no statistics update), then runs the training backward with the three entry points below. The cost of one
+ * backward is therefore one extra forward on top of a training step's forward + backward; a forward with no backward
+ * costs what an inference forward costs. */
+/* BatchNorm2d on running statistics, backward over row lists: xhat = (raw - mean) * rsqrt(var + eps),
+ * dy = gin (fp32 or fp16) * colmul, masked by the ReLU derivative when act == FVIT_ACT_RELU (sign of xhat*w + b);
+ * out16[o_rows[r]] = w*rsqrt(var+eps)*dy; dw += *scalar * sum dy*xhat; db += *scalar * sum dy. One pass, no scratch.
+ * With C % 4 == 0, 16-byte aligned rows and every leading dimension a multiple of 8 elements (4 for fp32 gin), the
+ * padding columns of an out16 row up to the next multiple of 8 are written as zeros. */
+int fvit_bn_eval_bwd(const void* gin, int32_t g_is_f16, int64_t ldg, const int32_t* g_rows, const void* raw16,
+                     int64_t ldr, const int32_t* r_rows, int32_t nrows, int32_t C, const float* mean, const float* var,
+                     float eps, const float* w, const float* b, int32_t act, const float* colmul, const float* scalar,
+                     void* out16, int64_t ldo, const int32_t* o_rows, float* dw, float* db, void* stream);
+/* Backward of the head's running-statistics BatchNorm2d + AdaptiveAvgPool2d(1) (fv.py:953-958 under .eval()):
+ * g[row(b,t)][c] = dpool[b][c] / T * w[c] * rsqrt(var[c] + eps) (written); dw += *scalar * sum_b dpool * mean_t xhat;
+ * dbeta += *scalar * sum_b dpool. Row conventions as fvit_pool_bn_bwd. */
+int fvit_pool_bn_eval_bwd(const float* xs, int64_t ldx, const int32_t* rows, int32_t B, int32_t T, int32_t C,
+                          const float* mean, const float* var, float eps, const float* w, const float* dpool,
+                          int64_t lddp, const float* scalar, float* g, int64_t ldg, float* dw, float* dbeta,
+                          void* stream);
+/* Image gradient of the stem's first convolution (3x3, stride 2, pad 1, 3 input channels, fv.py:458):
+ * dx[b][ci][y][x] = *scalar * sum w[co][ci][ky][kx] * dz[(b*H1 + oy)*W1 + ox][co] over y = 2*oy - 1 + ky,
+ * x = 2*ox - 1 + kx, with H1 = (H+1)/2, W1 = (W+1)/2. dz: fp16 rows of stride lddz; w: fp32 [cout, 3, 3, 3],
+ * cout <= 512; dx: fp32 NCHW [B, 3, H, W], every element written. A gather (no atomics): deterministic. */
+int fvit_stem_conv_dgrad(const void* dz16, int64_t lddz, int32_t B, int32_t H, int32_t W, const float* wgt,
+                         int32_t cout, const float* scalar, float* dx, void* stream);
 /* dst[co][ci][tap] += src[co][tap * cin + ci] (row stride ld): the b_ntaps weight-gradient GEMM output ->
  * nn.Conv2d layout. */
 int fvit_unpack_conv_grad(const float* src, int32_t ld, float* dst, int32_t cout, int32_t cin, void* stream);
