@@ -269,6 +269,46 @@ stem_conv_dgrad_kernel(const __half* __restrict__ dz, long long lddz, int vec, i
   }
 }
 
+// col2im of the same convolution for any channel count: the tap products arrive precomputed as fp32 rows
+// dcol[(b*H1 + oy)*W1 + ox][ci*9 + ky*3 + kx] (the GEMM dz . W1), and dx gathers them exactly as above. A block owns
+// the same 15 x 15 positions / 30 x 30 pixels and walks the channels in chunks of SC_CH, staging each chunk's 16 x 16
+// window of tap entries in shared memory, so the tile does not grow with cin.
+constexpr int SC_CH = 4;
+__global__ void __launch_bounds__(256)
+stem_col2im_kernel(const float* __restrict__ dcol, long long ldc, int cin, int H, int W, int H1, int W1,
+                   float* __restrict__ dx) {
+  __shared__ float P[SD_WIN * SD_WIN * SC_CH * 9];   // [position][ci - c0][ky][kx]
+  const int b = blockIdx.z, oy0 = blockIdx.y * SD_OWN, ox0 = blockIdx.x * SD_OWN;
+  constexpr int SPAN = 2 * SD_OWN;
+  for (int c0 = 0; c0 < cin; c0 += SC_CH) {
+    const int nc = min(SC_CH, cin - c0), cols = nc * 9;
+    // positions outside the map stage zeros, so the gather below needs no bounds test on them
+    for (int i = threadIdx.x; i < SD_WIN * SD_WIN * cols; i += 256) {
+      const int pos = i / cols, k = i - pos * cols;
+      const int oy = oy0 + pos / SD_WIN, ox = ox0 + pos % SD_WIN;
+      P[i] = (oy < H1 && ox < W1) ? __ldg(dcol + ((long long)(b * H1 + oy) * W1 + ox) * ldc + c0 * 9 + k) : 0.f;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < nc * SPAN * SPAN; i += 256) {
+      const int cl = i / (SPAN * SPAN), yy = (i / SPAN) % SPAN, xx = i % SPAN;
+      const int y = 2 * oy0 + yy, x = 2 * ox0 + xx;
+      if (y >= H || x >= W) continue;
+      // even coordinate: tap 1 of output position c/2; odd: tap 0 of (c+1)/2 and tap 2 of (c-1)/2
+      const int nky = (yy & 1) ? 2 : 1, nkx = (xx & 1) ? 2 : 1;
+      float v = 0.f;
+      for (int a = 0; a < nky; ++a) {
+        const int ky = (yy & 1) ? 2 * a : 1, ly = (yy & 1) ? (yy + 1) / 2 - a : yy / 2;
+        for (int e = 0; e < nkx; ++e) {
+          const int kx = (xx & 1) ? 2 * e : 1, lx = (xx & 1) ? (xx + 1) / 2 - e : xx / 2;
+          v += P[(ly * SD_WIN + lx) * cols + cl * 9 + ky * 3 + kx];
+        }
+      }
+      dx[(((long long)b * cin + c0 + cl) * H + y) * W + x] = v;
+    }
+    __syncthreads();
+  }
+}
+
 }  // namespace fvit
 
 using namespace fvit;
@@ -350,6 +390,18 @@ int fvit_stem_conv_dgrad(const void* dz16, int64_t lddz, int32_t B, int32_t H, i
   stem_conv_dgrad_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>((const __half*)dz16, lddz, vec, H, W, H1, W1, wgt,
                                                                      cout, scalar, dx);
   return post_launch("stem_conv_dgrad_kernel");
+}
+
+int fvit_stem_col2im(const float* dcol, int64_t ldc, int32_t B, int32_t cin, int32_t H, int32_t W, float* dx,
+                     void* stream) {
+  FVIT_CHECK(dcol && dx && B > 0 && H > 0 && W > 0 && ldc >= 9 * (int64_t)cin, "fvit_stem_col2im: bad arguments");
+  FVIT_CHECK(cin >= 1 && cin <= FVIT_STEM_MAX_CIN, "fvit_stem_col2im: in_chans=%d must be in [1, %d]", cin,
+             FVIT_STEM_MAX_CIN);
+  const int H1 = (H + 1) / 2, W1 = (W + 1) / 2;
+  FVIT_CHECK(B <= 65535 && (H1 + SD_OWN - 1) / SD_OWN <= 65535, "fvit_stem_col2im: B=%d H=%d too large", B, H);
+  dim3 grid((unsigned)((W1 + SD_OWN - 1) / SD_OWN), (unsigned)((H1 + SD_OWN - 1) / SD_OWN), (unsigned)B);
+  stem_col2im_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(dcol, ldc, cin, H, W, H1, W1, dx);
+  return post_launch("stem_col2im_kernel");
 }
 
 }  // extern "C"

@@ -335,6 +335,36 @@ __global__ void __launch_bounds__(256)
   for (int q = KP / 8; q < ldo / 8; ++q) o[q] = make_uint4(0, 0, 0, 0);
 }
 
+// The same im2col for any channel count (in_chans != 3): one thread per (pixel, 8-column group), so a thread holds
+// 8 taps whatever cin is. Consecutive threads write consecutive 16-byte pieces of the (contiguous) output rows.
+__global__ void __launch_bounds__(256)
+    stem_im2col_any_kernel(const float* __restrict__ x, long long sb, long long sc, long long sh, long long sw,
+                           int B, int cin, int H, int W, __half* __restrict__ out, int ldo) {
+  const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
+  const int groups = ldo / 8, K = cin * 9;
+  const long long total = (long long)B * Ho * Wo * groups;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int q = (int)(i % groups);
+    const long long pix = i / groups;
+    const int ow = (int)(pix % Wo);
+    const int oh = (int)((pix / Wo) % Ho);
+    const int b = (int)(pix / ((long long)Wo * Ho));
+    __align__(16) __half v[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      const int k = q * 8 + u;
+      float f = 0.f;
+      if (k < K) {
+        const int c = k / 9, t = k - c * 9;
+        const int ih = 2 * oh + t / 3 - 1, iw = 2 * ow + t % 3 - 1;
+        if (ih >= 0 && ih < H && iw >= 0 && iw < W) f = __ldg(x + b * sb + c * sc + ih * sh + iw * sw);
+      }
+      v[u] = __float2half_rn(f);
+    }
+    *reinterpret_cast<uint4*>(out + pix * ldo + q * 8) = *reinterpret_cast<const uint4*>(v);
+  }
+}
+
 // ------------------------------------------------------------------------------ LayerNorm forward
 // One warp per row. v = x[in_map ? in_map[r] : r] (+ add[(r % group) - skip] if (r % group) >= skip);
 // optionally written back as fp32 to wb[r]; y = (v - mean) * rstd * gamma + beta written as fp16 to
@@ -931,11 +961,19 @@ int fvit_stem_conv_fwd(const float* x, int64_t sb, int64_t sc, int64_t sh, int64
 int fvit_stem_im2col(const float* x, int64_t sb, int64_t sc, int64_t sh, int64_t sw, int32_t B, int32_t cin,
                      int32_t H, int32_t W, void* out, int32_t ldo, void* stream) {
   FVIT_CHECK(x && out && B > 0 && H > 0 && W > 0, "fvit_stem_im2col: bad arguments");
-  FVIT_CHECK(cin == 3, "fvit_stem_im2col: only in_chans == 3 is supported (got %d)", cin);
-  FVIT_CHECK(ldo % 8 == 0 && ldo >= 32, "fvit_stem_im2col: ldo=%d must be a multiple of 8 and >= 32", ldo);
+  FVIT_CHECK(cin >= 1 && cin <= FVIT_STEM_MAX_CIN, "fvit_stem_im2col: in_chans=%d must be in [1, %d]", cin,
+             FVIT_STEM_MAX_CIN);
+  const int stem_ld = (9 * cin + 31) / 32 * 32;
+  FVIT_CHECK(ldo % 8 == 0 && ldo >= stem_ld, "fvit_stem_im2col: ldo=%d must be a multiple of 8 and >= %d", ldo,
+             stem_ld);
   FVIT_CHECK((reinterpret_cast<uintptr_t>(out) & 15) == 0, "fvit_stem_im2col: out must be 16-byte aligned");
   const long long total = (long long)B * ((H + 1) / 2) * ((W + 1) / 2);
   FVIT_CHECK(total < (1ll << 31), "fvit_stem_im2col: too many pixels");
+  if (cin != 3) {
+    stem_im2col_any_kernel<<<grid_for(total * (ldo / 8), 256), 256, 0, (cudaStream_t)stream>>>(
+        x, sb, sc, sh, sw, B, cin, H, W, (__half*)out, ldo);
+    return post_launch("stem_im2col_any_kernel");
+  }
   stem_im2col_kernel<3><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       x, sb, sc, sh, sw, B, H, W, (__half*)out, ldo);
   return post_launch("stem_im2col_kernel");

@@ -24,6 +24,8 @@ import torch.nn as nn
 
 from . import lib as L
 
+STEM_MAX_CIN = 64   # in_chans limit of the stem kernels (FVIT_STEM_MAX_CIN, include/fvit.h)
+
 
 def _ru(x: int, m: int) -> int:
     return (x + m - 1) // m * m
@@ -242,19 +244,18 @@ class Plan:
                                        + ((yi >> 1) + 1) * (W0 + 1) + (xi >> 1) + 1).reshape(-1))
         pe = m.patch_embed.conv_down
         s1, t1 = self._fold("stem.bn1", in_dim, pe[1])
-        # conv1 (fv.py:458-460) on tensor cores: im2col rows [pixel, 27 -> STEM_LD] (one HBM-bound
-        # kernel), then a single-K-block GEMM with the BN + ReLU epilogue scattering into the planes
-        col16 = nb.new("stem.col16", (B * H1 * W1, self.STEM_LD), torch.float16)
-        self._x_args.append(dict(B=B, cin=cfg["in_chans"], H=self.H, W=self.W, out=col16.data_ptr(),
-                                 ldo=self.STEM_LD))
+        # conv1 (fv.py:458-460) on tensor cores: im2col rows [pixel, 9*in_chans -> stem_ld] (one HBM-bound
+        # kernel), then a GEMM (one K block up to 7 channels) with the BN + ReLU epilogue scattering into the planes
+        k1, sld = self.stem_cols()
+        col16 = nb.new("stem.col16", (B * H1 * W1, sld), torch.float16)
+        self._x_args.append(dict(B=B, cin=cfg["in_chans"], H=self.H, W=self.W, out=col16.data_ptr(), ldo=sld))
         self.ops.append(("im2col", len(self._x_args) - 1, "fvit_stem_im2col"))
-        w1 = nb.new("stem.conv1.w16", (in_dim, self.STEM_LD), torch.float16)
-        self._op(self.prep_ops, "fvit_cast_pad_f16", pe[0].weight.data_ptr(), 27, w1.data_ptr(), self.STEM_LD,
-                 in_dim, 27, 32)
-        self._gemm(a=col16.data_ptr(), a_rows=B * H1 * W1, lda=self.STEM_LD, b=w1.data_ptr(), ldb=self.STEM_LD,
-                   m=B * H1 * W1, n=in_dim, kc=32, col_scale=s1.data_ptr(), col_shift=t1.data_ptr(),
+        w1 = nb.new("stem.conv1.w16", (in_dim, sld), torch.float16)
+        self._op(self.prep_ops, "fvit_cast_pad_f16", pe[0].weight.data_ptr(), k1, w1.data_ptr(), sld, in_dim, k1, sld)
+        self._gemm(a=col16.data_ptr(), a_rows=B * H1 * W1, lda=sld, b=w1.data_ptr(), ldb=sld,
+                   m=B * H1 * W1, n=in_dim, kc=sld, col_scale=s1.data_ptr(), col_shift=t1.data_ptr(),
                    act=L.ACT_RELU, row_map=stem_map.data_ptr(), out_f16=stem_planes.data_ptr(), ld_o16=ld_in)
-        self.op_flops[len(self.ops) - 1] = 2.0 * B * H1 * W1 * in_dim * 27
+        self.op_flops[len(self.ops) - 1] = 2.0 * B * H1 * W1 * in_dim * k1
 
         lvl = self._conv_level_buffers(0, dim, H0, W0)
         w16, ldw = self._pack_conv("stem.conv2", pe[3])
@@ -315,6 +316,14 @@ class Plan:
             self.logits = None
 
     # ---- geometry helpers -----------------------------------------------------------------------
+    def stem_cols(self) -> tuple[int, int]:
+        """(9 * in_chans, stem_ld): the taps of the first stem convolution and the fp16 row width of its im2col matrix,
+        zero padded to a multiple of 32 (STEM_LD for RGB)"""
+        cin = self.model.cfg["in_chans"]
+        if not 1 <= cin <= STEM_MAX_CIN:
+            raise L.FvitError(f"in_chans={cin}: the stem kernels support 1 <= in_chans <= {STEM_MAX_CIN}")
+        return 9 * cin, (self.STEM_LD if cin == 3 else _ru(9 * cin, 32))
+
     def _s2_taps(self, Wo: int) -> list[tuple[int, int]]:
         """9 taps of a 3x3 stride-2 pad-1 convolution over the parity-plane layout: input row 2*oh+r-1
         lives in plane parity (r+1)&1 at plane row oh + (r==0 ? -1 : 0) (+1 border offset cancels)."""
@@ -876,6 +885,8 @@ class Engine:
                               "CUDA device (`.cuda()`); there is no CPU / PyTorch fallback path")
         if x.dim() != 4 or x.dtype != torch.float32:
             raise L.FvitError(f"expected a float32 [B, C, H, W] tensor, got {tuple(x.shape)} {x.dtype}")
+        if x.shape[1] != self.model.cfg["in_chans"]:
+            raise L.FvitError(f"the model takes {self.model.cfg['in_chans']}-channel images, got {tuple(x.shape)}")
         p0 = next(self.model.parameters())
         if p0.device != x.device:
             raise L.FvitError(f"model is on {p0.device} but the input is on {x.device}")

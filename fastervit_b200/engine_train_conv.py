@@ -87,19 +87,21 @@ def _emit_conv_part_train(self) -> dict:
     pe = m.patch_embed.conv_down
     st = dict(H1=H1, W1=W1, H0=H0, W0=W0, pl_rows=pl_rows, ld_in=ld_in, npix1=npix1, stem_map=stem_map)
     # conv1: im2col + GEMM -> raw1 (plane layout) + statistics
-    col16 = nb.new("stem.col16", (npix1, self.STEM_LD), torch.float16)
-    self._x_args.append(dict(B=B, cin=cfg["in_chans"], H=self.H, W=self.W, out=col16.data_ptr(), ldo=self.STEM_LD))
+    k1, sld = self.stem_cols()
+    st.update(k1=k1, sld=sld)
+    col16 = nb.new("stem.col16", (npix1, sld), torch.float16)
+    self._x_args.append(dict(B=B, cin=cfg["in_chans"], H=self.H, W=self.W, out=col16.data_ptr(), ldo=sld))
     self.ops.append(("im2col", len(self._x_args) - 1, "fvit_stem_im2col"))
-    w1 = nb.new("stem.conv1.w16", (in_dim, self.STEM_LD), torch.float16)
-    self._op(self.prep_ops, "fvit_cast_pad_f16", pe[0].weight.data_ptr(), 27, w1.data_ptr(), self.STEM_LD, in_dim, 27, 32)
+    w1 = nb.new("stem.conv1.w16", (in_dim, sld), torch.float16)
+    self._op(self.prep_ops, "fvit_cast_pad_f16", pe[0].weight.data_ptr(), k1, w1.data_ptr(), sld, in_dim, k1, sld)
     raw1 = nb.new("stem.raw1", (4 * pl_rows, ld_in), torch.float16)
     planes = nb.new("stem.planes", (4 * pl_rows, ld_in), torch.float16)
     bn1 = _bn_train(self, "stem.bn1", pe[1], npix1)
-    self._gemm(a=col16.data_ptr(), a_rows=npix1, lda=self.STEM_LD, b=w1.data_ptr(), ldb=self.STEM_LD, m=npix1, n=in_dim,
-               kc=32, col_shift=_bn_col_shift(self, bn1, None), row_map=stem_map.data_ptr(), out_f16=raw1.data_ptr(),
+    self._gemm(a=col16.data_ptr(), a_rows=npix1, lda=sld, b=w1.data_ptr(), ldb=sld, m=npix1, n=in_dim,
+               kc=sld, col_shift=_bn_col_shift(self, bn1, None), row_map=stem_map.data_ptr(), out_f16=raw1.data_ptr(),
                ld_o16=ld_in, col_sum=bn1["col_sum"],
                col_sumsq=bn1["col_sumsq"])
-    self.op_flops[len(self.ops) - 1] = 2.0 * npix1 * in_dim * 27
+    self.op_flops[len(self.ops) - 1] = 2.0 * npix1 * in_dim * k1
     _bn_finalize(self, bn1)
     self._op(self.ops, "fvit_affine_rows", raw1.data_ptr(), ld_in, stem_map.data_ptr(), npix1, in_dim, bn1["sc"].data_ptr(),
              bn1["sh"].data_ptr(), L.ACT_RELU, None, 0, None, 0, planes.data_ptr(), ld_in, None)
@@ -407,14 +409,24 @@ def _emit_conv_part_bwd(self) -> None:
     dz1 = nb.new("stem.dz1", (npix1, ld_in), torch.float16)
     _bn_bwd(self, bn1, dplanes.data_ptr(), 1, ld_in, st["stem_map"].data_ptr(), st["raw1"].data_ptr(), ld_in,
             st["stem_map"].data_ptr(), npix1, L.ACT_RELU, dz1.data_ptr(), ld_in, None)
-    self._bgemm(a=dz1.data_ptr(), a_rows=npix1, lda=ld_in, a_mn=True, b=st["col16"].data_ptr(), b_rows=npix1, ldb=self.STEM_LD,
-                b_mn=True, m=in_dim, n=27, kc=npix1, split_k=self._split_k(in_dim, 27, npix1), alpha_ptr=inv,
-                out_f32=self.G(pe[0].weight), ld_o32=27, flops=2.0 * npix1 * in_dim * 27)
+    k1, sld = st["k1"], st["sld"]
+    self._bgemm(a=dz1.data_ptr(), a_rows=npix1, lda=ld_in, a_mn=True, b=st["col16"].data_ptr(), b_rows=npix1, ldb=sld,
+                b_mn=True, m=in_dim, n=k1, kc=npix1, split_k=self._split_k(in_dim, k1, npix1), alpha_ptr=inv,
+                out_f32=self.G(pe[0].weight), ld_o32=k1, flops=2.0 * npix1 * in_dim * k1)
     if self.eval_grad:
         # the image gradient (fp32 NCHW, like x): the backward of conv1, 3x3 / stride 2 / pad 1, as a gather
-        self.dx = nb.new("stem.dx", (B, m.cfg["in_chans"], self.H, self.W), torch.float32)
-        self._op(ops, "fvit_stem_conv_dgrad", dz1.data_ptr(), ld_in, B, self.H, self.W, pe[0].weight.data_ptr(), in_dim,
-                 inv, self.dx.data_ptr())
+        cin = m.cfg["in_chans"]
+        self.dx = nb.new("stem.dx", (B, cin, self.H, self.W), torch.float32)
+        if cin == 3:
+            self._op(ops, "fvit_stem_conv_dgrad", dz1.data_ptr(), ld_in, B, self.H, self.W, pe[0].weight.data_ptr(),
+                     in_dim, inv, self.dx.data_ptr())
+        else:
+            # any other channel count: the tap products dcol = dz1 . W1 / S on tensor cores, then a gather of them
+            ldc = _ru(k1, 4)
+            dcol = nb.new("stem.dcol", (npix1, ldc), torch.float32)
+            self._bgemm(a=dz1.data_ptr(), a_rows=npix1, lda=ld_in, b=st["w1"].data_ptr(), b_rows=in_dim, ldb=sld, b_mn=True,
+                        m=npix1, n=k1, kc=in_dim, alpha_ptr=inv, out_f32=dcol.data_ptr(), ld_o32=ldc)
+            self._op(ops, "fvit_stem_col2im", dcol.data_ptr(), ldc, B, cin, self.H, self.W, self.dx.data_ptr())
 
 
 class ConvPartEmitters:

@@ -169,8 +169,12 @@ int fvit_stem_conv_fwd(const float* x, int64_t sb, int64_t sc, int64_t sh, int64
                        void* out, int64_t ldo, float* col_sum, float* col_sumsq, void* stream);
 
 /* im2col of the same convolution for the tensor-core path: out[pixel][c*9 + r*3 + s] = (half) input tap
- * (zero outside the image and in the padding columns up to ldo); the 27-deep contraction then runs as a
- * plain fvit_gemm with the BatchNorm/ReLU epilogue. */
+ * (zero outside the image and in the padding columns up to ldo); the 9*cin-deep contraction then runs as a
+ * plain fvit_gemm with the BatchNorm/ReLU epilogue (kc = stem_ld, one K block up to cin = 7). Any channel count
+ * 1 <= cin <= FVIT_STEM_MAX_CIN; ldo must be a multiple of 8 and at least stem_ld = round_up(9*cin, 32) (32 for
+ * RGB). cin == 3 has a kernel of its own (one thread per pixel row); every other cin writes one 16-byte piece of a
+ * row per thread. */
+#define FVIT_STEM_MAX_CIN 64
 int fvit_stem_im2col(const float* x, int64_t sb, int64_t sc, int64_t sh, int64_t sw, int32_t B, int32_t cin,
                      int32_t H, int32_t W, void* out, int32_t ldo, void* stream);
 
@@ -439,6 +443,13 @@ int fvit_pool_bn_eval_bwd(const float* xs, int64_t ldx, const int32_t* rows, int
  * cout <= 512; dx: fp32 NCHW [B, 3, H, W], every element written. A gather (no atomics): deterministic. */
 int fvit_stem_conv_dgrad(const void* dz16, int64_t lddz, int32_t B, int32_t H, int32_t W, const float* wgt,
                          int32_t cout, const float* scalar, float* dx, void* stream);
+/* The image gradient of the same convolution for any channel count, second half: the tap products come as fp32 rows
+ * dcol[(b*H1 + oy)*W1 + ox][ci*9 + ky*3 + kx] (row stride ldc >= 9*cin; the fvit_gemm dz . W1 with W1 the conv weight
+ * viewed as [cout, 9*cin], scaled as the gradient needs), and dx[b][ci][y][x] = sum of the 1, 2 or 4 entries whose
+ * tap reads (y, x). dx: fp32 NCHW [B, cin, H, W], every element written, 1 <= cin <= FVIT_STEM_MAX_CIN. A gather
+ * (no atomics): deterministic. The plans use it for in_chans != 3 and fvit_stem_conv_dgrad for 3. */
+int fvit_stem_col2im(const float* dcol, int64_t ldc, int32_t B, int32_t cin, int32_t H, int32_t W, float* dx,
+                     void* stream);
 /* dst[co][ci][tap] += src[co][tap * cin + ci] (row stride ld): the b_ntaps weight-gradient GEMM output ->
  * nn.Conv2d layout. */
 int fvit_unpack_conv_grad(const float* src, int32_t ld, float* dst, int32_t cout, int32_t cin, void* stream);
