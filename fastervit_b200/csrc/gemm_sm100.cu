@@ -16,6 +16,13 @@
 // The A operand of K-block kb is the 2-D box at row (m0 + tap_shift[tap]) of plane tap_plane[tap]:
 // with 9 taps this is an im2col-free 3x3 convolution over a zero-bordered NHWC activation matrix
 // (out-of-range rows are zero-filled by TMA). See include/fvit.h for the exact contract.
+//
+// Slab mode (stride-1 3x3 taps, tap_shift[3 dy + dx] = (dy - 1) P + (dx - 1) on one plane, kc > 128): the three
+// taps of a kernel row read the same activation rows one row apart, so per (K block, dy) the producer loads one
+// 136-row slab, rows
+// m0 + (dy - 1) P - 1 .. +136, into a two-buffer slab ring, and only the weight tiles go through the stage ring (one
+// stage per tap and K block). Tap dx of MMA warpgroup g reads slab rows [64g + dx, 64g + dx + 64). The K loop runs
+// in (K block, dy, dx) order. Per K block this moves 3 x 17 KB of A instead of 9 x 16 KB.
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
 
@@ -42,8 +49,11 @@ constexpr int GEMM_THREADS = MMA_THREADS + EPI_THREADS + 128;
 // surplus goes to the epilogue: 40 + 128 + 128 + 216 = 4 x 128.
 constexpr uint32_t PRODUCER_REGS = 40;
 constexpr uint32_t EPILOGUE_REGS = 216;
-constexpr int MAX_STAGES = 8;
+constexpr int MAX_STAGES = 12;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
+constexpr int SLAB_ROWS = BM + 8;           // slab mode: the 128 + 2 rows of three dx taps, rounded up to 8 rows
+constexpr int SLAB_BYTES = SLAB_ROWS * BK * 2;  // 17 KB: a whole number of 1024-byte swizzle patterns
+constexpr int SLAB_BUFS = 2;
 constexpr int MAX_TILE_N = 128;             // widest MMA of the kernel (the accumulator tile lives in shared memory)
 constexpr int SMEM_BUDGET = 227 * 1024;
 constexpr int SMEM_CTRL_BYTES = 1024;  // barriers, placed after the stage ring
@@ -65,6 +75,7 @@ struct GemmParams {
   int b_ntaps, tiles_per_tap;  // >1: N tiles enumerate (tap, n tile); tap t reads B rows shifted by tap_shift[t]
   int atomic_out;  // split-K style accumulation: atomicAdd(alpha * acc) into out_f32
   int stages;
+  int slab_pitch;  // > 0: slab mode (see the top of this file); the row pitch P of the 3x3 taps
   int tap_shift[16];
   int tap_plane[16];
   // epilogue
@@ -222,14 +233,17 @@ __device__ __forceinline__ void unit_cols(const GemmParams& p, int tn, int& n0, 
 // Main loop of one work unit for MMA width N: the MMA warpgroup g accumulates rows [64g, 64g + 64) of the tile
 // over K blocks [kb0, kb1) and leaves them in the shared-memory accumulator tile. One K block's MMAs stay in flight
 // while the next block's are issued; each warp releases a ring stage once its warpgroup's MMAs on it have completed.
+// In slab mode a "K block" kb is (channel block kb / 9, tap kb % 9): A comes from the slab ring (a stage holds only
+// the weight tile) and a slab is released with the stage of its third tap.
 // The accumulator tile is written once the epilogue has released it (acc_empty of the previous unit, acc_parity =
 // the parity of this CTA's unit count) and handed over through acc_full. Columns >= N of the tile keep the values
 // of an earlier unit: the epilogue only reads the unit's valid columns.
-template <int N, int TA, int TB, int BF16>
-__device__ __forceinline__ void gemm_mainloop(const GemmParams& p, uint8_t* smem, int stage_bytes, uint64_t* full_bar,
-                                              uint64_t* empty_bar, int& stage, uint32_t& phase, int kb0, int kb1,
-                                              float* accbuf, uint64_t* acc_full, uint64_t* acc_empty,
-                                              uint32_t acc_parity) {
+template <int N, int TA, int TB, int BF16, bool SLAB>
+__device__ __forceinline__ void gemm_mainloop(const GemmParams& p, uint8_t* smem, int stage_bytes, int a_stage_bytes,
+                                              uint64_t* full_bar, uint64_t* empty_bar, int& stage, uint32_t& phase,
+                                              uint8_t* slabs, uint64_t* slab_full, uint64_t* slab_empty, int& slab,
+                                              uint32_t& slab_phase, int kb0, int kb1, float* accbuf,
+                                              uint64_t* acc_full, uint64_t* acc_empty, uint32_t acc_parity) {
   const int g = (threadIdx.x >> 7) & 1;
   const int lane = threadIdx.x & 31;
   // K-major SW128: SBO = 1024 (8 rows x 128 B), LBO unused; MN-major SW128: LBO = BK*128 (next 64-wide MN atom),
@@ -241,18 +255,37 @@ __device__ __forceinline__ void gemm_mainloop(const GemmParams& p, uint8_t* smem
   float d[N / 2];
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
-  int prev = -1;  // ring stage of the K block whose MMAs are still in flight
+  int prev = -1;       // ring stage of the K block whose MMAs are still in flight
+  int prev_slab = -1;  // slab mode: the slab to release with it (its third tap), or -1
   for (int kb = kb0; kb < kb1; ++kb) {
+    uint32_t sa;
+    int last_kb, done_slab = -1;
+    if constexpr (SLAB) {
+      const int dx = kb % 3;
+      if (dx == 0) mbar_wait(&slab_full[slab], slab_phase);
+      // rows 64g + dx .. of the slab (the swizzle phase follows the address: see make_smem_desc)
+      sa = smem_u32(slabs + slab * SLAB_BYTES) + (64 * g + dx) * 128;
+      last_kb = kb / 9 == p.kb_per_tap - 1;
+      if (dx == 2) {
+        done_slab = slab;
+        if (++slab == SLAB_BUFS) {
+          slab = 0;
+          slab_phase ^= 1;
+        }
+      }
+    } else {
+      sa = smem_u32(smem + stage * stage_bytes) + g * 8192;
+      last_kb = (kb + 1) % p.kb_per_tap == 0;
+    }
     mbar_wait(&full_bar[stage], phase);
-    const uint32_t sa = smem_u32(smem + stage * stage_bytes) + g * 8192;
-    const uint32_t sb = smem_u32(smem + stage * stage_bytes) + A_STAGE_BYTES;
+    const uint32_t sb = smem_u32(smem + stage * stage_bytes) + a_stage_bytes;
     auto mma = [&](int k) {
       Wgmma<N, TA, TB, BF16>::mma(d, make_smem_desc(sa + k * a_kstep, a_lbo, 1024, SWZ_128B),
                                   make_smem_desc(sb + k * b_kstep, b_lbo, 1024, SWZ_128B), 1u);
     };
     // a tap's last K-block is zero beyond kc (TMA out-of-bounds fill / zero-padded weights): its all-zero
     // 16-wide steps are not issued (K = 196 per conv tap: 13 instead of 16 MMAs; K = 784: 49 instead of 52)
-    const int nk = (kb + 1) % p.kb_per_tap == 0 ? p.k_tail16 : BK / MMA_K;
+    const int nk = last_kb ? p.k_tail16 : BK / MMA_K;
     // (each case is a complete wgmma group: a branch between the MMAs of one group would serialize them)
     switch (nk) {
       case 1: wgmma_fence(); mma(0); wgmma_commit(); break;
@@ -263,9 +296,13 @@ __device__ __forceinline__ void gemm_mainloop(const GemmParams& p, uint8_t* smem
     wgmma_wait1();  // the previous K block's MMAs are complete
     if (prev >= 0) {
       __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      if (lane == 0) {
+        mbar_arrive(&empty_bar[prev]);
+        if (prev_slab >= 0) mbar_arrive(&slab_empty[prev_slab]);
+      }
     }
     prev = stage;
+    prev_slab = done_slab;
     if (++stage == p.stages) {
       stage = 0;
       phase ^= 1;
@@ -274,21 +311,27 @@ __device__ __forceinline__ void gemm_mainloop(const GemmParams& p, uint8_t* smem
   wgmma_wait0();
   if (prev >= 0) {
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    if (lane == 0) {
+      mbar_arrive(&empty_bar[prev]);
+      if (prev_slab >= 0) mbar_arrive(&slab_empty[prev_slab]);
+    }
   }
   mbar_wait(acc_empty, acc_parity ^ 1);  // the epilogue has read the previous unit's tile
   acc_store<N>(accbuf + g * 64 * ACC_LD, ACC_LD, d);
   mbar_arrive(acc_full);
 }
 
-template <int TA, int TB, int BF16>
+template <int TA, int TB, int BF16, bool SLAB>
 __device__ __forceinline__ void gemm_mainloop_n(int mma_n, const GemmParams& p, uint8_t* smem, int stage_bytes,
-                                                uint64_t* full_bar, uint64_t* empty_bar, int& stage, uint32_t& phase,
-                                                int kb0, int kb1, float* accbuf, uint64_t* acc_full,
-                                                uint64_t* acc_empty, uint32_t acc_parity) {
-#define FVIT_MAINLOOP(N)                                                                                              \
-  gemm_mainloop<N, TA, TB, BF16>(p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf, acc_full, \
-                                 acc_empty, acc_parity)
+                                                int a_stage_bytes, uint64_t* full_bar, uint64_t* empty_bar, int& stage,
+                                                uint32_t& phase, uint8_t* slabs, uint64_t* slab_full,
+                                                uint64_t* slab_empty, int& slab, uint32_t& slab_phase, int kb0,
+                                                int kb1, float* accbuf, uint64_t* acc_full, uint64_t* acc_empty,
+                                                uint32_t acc_parity) {
+#define FVIT_MAINLOOP(N)                                                                                          \
+  gemm_mainloop<N, TA, TB, BF16, SLAB>(p, smem, stage_bytes, a_stage_bytes, full_bar, empty_bar, stage, phase, slabs,   \
+                                 slab_full, slab_empty, slab, slab_phase, kb0, kb1, accbuf, acc_full, acc_empty, \
+                                 acc_parity)
   switch (mma_n) {
     case 16: FVIT_MAINLOOP(16); break;
     case 32: FVIT_MAINLOOP(32); break;
@@ -315,12 +358,16 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   const int unit0 = blockIdx.x, nunits = gridDim.x;  // work units are dealt to CTAs round-robin
   // MN-major B is staged as whole 64-column atoms (the MMA reads the first columns of them)
   const int b_stage_bytes = (p.b_mn ? ((p.tile_n + 63) & ~63) : p.tile_n) * BK * 2;
-  const int stage_bytes = A_STAGE_BYTES + b_stage_bytes;
-  uint8_t* ctrl = smem + p.stages * stage_bytes;
+  const int a_stage_bytes = p.slab_pitch ? 0 : A_STAGE_BYTES;  // slab mode: A lives in the slab ring
+  const int stage_bytes = a_stage_bytes + b_stage_bytes;
+  uint8_t* slabs = smem + p.stages * stage_bytes;  // (stage sizes are multiples of 2 KB: slabs stay 1024-aligned)
+  uint8_t* ctrl = slabs + (p.slab_pitch ? SLAB_BUFS * SLAB_BYTES : 0);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ctrl);
   uint64_t* empty_bar = full_bar + MAX_STAGES;
   uint64_t* acc_full = empty_bar + MAX_STAGES;  // accumulator tile written (MMA warpgroups -> epilogue)
   uint64_t* acc_empty = acc_full + 1;           // accumulator tile read (epilogue -> MMA warpgroups)
+  uint64_t* slab_full = acc_empty + 1;          // slab mode: slab loaded (producer -> MMA warpgroups)
+  uint64_t* slab_empty = slab_full + SLAB_BUFS; // slab mode: slab's three taps done (MMA warps -> producer)
   float* accbuf = reinterpret_cast<float*>(ctrl + SMEM_CTRL_BYTES);
 
   if (warp == TMA_WARP && lane == 0) {
@@ -332,6 +379,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     }
     mbar_init(acc_full, MMA_THREADS);  // every thread arrives after its own accumulator stores
     mbar_init(acc_empty, EPI_THREADS);  // every thread arrives after its own accumulator reads
+    for (int s = 0; s < SLAB_BUFS; ++s) {
+      mbar_init(&slab_full[s], 1);
+      mbar_init(&slab_empty[s], MMA_WARPS);
+    }
     fence_mbar_init();
   }
   __syncthreads();
@@ -342,8 +393,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     // ===================================================================== TMA producer
     setmaxnreg_dec<PRODUCER_REGS>();
     if (warp == TMA_WARP && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      int stage = 0, slab = 0;
+      uint32_t phase = 0, slab_phase = 0;
       for (int w = unit0; w < work_total; w += nunits) {
         int tm, tn, split;
         decode_work(p, w, tm, tn, split);
@@ -358,6 +409,29 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         const int kb0 = (int)((long long)p.num_kb * split / p.split_k);
         const int kb1 = (int)((long long)p.num_kb * (split + 1) / p.split_k);
         for (int kb = kb0; kb < kb1; ++kb) {
+          if (p.slab_pitch) {
+            // kb = 9 x channel block + 3 dy + dx; the slab of (channel block, dy) serves taps dx = 0, 1, 2
+            const int dx = kb % 3, dy = kb / 3 % 3, kc0 = kb / 9 * BK;
+            if (dx == 0) {
+              mbar_wait(&slab_empty[slab], slab_phase ^ 1);
+              mbar_expect_tx(&slab_full[slab], (uint32_t)SLAB_BYTES);
+              tma_load_3d(slabs + slab * SLAB_BYTES, &tmap_a, &slab_full[slab], kc0,
+                          m0 + (dy - 1) * p.slab_pitch - 1, p.tap_plane[0]);
+            }
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            mbar_expect_tx(&full_bar[stage], (uint32_t)(p.tile_n * BK * 2));
+            tma_load_2d(smem + stage * stage_bytes, &tmap_b, &full_bar[stage], ((3 * dy + dx) * p.kb_per_tap) * BK + kc0,
+                        n0);
+            if (dx == 2 && ++slab == SLAB_BUFS) {
+              slab = 0;
+              slab_phase ^= 1;
+            }
+            if (++stage == p.stages) {
+              stage = 0;
+              phase ^= 1;
+            }
+            continue;
+          }
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * stage_bytes;
           uint8_t* sb = sa + A_STAGE_BYTES;
@@ -387,8 +461,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     }
   } else if (warp < MMA_WARPS) {
     // ===================================================================== MMA warpgroups
-    int stage = 0;
-    uint32_t phase = 0;
+    int stage = 0, slab = 0;
+    uint32_t phase = 0, slab_phase = 0;
     uint32_t acc_parity = 0;
     for (int w = unit0; w < work_total; w += nunits, acc_parity ^= 1) {
       int tm, tn, split_;
@@ -398,19 +472,22 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       const int mma_n = (n_end - n0 + 15) & ~15;  // a partial last N tile issues only its own columns
       const int kb0 = (int)((long long)p.num_kb * split_ / p.split_k);
       const int kb1 = (int)((long long)p.num_kb * (split_ + 1) / p.split_k);
-#define FVIT_MAINLOOP_N(TA, TB, BF)                                                                        \
-  gemm_mainloop_n<TA, TB, BF>(mma_n, p, smem, stage_bytes, full_bar, empty_bar, stage, phase, kb0, kb1, accbuf, \
-                              acc_full, acc_empty, acc_parity)
+#define FVIT_MAINLOOP_N(TA, TB, BF, SLAB)                                                                  \
+  gemm_mainloop_n<TA, TB, BF, SLAB>(mma_n, p, smem, stage_bytes, a_stage_bytes, full_bar, empty_bar, stage, phase, slabs, \
+                              slab_full, slab_empty, slab, slab_phase, kb0, kb1, accbuf, acc_full, acc_empty,     \
+                              acc_parity)
       if ((FEAT & EF_GENERIC) && p.bf16) {
-        if (!p.a_mn && !p.b_mn) FVIT_MAINLOOP_N(0, 0, 1);
-        else if (!p.a_mn) FVIT_MAINLOOP_N(0, 1, 1);
-        else if (!p.b_mn) FVIT_MAINLOOP_N(1, 0, 1);
-        else FVIT_MAINLOOP_N(1, 1, 1);
+        if (p.slab_pitch) FVIT_MAINLOOP_N(0, 0, 1, true);
+        else if (!p.a_mn && !p.b_mn) FVIT_MAINLOOP_N(0, 0, 1, false);
+        else if (!p.a_mn) FVIT_MAINLOOP_N(0, 1, 1, false);
+        else if (!p.b_mn) FVIT_MAINLOOP_N(1, 0, 1, false);
+        else FVIT_MAINLOOP_N(1, 1, 1, false);
       } else {
-        if (!p.a_mn && !p.b_mn) FVIT_MAINLOOP_N(0, 0, 0);
-        else if (!p.a_mn) FVIT_MAINLOOP_N(0, 1, 0);
-        else if (!p.b_mn) FVIT_MAINLOOP_N(1, 0, 0);
-        else FVIT_MAINLOOP_N(1, 1, 0);
+        if (p.slab_pitch) FVIT_MAINLOOP_N(0, 0, 0, true);
+        else if (!p.a_mn && !p.b_mn) FVIT_MAINLOOP_N(0, 0, 0, false);
+        else if (!p.a_mn) FVIT_MAINLOOP_N(0, 1, 0, false);
+        else if (!p.b_mn) FVIT_MAINLOOP_N(1, 0, 0, false);
+        else FVIT_MAINLOOP_N(1, 1, 0, false);
       }
 #undef FVIT_MAINLOOP_N
     }
@@ -819,12 +896,20 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 // (M x N x K = 27136 x 784 x 784, 27136 x 3136 x 784, 27136 x 784 x 3136, 6272 x 1568 x 1568; fv4 levels 2 and 3) on
 // an H100 SXM at 400 W; times relative to tile_n 128:
 //   tile_n 32: 1.96 / 2.47 / 3.06 / 2.76   64: 1.27 / 1.39 / 1.56 / 1.61   96: 1.09 / 1.05 / 1.14 / 1.24
+// Slab mode moves 17 KB of A per three taps instead of 16 KB per tap, and its per-column cost drops more than its
+// per-unit cost: its fixed part, 140 columns, is fitted (least squares of the log time ratios) to tile_n 32 / 64 / 96
+// / 128 timings of the two conv levels of fv4 at batch 128 (M x N x kc = 430592 x 196 x 196 and 115200 x 392 x 392,
+// 9 taps; forward with BatchNorm statistics, data gradient * GELU', data gradient + residual) on an H100 SXM at 700 W;
+// times relative to tile_n 128 (level 0 forward / dgrad, level 1 forward / dgrad):
+//   tile_n 32: 2.52 / 2.46 / 2.33 / 2.29   64: 1.55 / 1.52 / 1.33 / 1.31   96: 1.41 / 1.38 / 1.01 / 1.01
+// (The same shapes through per-tap boxes fit 88 columns: 2.23 / 2.20 / 2.04 / 2.01, 1.49 / 1.46 / 1.21 / 1.20,
+// 1.41 / 1.41 / 1.00 / 0.99.)
 // Units enumerate N tiles in decode_work's order. Cached per shape.
-static int pick_tile_n(int m, int n, int split_k, int b_ntaps, int sms) {
-  constexpr double kUnitFixed = 160.0;
+static int pick_tile_n(int m, int n, int split_k, int b_ntaps, bool slab, int sms) {
+  const double kUnitFixed = slab ? 140.0 : 160.0;
   static std::mutex mu;
-  static std::map<std::tuple<int, int, int, int, int>, int> cache;
-  const auto key = std::make_tuple(m, n, split_k, b_ntaps, sms);
+  static std::map<std::tuple<int, int, int, int, bool, int>, int> cache;
+  const auto key = std::make_tuple(m, n, split_k, b_ntaps, slab, sms);
   std::lock_guard<std::mutex> lock(mu);
   auto it = cache.find(key);
   if (it != cache.end()) return it->second;
@@ -901,7 +986,19 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   const int sms = num_sms();
   // a requested width above the widest MMA is split into two equal tiles (multiples of 16)
   const int num_kb = ceil_div(a->kc, BK) * a->ntaps;
-  int tile_n = a->tile_n > 0 ? a->tile_n : pick_tile_n(a->m, a->n, split_k < num_kb ? split_k : num_kb, b_ntaps, sms);
+  // slab mode: stride-1 3x3 taps on one plane, tap (dy, dx) shifted by (dy - 1) P + (dx - 1) rows. With one or two
+  // K blocks per tap (kc <= 128) it was not faster on H100 (fv0's C = 64 / 128 levels: 0.98 ... 1.07x the time of
+  // per-tap boxes), so those keep per-tap boxes.
+  int slab_pitch = 0;
+  if (a->ntaps == 9 && a->kc > 2 * BK && !a->a_mn_major && !a->b_mn_major && b_ntaps == 1 && split_k == 1) {
+    const int P = a->tap_shift[7] - a->tap_shift[4];
+    bool ok = P > 0;
+    for (int t = 0; t < 9 && ok; ++t)
+      ok = a->tap_plane[t] == a->tap_plane[0] && a->tap_shift[t] == (t / 3 - 1) * P + (t % 3 - 1);
+    if (ok) slab_pitch = P;
+  }
+  int tile_n = a->tile_n > 0 ? a->tile_n
+                             : pick_tile_n(a->m, a->n, split_k < num_kb ? split_k : num_kb, b_ntaps, slab_pitch > 0, sms);
   if (tile_n > MAX_TILE_N) tile_n = ceil_div(tile_n, 32) * 16;
 
   GemmParams p;
@@ -932,9 +1029,12 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   p.split_k = split_k < p.num_kb ? split_k : p.num_kb;
   if (p.split_k < 1) p.split_k = 1;
   p.atomic_out = split_k > 1 ? 1 : 0;
-  const int stage_bytes = A_STAGE_BYTES + (a->b_mn_major ? ((tile_n + 63) & ~63) : tile_n) * BK * 2;
+  p.slab_pitch = slab_pitch;
+  const int stage_bytes = (slab_pitch ? 0 : A_STAGE_BYTES) + (a->b_mn_major ? ((tile_n + 63) & ~63) : tile_n) * BK * 2;
+  const int slab_bytes = slab_pitch ? SLAB_BUFS * SLAB_BYTES : 0;
   const int stats_bytes = a->col_sum ? SMEM_STATS_BYTES : (a->out_colsum ? 256 * 4 : 0);
-  int stages = (SMEM_BUDGET - SMEM_CTRL_BYTES - SMEM_ALIGN_SLACK - SMEM_ACC_BYTES - stats_bytes) / stage_bytes;
+  int stages =
+      (SMEM_BUDGET - SMEM_CTRL_BYTES - SMEM_ALIGN_SLACK - SMEM_ACC_BYTES - stats_bytes - slab_bytes) / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   FVIT_CHECK(stages >= 2, "fvit_gemm: not enough shared memory for 2 stages");
   p.stages = stages;
@@ -987,7 +1087,8 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
     const int planes = a->a_planes > 0 ? a->a_planes : 1;
     rc = get_tmap(&tma, a->a, (uint64_t)a->kc, (uint64_t)a->a_rows, (uint64_t)planes,
                   (uint64_t)a->lda * 2,
-                  (uint64_t)(planes > 1 ? a->a_plane_stride : a->a_rows * a->lda) * 2, BK, BM, 3);
+                  (uint64_t)(planes > 1 ? a->a_plane_stride : a->a_rows * a->lda) * 2, BK,
+                  slab_pitch ? SLAB_ROWS : BM, 3);
   } else {
     rc = get_tmap(&tma, a->a, (uint64_t)a->m, (uint64_t)a->a_rows, 1, (uint64_t)a->lda * 2,
                   (uint64_t)a->a_rows * a->lda * 2, 64, BK, 3);
@@ -1003,7 +1104,8 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   }
   if (rc) return rc;
 
-  const int smem_bytes = stages * stage_bytes + SMEM_CTRL_BYTES + SMEM_ALIGN_SLACK + SMEM_ACC_BYTES + stats_bytes;
+  const int smem_bytes =
+      stages * stage_bytes + slab_bytes + SMEM_CTRL_BYTES + SMEM_ALIGN_SLACK + SMEM_ACC_BYTES + stats_bytes;
   const long long work = (long long)p.tiles_m * p.tiles_n * p.split_k;
   const int grid = (int)(work < sms ? work : sms);
   // feature mask of this call; launch the matching specialisation if one was instantiated

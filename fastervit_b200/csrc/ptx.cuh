@@ -95,6 +95,9 @@ __device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.s
 // Shared-memory matrix descriptor (64 bit):
 //  [0,14) start address >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte offset >> 4
 //  [49,52) base offset | [62,64) layout (0 none, 1 128B, 2 64B, 3 32B swizzle)
+// The base offset stays 0: the swizzle phase of a row comes from the address bits themselves, so a K-major SW128
+// matrix may start at any 128-byte row of a buffer that TMA wrote from a 1024-byte boundary (measured on H100:
+// setting the field to (start >> 7) & 7 for such a start shifts the phase twice and gives wrong products).
 // K-major SW128: SBO = 1024 (8 rows x 128 B), LBO unused; MN-major SW128: LBO = next 64-wide MN atom, SBO = next
 // 8 K rows. The SWZ_* values below are the layout field shifted to bit 61.
 enum : uint32_t { SWZ_NONE = 0, SWZ_128B = 2, SWZ_64B = 4, SWZ_32B = 6 };
