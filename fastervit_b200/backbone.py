@@ -7,7 +7,8 @@ mask resized to every level (fastervit.py:829-846), frozen stages (fastervit.py:
 The hot path is the same sm_90a launch list as classification: in eval the wrapped model's eval plan is run up to the
 points where the level outputs are live and `fvit_feature_map_fwd` applies the level's folded BatchNorm while
 converting the token-major activation to NCHW. In train mode a levels-mode train plan (engine_train.py) applies each
-norm{i} with batch statistics and differentiates through it (`fvit_feature_map_bwd`). Variable input sizes go through the any-res entrypoints (one cached plan per shape; the
+norm{i} with batch statistics and differentiates through it (`fvit_feature_map_bwd`); a grad-enabled eval forward is
+differentiable through the running-statistics norms (`fvit_feature_map_eval_bwd`, engine_train._EvalDenseGradFunction). Variable input sizes go through the any-res entrypoints (one cached plan per shape; the
 level geometry is padded to window multiples exactly as faster_vit_any_res.py:851-867 does).
 """
 from __future__ import annotations
@@ -15,7 +16,6 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from . import lib as L
 from .registry import create_model
 
 
@@ -58,29 +58,12 @@ class FasterViTBackbone(nn.Module):
         """fastervit.py:816-827: tuple of the normalised level outputs, NCHW. Under .train() (detector fine-tuning,
         dino/backbone.py:158-160) the body runs its training launch list up to the highest requested level, every
         norm{i} normalises with batch statistics (running statistics updated) and the outputs are differentiable;
-        the frozen prefix runs on running statistics and gets no gradient."""
-        if self.training:
-            norms = [getattr(self, f"norm{i}") for i in self.out_indices]
-            return self.body._get_engine().forward_levels(x, self.out_indices, norms=norms,
-                                                          frozen_stages=self.frozen_stages)
-        with torch.no_grad():
-            return self._forward_raw_eval(x)
-
-    def _forward_raw_eval(self, x: torch.Tensor) -> tuple:
-        feats = self.body.forward_levels(x, self.out_indices)
-        outs = []
-        for idx, f in zip(self.out_indices, feats):
-            bn: nn.BatchNorm2d = getattr(self, f"norm{idx}")
-            B, C, H, W = f.shape
-            scale = (bn.weight * torch.rsqrt(bn.running_var + bn.eps)).float().contiguous()
-            shift = (bn.bias - bn.running_mean * scale).float().contiguous()
-            rows = f.permute(0, 2, 3, 1).reshape(B * H * W, C).contiguous()     # token-major view of the level output
-            out = torch.empty(B, C, H, W, dtype=torch.float32, device=f.device)
-            with torch.cuda.device(f.device):
-                L.call("fvit_feature_map_fwd", rows.data_ptr(), C, None, B, H * W, C, scale.data_ptr(), shift.data_ptr(),
-                       out.data_ptr())
-            outs.append(out)
-        return tuple(outs)
+        the frozen prefix runs on running statistics and gets no gradient. Under .eval() every norm{i} uses its running
+        statistics; with grad enabled the outputs are differentiable too (norm-eval fine-tuning, perceptual losses:
+        parameter gradients, and the image gradient when x requires grad), and a forward without backward costs what
+        the inference forward costs."""
+        norms = [getattr(self, f"norm{i}") for i in self.out_indices]
+        return self.body._get_engine().forward_levels(x, self.out_indices, norms=norms, frozen_stages=self.frozen_stages)
 
     def forward(self, tensors: torch.Tensor, mask: torch.Tensor | None = None) -> dict:
         """fastervit.py:829-846 without the NestedTensor wrapper type: {idx: (features, mask resized to the level)}."""

@@ -119,6 +119,46 @@ feature_map_bwd_apply_kernel(const float* __restrict__ dy, const float* __restri
   }
 }
 
+// The same transposes for a running-statistics BatchNorm (eval mode): the map gradient is a per-channel scale of dy, so
+// the apply reads dy and read-modify-writes g, and never touches xs (no mean(dy) / mean(dy*xhat) terms). With no xs
+// stream to overlap, a block takes 32 channels x 64 tokens and every thread issues its 8 dy loads, then its 8 g loads,
+// before any store: enough bytes in flight per SM for the HBM-bound pass.
+constexpr int kEvalTok = 64;
+__global__ void __launch_bounds__(256)
+feature_map_eval_bwd_apply_kernel(const float* __restrict__ dy, const int* __restrict__ row_map, int T, int C,
+                                  const float* __restrict__ rstd, const float* __restrict__ w,
+                                  const float* __restrict__ gs, float* __restrict__ g, long long ldg) {
+  __shared__ float tile[32][kEvalTok + 1];
+  const int b = blockIdx.z, t0 = blockIdx.x * kEvalTok, c0 = blockIdx.y * 32;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int i = threadIdx.y + 8 * k, c = c0 + i;
+#pragma unroll
+    for (int h = 0; h < kEvalTok / 32; ++h) {
+      const int t = t0 + 32 * h + threadIdx.x;
+      tile[i][32 * h + threadIdx.x] = (t < T && c < C) ? dy[((long long)b * C + c) * T + t] : 0.f;
+    }
+  }
+  __syncthreads();
+  const int c = c0 + threadIdx.x;
+  if (c >= C) return;
+  float k1 = __ldg(gs);
+  if (w) k1 = k1 * __ldg(w + c) * __ldg(rstd + c);
+  constexpr int kPer = kEvalTok / 8;
+  long long row[kPer];
+  float gv[kPer];
+#pragma unroll
+  for (int k = 0; k < kPer; ++k) {
+    const int t = t0 + threadIdx.y + 8 * k;
+    row[k] = t < T ? (row_map ? (long long)row_map[(long long)b * T + t] : (long long)b * T + t) : -1;
+  }
+#pragma unroll
+  for (int k = 0; k < kPer; ++k) gv[k] = row[k] >= 0 ? g[row[k] * ldg + c] : 0.f;
+#pragma unroll
+  for (int k = 0; k < kPer; ++k)
+    if (row[k] >= 0) g[row[k] * ldg + c] = gv[k] + k1 * tile[threadIdx.x][threadIdx.y + 8 * k];
+}
+
 // dw[c] += s2[c] * scalar, dbeta[c] += s1[c] * scalar
 __global__ void bn_affine_grad_kernel(const float* __restrict__ s1, const float* __restrict__ s2,
                                       const float* __restrict__ scalar, int C, float* __restrict__ dw,
@@ -138,6 +178,67 @@ __global__ void grad_scale_finalize_kernel(const float* __restrict__ amax, float
   S = fminf(fmaxf(S, 1.f / 16777216.f), 16777216.f * 65536.f);
   gs[0] = S;
   gs[1] = 1.f / S;
+}
+
+// ---- backward of forward_head (avg-pool + Linear) in fp32
+// pooled[r] = mean_t x[r][t] over rows r = b*C + c of an NCHW map: one warp per row, lanes along t
+__global__ void nchw_row_mean_kernel(const float* __restrict__ x, long long rows, int T, float* __restrict__ pooled) {
+  const long long r = (long long)blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+  if (r >= rows) return;
+  const int lane = threadIdx.x & 31;
+  float s = 0.f;
+  for (int t = lane; t < T; t += 32) s += x[r * T + t];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) pooled[r] = s / (float)T;
+}
+
+// dfeats[b][c][t] = (sum_k dl[b][k] * W[k][c]) / T (W NULL: dl[b][c] / T). grid = (channel tiles of 128, B); the
+// dlogits row is staged in shared memory in chunks, W is read along c (coalesced); the block's [128 x T] output slab
+// is contiguous in NCHW and written linearly.
+__global__ void __launch_bounds__(128)
+head_eval_dgrad_kernel(const float* __restrict__ dl, long long ldl, int ncls, const float* __restrict__ W, int C, int T,
+                       float* __restrict__ dfeats) {
+  __shared__ float dls[128];
+  __shared__ float dps[128];
+  const int b = blockIdx.y, c0 = blockIdx.x * 128, c = c0 + threadIdx.x;
+  float acc = 0.f;
+  if (W) {
+    for (int k0 = 0; k0 < ncls; k0 += 128) {
+      __syncthreads();
+      dls[threadIdx.x] = (k0 + threadIdx.x < ncls) ? dl[b * ldl + k0 + threadIdx.x] : 0.f;
+      __syncthreads();
+      if (c < C) {
+        const int kn = min(128, ncls - k0);
+        for (int j = 0; j < kn; ++j) acc = fmaf(dls[j], __ldg(W + (long long)(k0 + j) * C + c), acc);
+      }
+    }
+  } else if (c < C) {
+    acc = dl[b * ldl + c];
+  }
+  dps[threadIdx.x] = acc / (float)T;
+  __syncthreads();
+  const long long n = (long long)min(128, C - c0) * T;
+  float* out = dfeats + ((long long)b * C + c0) * T;
+  for (long long i = threadIdx.x; i < n; i += 128) out[i] = dps[i / T];
+}
+
+// dW[k][c] += sum_b dl[b][k] * pooled[b][c]; db[k] += sum_b dl[b][k]. grid = (channel tiles of 128, ncls): pooled is
+// read along c (coalesced), the dlogits column value is the same for the whole block.
+__global__ void __launch_bounds__(128)
+head_eval_wgrad_kernel(const float* __restrict__ dl, long long ldl, int B, const float* __restrict__ pooled, int C,
+                       float* __restrict__ dW, float* __restrict__ db) {
+  const int k = blockIdx.y, c = blockIdx.x * 128 + threadIdx.x;
+  if (c < C) {
+    float acc = 0.f;
+    for (int b = 0; b < B; ++b) acc = fmaf(__ldg(dl + b * ldl + k), __ldg(pooled + (long long)b * C + c), acc);
+    dW[(long long)k * C + c] += acc;
+  }
+  if (db && blockIdx.x == 0 && threadIdx.x == 0) {
+    float s = 0.f;
+    for (int b = 0; b < B; ++b) s += dl[b * ldl + k];
+    db[k] += s;
+  }
 }
 
 }  // namespace fvit
@@ -185,6 +286,61 @@ int fvit_feature_map_bwd(const float* dy, const float* xs, int64_t ldx, const in
   if (dw) {
     bn_affine_grad_kernel<<<ceil_div(C, 128), 128, 0, (cudaStream_t)stream>>>(s1, s2, scalar, C, dw, dbeta);
     return post_launch("bn_affine_grad_kernel");
+  }
+  return 0;
+}
+
+int fvit_feature_map_eval_bwd(const float* dy, const int32_t* row_map, int32_t B, int32_t T, int32_t C,
+                              const float* rstd, const float* w, const float* s1, const float* s2, const float* gs,
+                              const float* scalar, float* g, int64_t ldg, float* dw, float* dbeta, void* stream) {
+  FVIT_CHECK(B > 0 && T > 0 && C > 0 && B <= 65535, "fvit_feature_map_eval_bwd: bad arguments");
+  FVIT_CHECK((w == nullptr) == (rstd == nullptr), "fvit_feature_map_eval_bwd: w and rstd come in pairs");
+  FVIT_CHECK(!g || (dy && gs), "fvit_feature_map_eval_bwd: the map gradient needs dy and gs");
+  FVIT_CHECK((dw == nullptr) == (dbeta == nullptr) && (!dw || (w && s1 && s2)), "fvit_feature_map_eval_bwd: dw / dbeta "
+             "come in pairs and need the BatchNorm mode (w, rstd) and s1, s2");
+  if (g) {
+    dim3 grid((T + kEvalTok - 1) / kEvalTok, (C + 31) / 32, B);
+    feature_map_eval_bwd_apply_kernel<<<grid, dim3(32, 8), 0, (cudaStream_t)stream>>>(dy, row_map, T, C, rstd, w, gs,
+                                                                                       g, ldg);
+    const int rc = post_launch("feature_map_eval_bwd_apply_kernel");
+    if (rc) return rc;
+  }
+  if (dw) {
+    bn_affine_grad_kernel<<<ceil_div(C, 128), 128, 0, (cudaStream_t)stream>>>(s1, s2, scalar, C, dw, dbeta);
+    return post_launch("bn_affine_grad_kernel");
+  }
+  return 0;
+}
+
+int fvit_head_eval_bwd(const float* dlogits, int64_t ldl, int32_t B, int32_t ncls, const float* feats, int32_t C,
+                       int32_t T, const float* W, float* pooled_ws, float* dfeats, float* dW, float* db, void* stream) {
+  FVIT_CHECK(dlogits && B > 0 && ncls > 0 && C > 0 && T > 0 && B <= 65535 && ncls <= 65535,
+             "fvit_head_eval_bwd: bad arguments");
+  FVIT_CHECK(W || ncls == C, "fvit_head_eval_bwd: an identity head (W NULL) has ncls == C");
+  FVIT_CHECK(ldl >= ncls, "fvit_head_eval_bwd: ldl < ncls");
+  FVIT_CHECK(!dW || (W && feats && (T == 1 || pooled_ws)), "fvit_head_eval_bwd: dW needs W, feats and (T > 1) pooled_ws");
+  FVIT_CHECK(!db || W, "fvit_head_eval_bwd: db needs a Linear head");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dfeats) {
+    head_eval_dgrad_kernel<<<dim3(ceil_div(C, 128), B), 128, 0, st>>>(dlogits, ldl, ncls, W, C, T, dfeats);
+    const int rc = post_launch("head_eval_dgrad_kernel");
+    if (rc) return rc;
+  }
+  if (dW) {
+    const float* pooled = feats;
+    if (T > 1) {
+      const long long rows = (long long)B * C;
+      nchw_row_mean_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(feats, rows, T, pooled_ws);
+      const int rc = post_launch("nchw_row_mean_kernel");
+      if (rc) return rc;
+      pooled = pooled_ws;
+    }
+    head_eval_wgrad_kernel<<<dim3(ceil_div(C, 128), ncls), 128, 0, st>>>(dlogits, ldl, B, pooled, C, dW, db);
+    return post_launch("head_eval_wgrad_kernel");
+  }
+  if (db) {   // (a bias without a weight gradient: the column sums alone, through the same kernel with no channels)
+    head_eval_wgrad_kernel<<<dim3(1, ncls), 128, 0, st>>>(dlogits, ldl, B, nullptr, 0, nullptr, db);
+    return post_launch("head_eval_wgrad_kernel");
   }
   return 0;
 }

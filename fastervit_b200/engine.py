@@ -965,7 +965,10 @@ class Engine:
                     return _FasterViTFunction.apply(plan, x, *plan.params)
                 return plan.run_forward(x).clone()
         params = self._params
-        if not features_only and torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params)):
+        if features_only:
+            # forward_features: the `norm`-ed last-level map, differentiable like forward_levels
+            return self._eval_dense(x, ((len(self.model.levels) - 1, self.model.norm),), -1, features=True)[0]
+        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params)):
             # differentiable eval forward: the inference launch list as below, the backward recomputes it
             # (engine_train._EvalGradFunction)
             from .engine_train import _EvalGradFunction
@@ -1014,16 +1017,79 @@ class Engine:
         return plan.logits.clone()
 
     def forward_levels(self, x: torch.Tensor, out_indices: tuple, norms=None, frozen_stages: int = -1) -> tuple:
-        """Each requested level's output before its Downsample as an NCHW fp32 map. Eval: the inference launch list is
-        run piecewise up to the marks where those activations are live (`norms` / `frozen_stages` are not used there).
-        Train: a levels-mode train plan, differentiable; `norms` = one BatchNorm2d (or None) per index applied with
-        batch statistics, `frozen_stages` = the backbone's frozen prefix (fastervit.py:801-812)."""
+        """Each requested level's output before its Downsample as an NCHW fp32 map; `norms` = one BatchNorm2d (or None)
+        per index, `frozen_stages` = the backbone's frozen prefix (fastervit.py:801-812).
+        Eval: the inference launch list is run piecewise up to the marks where those activations are live, and each
+        norm is applied with its running statistics. With grad enabled and the image or a parameter on the outputs'
+        path requiring grad, the outputs are differentiable (engine_train._EvalDenseGradFunction).
+        Train: a levels-mode train plan, differentiable; the norms use batch statistics."""
+        norms = tuple(norms) if norms is not None else (None,) * len(out_indices)
+        if len(norms) != len(out_indices) or (self.model.training and not out_indices):
+            raise L.FvitError("forward_levels: give one norm (or None) per requested level, and at least one level")
+        outs = tuple(zip(out_indices, norms))
         if self.model.training:
-            norms = tuple(norms) if norms is not None else (None,) * len(out_indices)
-            if len(norms) != len(out_indices) or not out_indices:
-                raise L.FvitError("forward_levels: give one norm (or None) per requested level, and at least one level")
-            return self._dense_train(x, dict(kind="levels", outs=tuple(zip(out_indices, norms)), frozen=int(frozen_stages)))
+            return self._dense_train(x, dict(kind="levels", outs=outs, frozen=int(frozen_stages)))
+        if not outs:
+            return self._eval_levels(self._plan(x), x, ())
+        return self._eval_dense(x, outs, int(frozen_stages), features=False)
+
+    def _eval_dense(self, x: torch.Tensor, outs: tuple, frozen: int, features: bool) -> tuple:
+        """Eval-mode dense outputs (forward_levels, forward_features): the inference launch list, wrapped in an
+        autograd node when a gradient can flow (nothing is built for it until its backward runs)."""
         plan = self._plan(x)
+        params = self._dense_params(outs)
+        if torch.is_grad_enabled() and (x.requires_grad or self._path_requires_grad(outs, params)):
+            from .engine_train import _EvalDenseGradFunction
+            return _EvalDenseGradFunction.apply(self, plan, (outs, frozen, features), x, *params)
+        return self._eval_dense_fwd(plan, x, outs, features)
+
+    def _dense_params(self, outs: tuple) -> list:
+        """the parameters an eval levels plan of these outputs hands gradients to, in its flat-buffer order
+        (TrainPlan._setup_train): the model's, then the level norms that are not the model's own (the backbone's)"""
+        params = list(self._params)
+        known = {id(p) for p in params}
+        for _, bn in outs:
+            for p in (() if bn is None else (bn.weight, bn.bias)):
+                if id(p) not in known:
+                    known.add(id(p))
+                    params.append(p)
+        return params
+
+    def _path_requires_grad(self, outs: tuple, params: list) -> bool:
+        from .engine_train import levels_path
+        on = levels_path(self.model, outs)
+        return any(p.requires_grad for p in params if id(p) in on)
+
+    def _eval_dense_fwd(self, plan: Plan, x: torch.Tensor, outs: tuple, features: bool) -> tuple:
+        if features:
+            return (self._run_eval(plan, x, features_only=True),)
+        feats = self._eval_levels(plan, x, tuple(i for i, _ in outs))
+        if all(bn is None for _, bn in outs):
+            return feats
+        res = []
+        for (idx, bn), f in zip(outs, feats):
+            if bn is None:
+                res.append(f)
+                continue
+            # the level norm folded into the layout-conversion kernel, running statistics (fastervit.py:816-827)
+            B, C, H, W = f.shape
+            scale = (bn.weight * torch.rsqrt(bn.running_var + bn.eps)).float().contiguous()
+            shift = (bn.bias - bn.running_mean * scale).float().contiguous()
+            rows = f.permute(0, 2, 3, 1).reshape(B * H * W, C).contiguous()     # token-major view of the level output
+            out = torch.empty(B, C, H, W, dtype=torch.float32, device=f.device)
+            with torch.cuda.device(f.device):
+                L.call("fvit_feature_map_fwd", rows.data_ptr(), C, None, B, H * W, C, scale.data_ptr(), shift.data_ptr(),
+                       out.data_ptr())
+            res.append(out)
+        return tuple(res)
+
+    def eval_dense_plan(self, x: torch.Tensor, outs: tuple, frozen: int) -> Plan:
+        """The plan the backward of a differentiable eval-mode dense output runs (built at the first such backward): a
+        levels-mode TrainPlan whose BatchNorms (the level norms too) use their running statistics; with frozen = -1 its
+        backward also writes the image gradient."""
+        return self._plan(x, dict(kind="levels", outs=outs, frozen=frozen, eval=True))
+
+    def _eval_levels(self, plan: Plan, x: torch.Tensor, out_indices: tuple) -> tuple:
         with torch.cuda.device(x.device):
             wk = plan.weights_key()
             if self._prepped.get(id(plan)) != wk:
@@ -1041,7 +1107,9 @@ class Engine:
 
     def forward_head(self, feats: torch.Tensor) -> torch.Tensor:
         """avgpool + flatten + head (fv.py:955-958) on the [B, C, H, W] map `forward_features` returns (an already
-        pooled [B, C] tensor is accepted too), eval mode: pooling kernel + one fvit_gemm."""
+        pooled [B, C] tensor is accepted too), eval mode: pooling kernel + one fvit_gemm. With grad enabled and the
+        features or the head's parameters requiring grad, the output is differentiable (engine_train._EvalHeadFunction:
+        fvit_head_eval_bwd, fp32)."""
         m = self.model
         if m.training and torch.is_grad_enabled():
             raise L.FvitError("forward_head is an inference helper; the autograd training path is forward()")
@@ -1050,6 +1118,14 @@ class Engine:
             raise L.FvitError(f"forward_head expects a CUDA float32 [B, {m.num_features}, H, W] (or pooled [B, "
                               f"{m.num_features}]) tensor, got {tuple(feats.shape)} {feats.dtype} on {feats.device}")
         self._check_weights()
+        params = tuple(m.head.parameters()) if isinstance(m.head, nn.Linear) else ()
+        if torch.is_grad_enabled() and (feats.requires_grad or any(p.requires_grad for p in params)):
+            from .engine_train import _EvalHeadFunction
+            return _EvalHeadFunction.apply(self, feats, *params)
+        return self._head_fwd(feats)
+
+    def _head_fwd(self, feats: torch.Tensor) -> torch.Tensor:
+        m = self.model
         with torch.cuda.device(feats.device):
             nf, Bf = m.num_features, feats.shape[0]
             ld = _ru(nf, 8)

@@ -26,6 +26,24 @@ from .engine_train_conv import ConvPartEmitters
 from .engine_train_levels import TokenLevelEmitters
 
 
+def levels_path(model, outs) -> set[int]:
+    """ids of the parameters the level outputs `outs` ((level, BatchNorm2d or None), ...) depend on: the stem, the levels
+    up to the highest requested one without its Downsample, and the level norms"""
+    stop = max(i for i, _ in outs)
+    on = set()
+    for name, p in model.named_parameters():
+        if name.startswith("levels."):
+            li = int(name.split(".")[1])
+            if li < stop or (li == stop and not name.startswith(f"levels.{li}.downsample.")):
+                on.add(id(p))
+        elif name.startswith("patch_embed."):
+            on.add(id(p))
+    for _, bn in outs:
+        if bn is not None:
+            on.update((id(bn.weight), id(bn.bias)))
+    return on
+
+
 def _sm_count() -> int:
     """SMs of the current device; plans built without one (host-side tests) assume an H100 SXM's 132."""
     if torch.cuda.is_available():
@@ -117,22 +135,9 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         """ids of the parameters the requested outputs depend on (the rest get no gradient: .grad stays None, as under
         autograd). Levels mode: the stem and levels up to the highest requested one without its Downsample, the level
         norms; not the frozen prefix, nor `norm` / `head` unless forward_features asked for `norm`."""
-        m = self.model
         if self.kind != "levels":
             return {id(p) for p in self.params}
-        on = set()
-        outs = self.spec["outs"]
-        for name, p in m.named_parameters():
-            if name.startswith("levels."):
-                li = int(name.split(".")[1])
-                if li < self.stop_level or (li == self.stop_level and not name.startswith(f"levels.{li}.downsample.")):
-                    on.add(id(p))
-            elif name.startswith("patch_embed."):
-                on.add(id(p))
-        for _, bn in outs:
-            if bn is not None:
-                on.update((id(bn.weight), id(bn.bias)))
-        return on - self._frozen_params
+        return levels_path(self.model, self.spec["outs"]) - self._frozen_params
 
     def grad_views_on_path(self) -> list:
         """grad_views() with None for the parameters off the path of the requested outputs"""
@@ -632,19 +637,7 @@ class _EvalGradFunction(torch.autograd.Function):
     def backward(ctx, gout):
         (x,) = ctx.saved_tensors
         engine, plan = ctx.engine, ctx.plan
-        m = engine.model
-        if plan.weights_key() != ctx.weights_key:
-            raise L.FvitError(
-                "backward of an eval-mode forward after a weight change: this model's parameters or buffers changed, "
-                "or any model's fused optimizer step, EMA update or train-mode forward ran in between (those write "
-                "through raw pointers and advance one library-wide epoch, so they count even for another model); the "
-                "recomputed forward might not be the one that ran: call backward before them")
-        if getattr(m, "_grad_allreduce", None) is not None:
-            raise L.FvitError("eval-mode gradients are not all-reduced across ranks: the gradient all-reduce "
-                              "(enable_grad_allreduce) only covers train-mode steps")
-        if any(getattr(mod, "deploy", False) for mod in m.modules()):
-            raise L.FvitError("eval-mode gradients need the relative-position-bias MLPs: a module was switched to "
-                              "deploy mode (switch_to_deploy caches their output), so they have no gradient path")
+        _check_eval_backward(engine.model, plan.weights_key() != ctx.weights_key)
         with torch.cuda.device(x.device):
             gp = engine.eval_grad_plan(x)
             gp.run_forward(x)
@@ -652,3 +645,100 @@ class _EvalGradFunction(torch.autograd.Function):
             gp.run_backward(g if gp.kind is None else [g])
             dx = gp.dx.clone() if ctx.needs_input_grad[2] else None
             return (None, None, dx, *gp.grad_views())
+
+
+def _check_eval_backward(m, weights_changed: bool, recomputes: bool = True) -> None:
+    """what makes the recompute of an eval-mode forward impossible or different from the forward that ran
+    (recomputes=False: a backward that reads only its saved input and the head, where deploy mode does not matter)"""
+    if weights_changed:
+        raise L.FvitError(
+            "backward of an eval-mode forward after a weight change: this model's parameters or buffers changed, "
+            "or any model's fused optimizer step, EMA update or train-mode forward ran in between (those write "
+            "through raw pointers and advance one library-wide epoch, so they count even for another model); the "
+            "recomputed forward might not be the one that ran: call backward before them")
+    if getattr(m, "_grad_allreduce", None) is not None:
+        raise L.FvitError("eval-mode gradients are not all-reduced across ranks: the gradient all-reduce "
+                          "(enable_grad_allreduce) only covers train-mode steps")
+    if recomputes and any(getattr(mod, "deploy", False) for mod in m.modules()):
+        raise L.FvitError("eval-mode gradients need the relative-position-bias MLPs: a module was switched to "
+                          "deploy mode (switch_to_deploy caches their output), so they have no gradient path")
+
+
+def _norm_versions(outs) -> tuple:
+    """autograd versions of the level norms' tensors (the backbone's norm{i} are not part of the model's weights key)"""
+    return tuple(t._version for _, bn in outs if bn is not None
+                 for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
+
+
+class _EvalDenseGradFunction(torch.autograd.Function):
+    """Autograd node of grad-enabled eval()-mode dense outputs: forward_levels, forward_features and the backbone's
+    forward_raw. forward runs the inference extraction unchanged (bitwise the no_grad outputs) and keeps x. backward
+    recomputes through the eval levels plan (Engine.eval_dense_plan: a levels-mode TrainPlan with every BatchNorm, the
+    level norms included, on running statistics and no stochastic depth), loads the output gradients (an unused output
+    is a zero gradient) and runs its backward. When x needs a gradient the plan is built without a frozen prefix
+    (frozen = -1): in eval mode the prefix computes the same arithmetic, and its weight gradients are computed and then
+    dropped (None for parameters that do not require grad) -- the price of the image gradient through it. Guards and
+    first-order restriction as _EvalGradFunction."""
+
+    @staticmethod
+    def forward(ctx, engine, plan, spec, x: torch.Tensor, *params):
+        outs, frozen, features = spec
+        ctx.engine, ctx.plan, ctx.outs, ctx.frozen, ctx.params = engine, plan, outs, frozen, params
+        res = engine._eval_dense_fwd(plan, x, outs, features)
+        ctx.weights_key = (engine._prepped[id(plan)], _norm_versions(outs))
+        ctx.save_for_backward(x)
+        ctx.set_materialize_grads(False)   # (an unused output stays None: the plan zeroes its gradient buffer)
+        return res
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, *grads):
+        (x,) = ctx.saved_tensors
+        engine, plan = ctx.engine, ctx.plan
+        _check_eval_backward(engine.model, (plan.weights_key(), _norm_versions(ctx.outs)) != ctx.weights_key)
+        want_dx = ctx.needs_input_grad[3]
+        with torch.cuda.device(x.device):
+            gp = engine.eval_dense_plan(x, ctx.outs, -1 if want_dx else ctx.frozen)
+            if len(gp.params) != len(ctx.params) or any(a is not b for a, b in zip(gp.params, ctx.params)):
+                raise L.FvitError("the model's parameters changed between an eval-mode forward and its backward")
+            gp.run_forward(x)
+            gp.run_backward([None if g is None else g.contiguous().float() for g in grads])
+            dx = gp.dx.clone() if want_dx else None
+            views = [g if p.requires_grad else None for p, g in zip(gp.params, gp.grad_views_on_path())]
+            return (None, None, None, dx, *views)
+
+
+class _EvalHeadFunction(torch.autograd.Function):
+    """Autograd node of forward_head under .eval(): forward is the inference helper (fp16 pooling + GEMM) unchanged;
+    backward is fvit_head_eval_bwd in fp32 -- the feature gradient through the pooling and the Linear, the head's weight
+    gradient from the pooled features recomputed from the saved input, and the bias gradient. First order only."""
+
+    @staticmethod
+    def forward(ctx, engine, feats: torch.Tensor, *params):
+        ctx.engine = engine
+        ctx.key = (tuple(p._version for p in params), L.weights_epoch())
+        ctx.save_for_backward(feats)
+        return engine._head_fwd(feats)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gout):
+        (feats,) = ctx.saved_tensors
+        m = ctx.engine.model
+        head = m.head if isinstance(m.head, torch.nn.Linear) else None
+        params = tuple(head.parameters()) if head is not None else ()
+        _check_eval_backward(m, (tuple(p._version for p in params), L.weights_epoch()) != ctx.key, recomputes=False)
+        B, nf = feats.shape[0], m.num_features
+        T = feats.shape[2] * feats.shape[3] if feats.dim() == 4 else 1
+        dl = gout.contiguous().float()
+        dev = feats.device
+        want = ctx.needs_input_grad
+        f32 = feats.contiguous()
+        dfeats = torch.empty(f32.shape, dtype=torch.float32, device=dev) if want[1] else None
+        dW = torch.zeros_like(head.weight) if head is not None and want[2] else None
+        db = torch.zeros_like(head.bias) if head is not None and head.bias is not None and want[3] else None
+        ws = torch.empty(B * nf, dtype=torch.float32, device=dev) if dW is not None and T > 1 else None
+        with torch.cuda.device(dev):
+            L.call("fvit_head_eval_bwd", dl.data_ptr(), dl.stride(0), B, dl.shape[1], f32.data_ptr(), nf, T,
+                   head.weight.data_ptr() if head is not None else None, L.ptr(ws), L.ptr(dfeats), L.ptr(dW), L.ptr(db))
+        return (None, dfeats, dW, db)[:2 + len(params)]

@@ -100,7 +100,10 @@ def _emit_dense_outputs(self) -> None:
     """Levels mode forward tail: every requested level output (x before its Downsample, live in the level's buffer
     until the plan's next forward: the backward never writes it) as an NCHW fp32 map in a static buffer, through its
     BatchNorm2d with batch statistics (fvit_colstats_pivot_f32 -> fvit_bn_finalize_pivot, which also updates the running
-    statistics -> fvit_feature_map_fwd), or raw."""
+    statistics -> fvit_feature_map_fwd), or raw.
+    Eval plan (engine_train._EvalDenseGradFunction): the outputs come from the inference launch list, so this forward
+    writes no output map; it only keeps each norm's running mean / rstd for the backward's xhat (one fvit_affine_fold
+    with unit weight and zero bias: rstd = rsqrt(running_var + eps), nothing updated)."""
     B, nb = self.B, self.bufs
     self.dense, self.outputs = [], []
     tot = 1
@@ -109,13 +112,24 @@ def _emit_dense_outputs(self) -> None:
         x, rows = _level_rows(lv)
         C, H, W = lv["C"], lv["H"], lv["W"]
         T = H * W
-        out = nb.new(f"dense.out{k}", (B, C, H, W), torch.float32)
+        out = None if self.eval_grad else nb.new(f"dense.out{k}", (B, C, H, W), torch.float32)
         d = dict(level=i, lv=lv, x=x, rows=rows, C=C, T=T, bn=bn, out=out,
                  dy=nb.new(f"dense.dy{k}", (B, C, H, W), torch.float32), acc=tot)
         tot += 2 * _ru(C, 4)
+        if bn is not None and bn.num_features != C:
+            raise L.FvitError(f"the norm of level {i} has {bn.num_features} features, the level has {C} channels")
+        if self.eval_grad:
+            if bn is not None:
+                rs = nb.new(f"dense.norm{k}.rstd", (C,), torch.float32)
+                self._op(self.ops, "fvit_affine_fold", rs.data_ptr(), nb.new(f"dense.norm{k}.nshift", (C,), torch.float32).data_ptr(),
+                         C, _const_vec(self, 1.0, C).data_ptr(), _const_vec(self, 0.0, C).data_ptr(),
+                         bn.running_mean.data_ptr(), bn.running_var.data_ptr(), float(bn.eps), None, None)
+                d.update(mu=bn.running_mean, rs=rs)
+            else:
+                d.update(mu=None, rs=None)
+            self.dense.append(d)
+            continue
         if bn is not None:
-            if bn.num_features != C:
-                raise L.FvitError(f"the norm of level {i} has {bn.num_features} features, the level has {C} channels")
             st = self._bn_train(f"dense.norm{k}", bn, B * T)
             self._op(self.ops, "fvit_colstats_pivot_f32", x.data_ptr(), C, rows.data_ptr(), B * T, C, st["pivot"].data_ptr(),
                      st["st"][0].data_ptr(), st["st"][1].data_ptr())
@@ -152,6 +166,13 @@ def _inject(self, level: int, g=True) -> None:
             continue
         bn, lv = d["bn"], d["lv"]
         if bn is None and not g:
+            continue
+        if self.eval_grad:   # running statistics: a per-channel scale of dy, and dw / dbeta straight from the stats pass
+            self._op(self.bwd_ops, "fvit_feature_map_eval_bwd", d["dy"].data_ptr(), d["rows"].data_ptr(), self.B, d["T"],
+                     d["C"], P(d["rs"]), bn.weight.data_ptr() if bn is not None else None,
+                     d["s1"] if bn is not None else None, d["s2"] if bn is not None else None, ("scal", 0), None,
+                     lv["g"].data_ptr() if g else None, d["C"], self.G(bn.weight) if bn is not None else None,
+                     self.G(bn.bias) if bn is not None else None)
             continue
         self._op(self.bwd_ops, "fvit_feature_map_bwd", d["dy"].data_ptr(), d["x"].data_ptr(), d["C"],
                  d["rows"].data_ptr(), self.B, d["T"], d["C"], P(d["mu"]), P(d["rs"]),

@@ -140,6 +140,9 @@ _OP_SIGS: dict[str, list] = {
     "fvit_feature_map_bwd_stats": [_P, _P, _L, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P],
     "fvit_feature_map_bwd": [_P, _P, _L, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _L, _P, _P, _P],
     "fvit_grad_scale_finalize": [_P, _F, _P, _P],
+    # dense-prediction outputs and forward_head in eval mode (include/fvit.h "running-statistics BatchNorm2d folded in")
+    "fvit_feature_map_eval_bwd": [_P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _L, _P, _P, _P],
+    "fvit_head_eval_bwd": [_P, _L, _I, _I, _P, _I, _I, _P, _P, _P, _P, _P, _P],
     # eval-mode gradients (include/fvit.h "Eval-mode gradients")
     "fvit_bn_eval_bwd": [_P, _I, _L, _P, _P, _L, _P, _I, _I, _P, _P, _F, _P, _P, _I, _P, _P, _P, _L, _P, _P, _P, _P],
     "fvit_pool_bn_eval_bwd": [_P, _L, _P, _I, _I, _I, _P, _P, _F, _P, _P, _L, _P, _P, _L, _P, _P, _P],

@@ -310,16 +310,19 @@ class FasterViT(nn.Module):
     def forward_levels(self, x, out_indices=(0, 1, 2, 3)):
         """Per-level feature maps [B, C_i, H_i, W_i] (each level's output before its Downsample), the `xo` a dense-
         prediction backbone taps (downstream/object_detection/dino/models/dino/fastervit.py:686-709, 816-827).
-        Under .train() the maps are differentiable (the forward stops after the highest requested level; parameters
-        above it, `norm` and `head` get no gradient)."""
+        Differentiable under .train(), and under .eval() with grad enabled (running-statistics BatchNorms; x.grad too
+        when x requires grad). Parameters above the highest requested level, `norm` and `head` get no gradient."""
         return self._get_engine().forward_levels(x, tuple(out_indices))
 
     def forward_features(self, x):
         """The `norm`-ed last-level map [B, C, H, W] (fv.py:949-953); under .train() with batch statistics (running
-        statistics updated) and differentiable."""
+        statistics updated), under .eval() with running statistics; differentiable in both (in eval when grad is
+        enabled and x or a parameter requires grad)."""
         return self._get_engine().forward(x, features_only=True)
 
     def forward_head(self, x):
+        """avg-pool + head (fv.py:955-958) of a forward_features map (or pooled features); eval mode only, and then
+        differentiable w.r.t. the features and the head's parameters."""
         return self._get_engine().forward_head(x)
 
     def forward(self, x):

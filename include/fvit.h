@@ -314,6 +314,22 @@ int fvit_feature_map_bwd(const float* dy, const float* xs, int64_t ldx, const in
                          const float* s2, const float* gs, const float* scalar, float* g, int64_t ldg, float* dw,
                          float* dbeta, void* stream);
 int fvit_grad_scale_finalize(const float* amax, float target, float* gs, void* stream);
+/* Backward of fvit_feature_map_fwd with a running-statistics BatchNorm2d folded in (eval-mode gradients of the level
+ * norms and of `norm` in forward_features): g[row_map[b*T+t]][c] += S * w[c] * rstd[c] * dy[b][c][t] (S = gs[0], rstd
+ * = rsqrt(running_var + eps)); w == rstd == NULL is the raw map (g += S * dy). Rows outside row_map are untouched.
+ * dw[c] += s2[c] * (*scalar), dbeta[c] += s1[c] * (*scalar) with s1 = sum dy, s2 = sum dy * xhat from
+ * fvit_feature_map_bwd_stats run with the running mean / rstd (scalar NULL = 1). g NULL: only dw / dbeta. Same 32 x 32
+ * transposed tiles as fvit_feature_map_bwd; the apply reads no activation. */
+int fvit_feature_map_eval_bwd(const float* dy, const int32_t* row_map, int32_t B, int32_t T, int32_t C,
+                              const float* rstd, const float* w, const float* s1, const float* s2, const float* gs,
+                              const float* scalar, float* g, int64_t ldg, float* dw, float* dbeta, void* stream);
+/* Backward of forward_head (faster_vit.py:955-958: AdaptiveAvgPool2d(1) + flatten + Linear), fp32 throughout, from
+ * dlogits [B, ncls] (row stride ldl). feats: the fp32 input, NCHW [B, C, T] (T = H*W) or pooled [B, C] (T = 1).
+ * dfeats[b][c][t] = (sum_k dlogits[b][k] * W[k][c]) / T (written); dW[k][c] += sum_b dlogits[b][k] * pooled[b][c] with
+ * pooled = mean_t feats, recomputed into pooled_ws [B*C] when T > 1; db[k] += sum_b dlogits[b][k]. W NULL: an
+ * identity head (num_classes = 0, ncls == C), the pooling backward alone. Any of dfeats / dW / db may be NULL. */
+int fvit_head_eval_bwd(const float* dlogits, int64_t ldl, int32_t B, int32_t ncls, const float* feats, int32_t C,
+                       int32_t T, const float* W, float* pooled_ws, float* dfeats, float* dW, float* db, void* stream);
 
 /* forward_head (faster_vit.py:955-958): AdaptiveAvgPool2d(1) + flatten of an NCHW fp32 map into the fp16 operand
  * [B, ldo] of the classifier GEMM. */
