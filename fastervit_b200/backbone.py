@@ -54,11 +54,17 @@ class FasterViTBackbone(nn.Module):
         self._freeze_stages()
         return self
 
+    def enable_input_grad(self, enabled: bool = True):
+        """train-mode image gradients through the backbone (FasterViT.enable_input_grad), the frozen prefix included"""
+        self.body.enable_input_grad(enabled)
+        return self
+
     def forward_raw(self, x: torch.Tensor) -> tuple:
         """fastervit.py:816-827: tuple of the normalised level outputs, NCHW. Under .train() (detector fine-tuning,
         dino/backbone.py:158-160) the body runs its training launch list up to the highest requested level, every
         norm{i} normalises with batch statistics (running statistics updated) and the outputs are differentiable;
-        the frozen prefix runs on running statistics and gets no gradient. Under .eval() every norm{i} uses its running
+        the frozen prefix runs on running statistics and gets no parameter gradient; when x requires grad (after
+        enable_input_grad()) the image gradient crosses it with a data-only backward (no weight gradients). Under .eval() every norm{i} uses its running
         statistics; with grad enabled the outputs are differentiable too (norm-eval fine-tuning, perceptual losses:
         parameter gradients, and the image gradient when x requires grad), and a forward without backward costs what
         the inference forward costs."""

@@ -159,6 +159,113 @@ bn_eval_bwd_kernel(const void* __restrict__ gin, long long ldg, const int* __res
   }
 }
 
+// ---------------------------------------------------------------------------------- BatchNorm2d, data gradient only
+// The same backward when nobody wants dw / db (a stage whose parameters get no gradient): out16 = k * dy with
+// k[c] = scale[c] * colmul[c] * *scalar, scale = w * rsqrt(var + eps) as the forward folded it, masked by ReLU'
+// (sign of raw * scale + shift, the forward's own pre-activation). No xhat, no sums, no atomics: raw is read only for
+// the mask, so without an activation the pass moves dy in and dz out and nothing else.
+// Layout as bn_eval_bwd_v8_kernel: a lane owns 8 channels, vpr lanes cover a row, R rows in flight per thread.
+template <int G16, int RELU>
+__global__ void __launch_bounds__(256, 3)
+bn_eval_dgrad_v8_kernel(const void* __restrict__ gin, long long ldg, const int* __restrict__ g_rows,
+                        const __half* __restrict__ raw, long long ldr, const int* __restrict__ r_rows, int nrows, int C,
+                        int vpr, const float* __restrict__ scale, const float* __restrict__ shift,
+                        const float* __restrict__ colmul, const float* __restrict__ scalar, __half* __restrict__ out,
+                        long long ldo, const int* __restrict__ o_rows) {
+  const int cx = threadIdx.x % vpr, rl = threadIdx.x / vpr, RL = 256 / vpr;
+  const int c = (blockIdx.y * vpr + cx) * 8;
+  const int nv = min(8, C - c);
+  if (nv <= 0) return;
+  constexpr int R = G16 ? BNE_ROWS : BNE_ROWS / 2;
+  const float s = scalar ? __ldg(scalar) : 1.f;
+  float sc[8], sh[8], kk[8];
+#pragma unroll
+  for (int u = 0; u < 8; ++u) {
+    const bool in = u < nv;
+    sc[u] = in ? __ldg(scale + c + u) : 0.f;
+    sh[u] = in && RELU ? __ldg(shift + c + u) : 0.f;
+    kk[u] = sc[u] * s * (in && colmul ? __ldg(colmul + c + u) : 1.f);
+  }
+  const bool same_rows = g_rows == r_rows, same_out = o_rows == g_rows;
+  const int rstep = gridDim.x * RL;
+  for (int r0 = blockIdx.x * RL + rl; r0 < nrows; r0 += R * rstep) {
+    long long rg[R], rr[R], ro[R];
+#pragma unroll
+    for (int t = 0; t < R; ++t) {
+      const int r = r0 + t * rstep;
+      const bool ok = r < nrows;
+      rg[t] = ok ? (g_rows ? (long long)g_rows[r] : (long long)r) : -1;
+      rr[t] = !RELU || same_rows ? rg[t] : (ok ? (r_rows ? (long long)r_rows[r] : (long long)r) : -1);
+      ro[t] = same_out ? rg[t] : (ok ? (o_rows ? (long long)o_rows[r] : (long long)r) : -1);
+      if (ro[t] < 0 || rr[t] < 0) rg[t] = -1;   // (a row any of the maps drops is skipped)
+    }
+    uint4 ga[R], gb[R], xp[R];
+#pragma unroll
+    for (int t = 0; t < R; ++t) {
+      ga[t] = gb[t] = xp[t] = make_uint4(0u, 0u, 0u, 0u);
+      if (rg[t] >= 0) {
+        if (G16) {
+          ga[t] = *reinterpret_cast<const uint4*>(reinterpret_cast<const __half*>(gin) + rg[t] * ldg + c);
+        } else {
+          const uint4* p4 = reinterpret_cast<const uint4*>(reinterpret_cast<const float*>(gin) + rg[t] * ldg + c);
+          ga[t] = p4[0];
+          if (nv > 4) gb[t] = p4[1];
+        }
+        if (RELU) xp[t] = *reinterpret_cast<const uint4*>(raw + rr[t] * ldr + c);
+      }
+    }
+#pragma unroll
+    for (int t = 0; t < R; ++t) {
+      if (rg[t] < 0) continue;
+      float dy[8];
+      if (G16) {
+        const __half2* h = reinterpret_cast<const __half2*>(&ga[t]);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) dy[2 * u] = __low2float(h[u]), dy[2 * u + 1] = __high2float(h[u]);
+      } else {
+        dy[0] = __uint_as_float(ga[t].x), dy[1] = __uint_as_float(ga[t].y);
+        dy[2] = __uint_as_float(ga[t].z), dy[3] = __uint_as_float(ga[t].w);
+        dy[4] = __uint_as_float(gb[t].x), dy[5] = __uint_as_float(gb[t].y);
+        dy[6] = __uint_as_float(gb[t].z), dy[7] = __uint_as_float(gb[t].w);
+      }
+      const __half2* hx = reinterpret_cast<const __half2*>(&xp[t]);
+      __half2 h[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        float o0 = kk[2 * u] * dy[2 * u], o1 = kk[2 * u + 1] * dy[2 * u + 1];   // (kk = 0 on padding columns)
+        if (RELU) {
+          if (fmaf(__low2float(hx[u]), sc[2 * u], sh[2 * u]) <= 0.f) o0 = 0.f;
+          if (fmaf(__high2float(hx[u]), sc[2 * u + 1], sh[2 * u + 1]) <= 0.f) o1 = 0.f;
+        }
+        h[u] = __floats2half2_rn(o0, o1);
+      }
+      *reinterpret_cast<uint4*>(out + ro[t] * ldo + c) = *reinterpret_cast<const uint4*>(h);
+    }
+  }
+}
+
+// Any layout: one thread per element.
+template <int G16>
+__global__ void __launch_bounds__(256)
+bn_eval_dgrad_kernel(const void* __restrict__ gin, long long ldg, const int* __restrict__ g_rows,
+                     const __half* __restrict__ raw, long long ldr, const int* __restrict__ r_rows, int nrows, int C,
+                     const float* __restrict__ scale, const float* __restrict__ shift, int relu,
+                     const float* __restrict__ colmul, const float* __restrict__ scalar, __half* __restrict__ out,
+                     long long ldo, const int* __restrict__ o_rows) {
+  const float s = scalar ? __ldg(scalar) : 1.f;
+  const long long total = (long long)nrows * C;
+  for (long long i = blockIdx.x * 256LL + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const int r = (int)(i / C), c = (int)(i % C);
+    const long long rg = g_rows ? g_rows[r] : r, rr = r_rows ? r_rows[r] : r, ro = o_rows ? o_rows[r] : r;
+    if (rg < 0 || ro < 0 || (relu && rr < 0)) continue;
+    float dy = G16 ? __half2float(reinterpret_cast<const __half*>(gin)[rg * ldg + c])
+                   : reinterpret_cast<const float*>(gin)[rg * ldg + c];
+    const float sc = scale[c];
+    if (relu && fmaf(__half2float(raw[rr * ldr + c]), sc, shift[c]) <= 0.f) dy = 0.f;
+    out[ro * ldo + c] = __float2half_rn(sc * s * (colmul ? colmul[c] : 1.f) * dy);
+  }
+}
+
 // ---------------------------------------------------------------------------------- head: running-statistics BN + pool
 // pooled[b,c] = mean_t (xhat[b,t,c]*w + beta): g[row(b,t)][c] = dpool[b,c]/T * w*rstd (the same for every t),
 // dw += scalar * sum_b dpool * mean_t xhat, dbeta += scalar * sum_b dpool. Block = 128 columns; blocks stride over b.
@@ -360,6 +467,52 @@ int fvit_bn_eval_bwd(const void* gin, int32_t g_is_f16, int64_t ldg, const int32
     bn_eval_bwd_kernel<0><<<grid, 256, 0, st>>>(gin, ldg, g_rows, (const __half*)raw16, ldr, r_rows, nrows, C, mean, var,
                                                 eps, w, b, act, colmul, scalar, (__half*)out16, ldo, o_rows, dw, db);
   return post_launch("bn_eval_bwd_kernel");
+}
+
+int fvit_bn_eval_dgrad(const void* gin, int32_t g_is_f16, int64_t ldg, const int32_t* g_rows, const void* raw16,
+                       int64_t ldr, const int32_t* r_rows, int32_t nrows, int32_t C, const float* scale,
+                       const float* shift, int32_t act, const float* colmul, const float* scalar, void* out16,
+                       int64_t ldo, const int32_t* o_rows, void* stream) {
+  FVIT_CHECK(gin && scale && out16 && nrows > 0 && C > 0, "fvit_bn_eval_dgrad: bad arguments");
+  FVIT_CHECK(act == FVIT_ACT_NONE || act == FVIT_ACT_RELU, "fvit_bn_eval_dgrad: act must be NONE or RELU");
+  const bool relu = act == FVIT_ACT_RELU;
+  FVIT_CHECK(!relu || (raw16 && shift), "fvit_bn_eval_dgrad: the ReLU mask needs raw16 and shift");
+  const cudaStream_t st = (cudaStream_t)stream;
+  const bool vec8 = C % 4 == 0 && ldg % (g_is_f16 ? 8 : 4) == 0 && (!relu || ldr % 8 == 0) && ldo % 8 == 0 &&
+                    reinterpret_cast<uintptr_t>(gin) % 16 == 0 && (!relu || reinterpret_cast<uintptr_t>(raw16) % 16 == 0) &&
+                    reinterpret_cast<uintptr_t>(out16) % 16 == 0;
+  if (vec8) {
+    const int c8 = (C + 7) / 8;
+    int vpr = 1;
+    while (vpr < 64 && vpr < c8) vpr *= 2;
+    const unsigned gy = (unsigned)((c8 + vpr - 1) / vpr);
+    const int RL = 256 / vpr;
+    long long gx = ((long long)num_sms() * 8 + gy - 1) / gy;
+    const long long gx_max = ((long long)nrows + RL * BNE_ROWS - 1) / (RL * BNE_ROWS);
+    if (gx > gx_max) gx = gx_max;
+    if (gx < 1) gx = 1;
+    dim3 grid((unsigned)gx, gy);
+#define FVIT_BN_DGRAD(G, R)                                                                                        \
+  bn_eval_dgrad_v8_kernel<G, R><<<grid, 256, 0, st>>>(gin, ldg, g_rows, (const __half*)raw16, ldr, r_rows, nrows, C, \
+                                                      vpr, scale, shift, colmul, scalar, (__half*)out16, ldo, o_rows)
+    if (g_is_f16) {
+      if (relu) FVIT_BN_DGRAD(1, 1); else FVIT_BN_DGRAD(1, 0);
+    } else {
+      if (relu) FVIT_BN_DGRAD(0, 1); else FVIT_BN_DGRAD(0, 0);
+    }
+#undef FVIT_BN_DGRAD
+    return post_launch("bn_eval_dgrad_v8_kernel");
+  }
+  long long gx = ((long long)nrows * C + 255) / 256;
+  const long long cap = (long long)num_sms() * 16;
+  if (gx > cap) gx = cap;
+  if (g_is_f16)
+    bn_eval_dgrad_kernel<1><<<(unsigned)gx, 256, 0, st>>>(gin, ldg, g_rows, (const __half*)raw16, ldr, r_rows, nrows, C,
+                                                          scale, shift, relu, colmul, scalar, (__half*)out16, ldo, o_rows);
+  else
+    bn_eval_dgrad_kernel<0><<<(unsigned)gx, 256, 0, st>>>(gin, ldg, g_rows, (const __half*)raw16, ldr, r_rows, nrows, C,
+                                                          scale, shift, relu, colmul, scalar, (__half*)out16, ldo, o_rows);
+  return post_launch("bn_eval_dgrad_kernel");
 }
 
 int fvit_pool_bn_eval_bwd(const float* xs, int64_t ldx, const int32_t* rows, int32_t B, int32_t T, int32_t C,

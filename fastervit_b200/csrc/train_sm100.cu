@@ -464,6 +464,40 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// The dx half of ln_bwd_generic_kernel alone (fvit_ln_dgrad on rows the vectorised kernel does not take): no shared
+// memory, no atomics.
+__global__ void __launch_bounds__(256)
+    ln_dgrad_generic_kernel(const __half* __restrict__ dy, long long lddy, const int* __restrict__ dy_map,
+                            const __half* __restrict__ xhat, long long ldxh, const float* __restrict__ rstd,
+                            const float* __restrict__ gamma, int rows, int C, float* __restrict__ g, long long ldg,
+                            const int* __restrict__ in_map, int use_g, int clear_moved) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  for (int r = blockIdx.x * nw + warp; r < rows; r += gridDim.x * nw) {
+    const long long rdy = dy_map ? dy_map[r] : r;
+    if (rdy < 0) continue;  // warp-uniform
+    const __half* dyr = dy + rdy * lddy;
+    const __half* xr = xhat + (long long)r * ldxh;
+    float s1 = 0.f, s2 = 0.f;
+    for (int c = lane; c < C; c += 32) {
+      const float gd = __half2float(dyr[c]) * __ldg(gamma + c);
+      s1 += gd;
+      s2 += gd * __half2float(xr[c]);
+    }
+    s1 = warp_sum_t(s1) / C;
+    s2 = warp_sum_t(s2) / C;
+    const float rs = rstd[r];
+    const long long src = in_map ? in_map[r] : r;
+    float* gr = g + (long long)r * ldg;
+    float* gs_ = g + src * ldg;
+    for (int c = lane; c < C; c += 32) {
+      float v = rs * (__half2float(dyr[c]) * __ldg(gamma + c) - s1 - __half2float(xr[c]) * s2);
+      if (use_g) v += gr[c];
+      if (clear_moved && src != r) gr[c] = 0.f;
+      gs_[c] = v;
+    }
+  }
+}
+
 constexpr int LNB_MAXV = 7;  // 8-half vectors per lane: C <= 32 * 8 * 7 = 1792
 // Vectorised dx part (C % 8 == 0): one warp per row, the row's dy / xhat live in registers between the two
 // passes. MAXV (vectors per lane) is a template parameter so narrow rows do not pay for wide rows' registers.
@@ -1632,6 +1666,36 @@ int fvit_group_sum(const float* a, int64_t lda, int32_t ngroups, int32_t group, 
   return post_launch("group_sum_kernel");
 }
 
+// the vectorised dx kernel of a LayerNorm backward (fvit_ln_bwd, fvit_ln_dgrad); the caller checked the layout
+static void ln_dx_launch(const __half* dyh, int64_t lddy, const int32_t* dy_map, const __half* xhh, int64_t ldxh,
+                         const float* rstd, const float* gamma, int32_t rows, int32_t C, float* g, int64_t ldg,
+                         const int32_t* in_map, int32_t use_g, int32_t clear_moved, cudaStream_t st) {
+  const int block = 256, wpb = 8;
+  long long grid = ((long long)rows + wpb - 1) / wpb;
+  const long long cap = (long long)num_sms() * 16;
+  if (grid > cap) grid = cap;
+  const int nvl = (C / 8 + 31) / 32;
+  static int prefetch_g = -1;  // fetch g with the operands instead of after the warp reductions ; FVIT_LN_PREFETCH=0 = A/B
+  if (prefetch_g < 0) {
+    const char* e = getenv("FVIT_LN_PREFETCH");
+    prefetch_g = e ? atoi(e) : 1;
+  }
+#define FVIT_LN_DX(MV)                                                                                              \
+  do {                                                                                                              \
+    if (prefetch_g)                                                                                                 \
+      ln_bwd_dx_kernel<MV, true><<<(unsigned)grid, block, 0, st>>>(dyh, lddy, dy_map, xhh, ldxh, rstd, gamma, rows, C, g, \
+                                                                   ldg, in_map, use_g, clear_moved);                \
+    else                                                                                                            \
+      ln_bwd_dx_kernel<MV, false><<<(unsigned)grid, block, 0, st>>>(dyh, lddy, dy_map, xhh, ldxh, rstd, gamma, rows, C, g, \
+                                                                    ldg, in_map, use_g, clear_moved);               \
+  } while (0)
+  if (nvl <= 1) FVIT_LN_DX(1);
+  else if (nvl <= 2) FVIT_LN_DX(2);
+  else if (nvl <= 4) FVIT_LN_DX(4);
+  else FVIT_LN_DX(LNB_MAXV);
+#undef FVIT_LN_DX
+}
+
 int fvit_ln_bwd(const void* dy16, int64_t lddy, const int32_t* dy_map, const void* xhat16, int64_t ldxh,
                 const float* rstd, const float* gamma, int32_t rows, int32_t C, float* g, int64_t ldg,
                 const int32_t* in_map, int32_t use_g, int32_t clear_moved, const float* scalar, float* dgamma,
@@ -1643,30 +1707,9 @@ int fvit_ln_bwd(const void* dy16, int64_t lddy, const int32_t* dy_map, const voi
   long long grid = ((long long)rows + wpb - 1) / wpb;
   const cudaStream_t st = (cudaStream_t)stream;
   if (vec) {
-    const long long cap = (long long)num_sms() * 16;
-    if (grid > cap) grid = cap;
     const __half* dyh = (const __half*)dy16;
     const __half* xhh = (const __half*)xhat16;
-    const int nvl = (C / 8 + 31) / 32;
-    static int prefetch_g = -1;  // fetch g with the operands instead of after the warp reductions ; FVIT_LN_PREFETCH=0 = A/B
-    if (prefetch_g < 0) {
-      const char* e = getenv("FVIT_LN_PREFETCH");
-      prefetch_g = e ? atoi(e) : 1;
-    }
-#define FVIT_LN_DX(MV)                                                                                              \
-  do {                                                                                                              \
-    if (prefetch_g)                                                                                                 \
-      ln_bwd_dx_kernel<MV, true><<<(unsigned)grid, block, 0, st>>>(dyh, lddy, dy_map, xhh, ldxh, rstd, gamma, rows, C, g, \
-                                                                   ldg, in_map, use_g, clear_moved);                \
-    else                                                                                                            \
-      ln_bwd_dx_kernel<MV, false><<<(unsigned)grid, block, 0, st>>>(dyh, lddy, dy_map, xhh, ldxh, rstd, gamma, rows, C, g, \
-                                                                    ldg, in_map, use_g, clear_moved);               \
-  } while (0)
-    if (nvl <= 1) FVIT_LN_DX(1);
-    else if (nvl <= 2) FVIT_LN_DX(2);
-    else if (nvl <= 4) FVIT_LN_DX(4);
-    else FVIT_LN_DX(LNB_MAXV);
-#undef FVIT_LN_DX
+    ln_dx_launch(dyh, lddy, dy_map, xhh, ldxh, rstd, gamma, rows, C, g, ldg, in_map, use_g, clear_moved, st);
     int vpr = 1;
     while (vpr < 32 && vpr < C / 8) vpr *= 2;
     const unsigned gy = (unsigned)((C / 8 + vpr - 1) / vpr);
@@ -1691,6 +1734,24 @@ int fvit_ln_bwd(const void* dy16, int64_t lddy, const int32_t* dy_map, const voi
                                                              ldxh, rstd, gamma, rows, C, g, ldg, in_map, use_g,
                                                              clear_moved, scalar, dgamma, dbeta);
   return post_launch("ln_bwd_kernel");
+}
+
+int fvit_ln_dgrad(const void* dy16, int64_t lddy, const int32_t* dy_map, const void* xhat16, int64_t ldxh,
+                  const float* rstd, const float* gamma, int32_t rows, int32_t C, float* g, int64_t ldg,
+                  const int32_t* in_map, int32_t use_g, int32_t clear_moved, void* stream) {
+  FVIT_CHECK(dy16 && xhat16 && rstd && gamma && g && rows > 0 && C > 0, "fvit_ln_dgrad: bad arguments");
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (C % 8 == 0 && C <= 32 * 8 * LNB_MAXV && lddy % 8 == 0 && ldxh % 8 == 0 && ldg % 4 == 0) {
+    ln_dx_launch((const __half*)dy16, lddy, dy_map, (const __half*)xhat16, ldxh, rstd, gamma, rows, C, g, ldg, in_map,
+                 use_g, clear_moved, st);
+    return post_launch("ln_bwd_dx_kernel");
+  }
+  long long grid = ((long long)rows + 7) / 8;
+  const long long cap = (long long)num_sms() * 8;
+  if (grid > cap) grid = cap;
+  ln_dgrad_generic_kernel<<<(unsigned)grid, 256, 0, st>>>((const __half*)dy16, lddy, dy_map, (const __half*)xhat16, ldxh,
+                                                          rstd, gamma, rows, C, g, ldg, in_map, use_g, clear_moved);
+  return post_launch("ln_dgrad_generic_kernel");
 }
 
 int fvit_attn_core_bwd(const void* qkv, int64_t ldq, const void* dout, int64_t lddo, int32_t groups, int32_t S,
@@ -1875,17 +1936,10 @@ int fvit_unpack_conv_grad(const float* src, int32_t ld_ci, float* dst, int32_t c
   return post_launch("unpack_conv_grad_kernel");
 }
 
-int fvit_token_init_bwd(const float* g, int64_t ldg, const void* x16, int64_t ldx, const int32_t* pix_map,
-                        const int32_t* ct_row_map, int32_t B, int32_t Hp, int32_t Wp, int32_t C, const float* w,
-                        int32_t kh, int32_t kw, int32_t sh, int32_t sw, int32_t oh, int32_t ow, const float* scalar,
-                        float* gx, int64_t ldgx, float* dw, float* dbias, void* stream) {
-  FVIT_CHECK(g && x16 && pix_map && ct_row_map && w && gx && dw && dbias, "fvit_token_init_bwd: null argument");
-  const int npos4 = (B * oh * ow + 3) / 4;
-  dim3 gw((unsigned)((C + 127) / 128), (unsigned)(npos4 < 512 ? npos4 : 512));
-  token_init_wgrad_kernel<<<gw, 512, 0, (cudaStream_t)stream>>>(g, ldg, (const __half*)x16, ldx, pix_map, ct_row_map, B, Hp, Wp, C, kh, kw,
-                                                                sh, sw, oh, ow, scalar, dw, dbias);
-  int rc = post_launch("token_init_wgrad_kernel");
-  if (rc) return rc;
+// the input-gradient kernels of the TokenInitializer backward (fvit_token_init_bwd, fvit_token_init_dgrad)
+static int token_init_dx_launch(const float* g, int64_t ldg, const int32_t* pix_map, const int32_t* ct_row_map, int32_t B,
+                                int32_t Hp, int32_t Wp, int32_t C, const float* w, int32_t kh, int32_t kw, int32_t sh,
+                                int32_t sw, int32_t oh, int32_t ow, float* gx, int64_t ldgx, void* stream) {
   const size_t tile_smem = ((size_t)oh * ow + (size_t)Hp * Wp) * 32 * sizeof(float);
   if (tile_smem <= 48 * 1024 && B <= 65535) {  // the whole map of one image fits: pool backward formed once per pixel
     dim3 gt((unsigned)((C + 31) / 32), (unsigned)B);
@@ -1899,6 +1953,27 @@ int fvit_token_init_bwd(const float* g, int64_t ldg, const void* x16, int64_t ld
   token_init_bwd_kernel<<<gd, cb, 0, (cudaStream_t)stream>>>(g, ldg, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw,
                                                              oh, ow, gx, ldgx);
   return post_launch("token_init_bwd_kernel");
+}
+
+int fvit_token_init_bwd(const float* g, int64_t ldg, const void* x16, int64_t ldx, const int32_t* pix_map,
+                        const int32_t* ct_row_map, int32_t B, int32_t Hp, int32_t Wp, int32_t C, const float* w,
+                        int32_t kh, int32_t kw, int32_t sh, int32_t sw, int32_t oh, int32_t ow, const float* scalar,
+                        float* gx, int64_t ldgx, float* dw, float* dbias, void* stream) {
+  FVIT_CHECK(g && x16 && pix_map && ct_row_map && w && gx && dw && dbias, "fvit_token_init_bwd: null argument");
+  const int npos4 = (B * oh * ow + 3) / 4;
+  dim3 gw((unsigned)((C + 127) / 128), (unsigned)(npos4 < 512 ? npos4 : 512));
+  token_init_wgrad_kernel<<<gw, 512, 0, (cudaStream_t)stream>>>(g, ldg, (const __half*)x16, ldx, pix_map, ct_row_map, B, Hp, Wp, C, kh, kw,
+                                                                sh, sw, oh, ow, scalar, dw, dbias);
+  int rc = post_launch("token_init_wgrad_kernel");
+  if (rc) return rc;
+  return token_init_dx_launch(g, ldg, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw, oh, ow, gx, ldgx, stream);
+}
+
+int fvit_token_init_dgrad(const float* g, int64_t ldg, const int32_t* pix_map, const int32_t* ct_row_map, int32_t B,
+                          int32_t Hp, int32_t Wp, int32_t C, const float* w, int32_t kh, int32_t kw, int32_t sh,
+                          int32_t sw, int32_t oh, int32_t ow, float* gx, int64_t ldgx, void* stream) {
+  FVIT_CHECK(g && pix_map && ct_row_map && w && gx && B > 0 && C > 0, "fvit_token_init_dgrad: bad arguments");
+  return token_init_dx_launch(g, ldg, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw, oh, ow, gx, ldgx, stream);
 }
 
 int fvit_propagate_bwd(float* g, int64_t ldg, const float* xs, int64_t ldx, const int32_t* src_map, int32_t rows, int32_t C,

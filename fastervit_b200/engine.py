@@ -903,7 +903,7 @@ class Engine:
         if spec is not None:
             # dense train plans: one per (requested outputs, norms present, frozen prefix) besides the input shape
             key += (spec["kind"], tuple((i, None if bn is None else id(bn)) for i, bn in spec.get("outs", ())),
-                    spec.get("frozen", -1), bool(spec.get("eval")))
+                    spec.get("frozen", -1), bool(spec.get("eval")), spec.get("want_dx"), spec.get("data_only"))
             # the level norms are not the model's own tensors (the backbone's norm{i}): the plan reads them through raw
             # pointers too, so a reallocation of one of them (`bn.weight.data = ...`) rebuilds it
             norm_sig = self._norm_sig(spec)
@@ -938,13 +938,27 @@ class Engine:
                 ptrs.append(t.data_ptr())
         return tuple(ptrs)
 
+    def _train_wants_dx(self, x: torch.Tensor) -> bool:
+        """does this train-mode forward need the plan with the image gradient; an input that requires grad on a model
+        that did not ask for it (FasterViT.enable_input_grad) raises"""
+        if not (torch.is_grad_enabled() and x.requires_grad):
+            return False
+        if not x.is_cuda:
+            return False    # (_plan raises for a CPU input, as for any other)
+        if not getattr(self.model, "_train_input_grad", False):
+            raise L.FvitError("the input requires grad, but train-mode image gradients are off for this model: call "
+                              "model.enable_input_grad() to get x.grad from the backward, or detach the input")
+        return True
+
     def _dense_train(self, x: torch.Tensor, spec: dict) -> tuple:
         """Train-mode forward of a pooled / levels plan: an autograd node whose backward runs the plan's backward
         launch list from the output gradients (engine_train._DenseFunction)."""
+        if self._train_wants_dx(x):
+            spec = dict(spec, want_dx=True)    # (its own plan: one built for a plain input keeps its launch lists)
         plan = self._plan(x, spec)
         from .engine_train import _DenseFunction
         with torch.cuda.device(x.device):
-            if torch.is_grad_enabled() and any(p.requires_grad for p in plan.params):
+            if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in plan.params)):
                 return _DenseFunction.apply(plan, x, *plan.params)
             plan.run_forward(x)
             return tuple(o.clone() for o in plan.outputs)
@@ -957,11 +971,12 @@ class Engine:
             if not isinstance(self.model.head, nn.Linear):
                 # num_classes = 0: the pooled features (fv.py:955-958)
                 return self._dense_train(x, dict(kind="pooled"))[0]
-        plan = self._plan(x)
+        want_dx = self.model.training and self._train_wants_dx(x)
+        plan = self._plan(x, dict(kind=None, want_dx=True) if want_dx else None)
         if plan.training:
             from .engine_train import _FasterViTFunction
             with torch.cuda.device(x.device):
-                if torch.is_grad_enabled() and any(p.requires_grad for p in plan.params):
+                if torch.is_grad_enabled() and (want_dx or any(p.requires_grad for p in plan.params)):
                     return _FasterViTFunction.apply(plan, x, *plan.params)
                 return plan.run_forward(x).clone()
         params = self._params
@@ -975,11 +990,15 @@ class Engine:
             return _EvalGradFunction.apply_fast(self, plan, x, *params)
         return self._run_eval(plan, x, features_only)
 
-    def eval_grad_plan(self, x: torch.Tensor) -> Plan:
+    def eval_grad_plan(self, x: torch.Tensor, want_dx: bool = True, data_only: tuple | None = None) -> Plan:
         """The plan the backward of a differentiable eval forward runs (built at the first such backward): a TrainPlan
-        whose BatchNorms use their running statistics and whose backward also writes the image gradient."""
+        whose BatchNorms use their running statistics and whose backward also writes the image gradient (want_dx).
+        data_only: engine_train.stage_mask of the stages that get no parameter gradient; one plan per mask."""
         kind = None if isinstance(self.model.head, nn.Linear) else "pooled"
-        return self._plan(x, dict(kind=kind, eval=True))
+        spec = dict(kind=kind, eval=True)
+        if not want_dx or (data_only is not None and any(data_only)):
+            spec.update(want_dx=bool(want_dx), data_only=None if data_only is None else tuple(map(bool, data_only)))
+        return self._plan(x, spec)
 
     def eval_grad_plans(self) -> list:
         """the eval-grad plans built so far (one per input shape)"""
@@ -1083,11 +1102,16 @@ class Engine:
             res.append(out)
         return tuple(res)
 
-    def eval_dense_plan(self, x: torch.Tensor, outs: tuple, frozen: int) -> Plan:
+    def eval_dense_plan(self, x: torch.Tensor, outs: tuple, frozen: int, want_dx: bool | None = None,
+                        data_only: tuple | None = None) -> Plan:
         """The plan the backward of a differentiable eval-mode dense output runs (built at the first such backward): a
-        levels-mode TrainPlan whose BatchNorms (the level norms too) use their running statistics; with frozen = -1 its
-        backward also writes the image gradient."""
-        return self._plan(x, dict(kind="levels", outs=outs, frozen=frozen, eval=True))
+        levels-mode TrainPlan whose BatchNorms (the level norms too) use their running statistics. want_dx (default:
+        frozen = -1): its backward also writes the image gradient, crossing the frozen prefix and the `data_only`
+        stages (engine_train.stage_mask) with the activation gradient alone."""
+        spec = dict(kind="levels", outs=outs, frozen=frozen, eval=True)
+        if want_dx is not None:
+            spec.update(want_dx=bool(want_dx), data_only=None if data_only is None else tuple(map(bool, data_only)))
+        return self._plan(x, spec)
 
     def _eval_levels(self, plan: Plan, x: torch.Tensor, out_indices: tuple) -> tuple:
         with torch.cuda.device(x.device):

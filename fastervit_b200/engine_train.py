@@ -44,6 +44,13 @@ def levels_path(model, outs) -> set[int]:
     return on
 
 
+def stage_mask(model, needs_grad) -> tuple:
+    """Per stage (0 = the stem, 1 + i = levels[i] with the Downsample that follows it) whether none of its parameters
+    takes a gradient: `needs_grad(p)` says which parameters do. Such a stage's backward is data-only."""
+    mods = [model.patch_embed, *model.levels]
+    return tuple(not any(needs_grad(p) for p in mod.parameters()) for mod in mods)
+
+
 def _sm_count() -> int:
     """SMs of the current device; plans built without one (host-side tests) assume an H100 SXM's 132."""
     if torch.cuda.is_available():
@@ -60,7 +67,12 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
     downstream/.../dino/fastervit.py:801-812, runs its BatchNorms on running statistics and gets no backward).
     {"kind": None | "pooled", "eval": True} = the eval-grad plan, the backward of an eval()-mode forward: every BatchNorm
     on its running statistics (not updated), no stochastic depth, and a backward that also yields the image gradient
-    `dx` (engine.Engine.forward)."""
+    `dx` (engine.Engine.forward).
+    "want_dx": the backward continues through conv1 into `self.dx`, the fp32 NCHW image gradient (default: an eval plan
+    without a frozen prefix). "data_only" (eval plans): a stage_mask() of stages whose parameters get no gradient; the
+    frozen prefix always is one. A data-only stage's backward carries the activation gradient alone (no weight-gradient
+    GEMM, no bias / norm / layer-scale / positional-MLP reduction), and is not emitted at all when nothing below it
+    reads that gradient (`_needed`)."""
 
     def __init__(self, model, B: int, H: int, W: int, device, spec: dict | None = None):
         self.bwd_ops: list[tuple] = []
@@ -85,7 +97,20 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         self._frozen_bn = {id(b) for fm in ([model] if self.eval_grad else frozen_mods) for b in fm.modules()
                            if isinstance(b, torch.nn.BatchNorm2d)}
         self._frozen_params = {id(p) for fm in frozen_mods for p in fm.parameters()}
+        stages = [model.patch_embed, *model.levels]
+        mask = spec.get("data_only") if spec is not None else None
+        if mask is not None and (not self.eval_grad or len(mask) != len(stages)):
+            raise L.FvitError("data_only is a per-stage mask (stem, then one entry per level) of an eval plan")
+        self.data_only = tuple(s < len(frozen_mods) or bool(mask is not None and mask[s]) for s in range(len(stages)))
+        self.want_dx = bool(spec.get("want_dx", self.eval_grad and fs < 0)) if spec is not None else False
+        # the lowest stage the backward has to reach: -1 = the image, else the first stage with a parameter gradient
+        self._bwd_low = -1 if self.want_dx else min((s for s, d in enumerate(self.data_only) if not d), default=len(stages))
+        self._data_only_params = {id(p) for s, mod in enumerate(stages) if self.data_only[s] for p in mod.parameters()}
         super().__init__(model, B, H, W, True, device)
+
+    def _needed(self, stage: int) -> bool:
+        """does anything read the gradient this stage's backward produces (a trained stage below it, or the image)"""
+        return stage >= self._bwd_low
 
     # ------------------------------------------------------------------------------ infrastructure
     def _setup_train(self) -> None:
@@ -104,6 +129,8 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         for k, p in enumerate(self.params):
             if k == n_model:
                 self._n_model_flat = n         # end of the model's own slices
+            if self.eval_grad and id(p) in self._data_only_params:
+                continue   # no slice: nothing accumulates a gradient for it (a train plan keeps one layout per model)
             offs[id(p)] = n
             n += _ru(p.numel(), 64)            # 256-byte aligned slices
         if n_model == len(self.params):
@@ -136,8 +163,8 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         autograd). Levels mode: the stem and levels up to the highest requested one without its Downsample, the level
         norms; not the frozen prefix, nor `norm` / `head` unless forward_features asked for `norm`."""
         if self.kind != "levels":
-            return {id(p) for p in self.params}
-        return levels_path(self.model, self.spec["outs"]) - self._frozen_params
+            return {id(p) for p in self.params} - self._data_only_params
+        return levels_path(self.model, self.spec["outs"]) - self._data_only_params
 
     def grad_views_on_path(self) -> list:
         """grad_views() with None for the parameters off the path of the requested outputs"""
@@ -158,7 +185,8 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         """Per-parameter views of a *copy* of the flat gradient buffer: autograd's AccumulateGrad may keep
         the tensors it is handed, and the flat buffer itself is reused (zeroed) by the next backward."""
         flat = self.gflat.clone()
-        return [flat[self._goff[id(p)]: self._goff[id(p)] + p.numel()].view_as(p) for p in self.params]
+        return [flat[self._goff[id(p)]: self._goff[id(p)] + p.numel()].view_as(p) if id(p) not in self._data_only_params
+                else None for p in self.params]   # (a data-only stage's parameters: None, as autograd expects)
 
     def _scratch(self, name: str, n: int) -> int:
         """reserve n zero-initialised fp32 (re-zeroed at the start of every backward); returns offset"""
@@ -295,19 +323,23 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
     # ------------------------------------------------------------------------------ linear layer backward
     def _linear_bwd(self, *, lin, w16, ldw, x16, ldx, dz16, lddz, rows, n_out, k_in, br, gW=None, gW_ld=None,
                     dx16=None, lddx=0, dx_act=L.ACT_NONE, dx_aux=None, ld_aux=0, dx_alpha=None, bias_to=None,
-                    flops_k=None, want_dgrad=True, bias_done=False, dx_colsum=None, gW_row_map=None) -> None:
-        """dW[n_out, k_in] += alpha_w * dz16^T @ x16 ; db += alpha_w * colsum(dz16) ; dx16 = alpha_d * dz16 @ W."""
-        gW = self.G(lin.weight) if gW is None else gW
-        gW_ld = k_in if gW_ld is None else gW_ld
+                    flops_k=None, want_dgrad=True, bias_done=False, dx_colsum=None, gW_row_map=None,
+                    data_only=False) -> None:
+        """dW[n_out, k_in] += alpha_w * dz16^T @ x16 ; db += alpha_w * colsum(dz16) ; dx16 = alpha_d * dz16 @ W.
+        data_only: the last of the three alone."""
         fk = k_in if flops_k is None else flops_k
-        n0 = len(self.bwd_ops)
-        self._bgemm(a=dz16, a_rows=rows, lda=lddz, a_mn=True, b=x16, b_rows=rows, ldb=ldx, b_mn=True, m=n_out, n=k_in,
-                    kc=rows, split_k=self._split_k(n_out, k_in, rows), alpha_ptr=br["w_alpha"], out_f32=gW,
-                    ld_o32=gW_ld, row_map=gW_row_map, flops=2.0 * rows * n_out * fk)
-        if (lin.bias is not None or bias_to is not None) and not bias_done:
-            dst = bias_to if bias_to is not None else self.G(lin.bias)
-            self._op(self.bwd_ops, "fvit_colsum", dz16, 1, lddz, None, None, 0, rows, n_out, None, br["w_alpha"], dst, None)
-        self._side_from(n0, dz16)   # (weight gradient + bias column sums: both only read dz16)
+        if not data_only:
+            gW = self.G(lin.weight) if gW is None else gW
+            gW_ld = k_in if gW_ld is None else gW_ld
+            n0 = len(self.bwd_ops)
+            self._bgemm(a=dz16, a_rows=rows, lda=lddz, a_mn=True, b=x16, b_rows=rows, ldb=ldx, b_mn=True, m=n_out, n=k_in,
+                        kc=rows, split_k=self._split_k(n_out, k_in, rows), alpha_ptr=br["w_alpha"], out_f32=gW,
+                        ld_o32=gW_ld, row_map=gW_row_map, flops=2.0 * rows * n_out * fk)
+            if (lin.bias is not None or bias_to is not None) and not bias_done:
+                dst = bias_to if bias_to is not None else self.G(lin.bias)
+                self._op(self.bwd_ops, "fvit_colsum", dz16, 1, lddz, None, None, 0, rows, n_out, None, br["w_alpha"], dst,
+                         None)
+            self._side_from(n0, dz16)   # (weight gradient + bias column sums: both only read dz16)
         if want_dgrad:
             self._before_write(dx16)
             self._bgemm(a=dz16, a_rows=rows, lda=lddz, b=w16, b_rows=n_out, ldb=ldw, b_mn=True, m=rows, n=k_in, kc=n_out,
@@ -560,15 +592,13 @@ class _FasterViTFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, plan: TrainPlan, x: torch.Tensor, *params):
-        if x.requires_grad:
-            raise L.FvitError("the input requires grad, but the backward plan stops at the first convolution (no "
-                              "gradient w.r.t. the image is computed); detach the input")
         ctx.plan = plan
         logits = plan.run_forward(x)
         ctx.generation = plan.fwd_generation
         return logits.clone()
 
     @staticmethod
+    @torch.autograd.function.once_differentiable
     def backward(ctx, dlogits):
         plan: TrainPlan = ctx.plan
         if ctx.generation != plan.fwd_generation:
@@ -577,7 +607,7 @@ class _FasterViTFunction(torch.autograd.Function):
                 "overwrote the saved activations of this one (one autograd node per step: call backward before the "
                 "next forward, or use different plans / model copies for multi-view losses)")
         plan.run_backward(dlogits.contiguous().float())
-        return (None, None, *plan.grad_views())
+        return (None, _train_dx(ctx, plan), *plan.grad_views())
 
 
 class _DenseFunction(torch.autograd.Function):
@@ -587,15 +617,13 @@ class _DenseFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, plan: TrainPlan, x: torch.Tensor, *params):
-        if x.requires_grad:
-            raise L.FvitError("the input requires grad, but the backward plan stops at the first convolution (no "
-                              "gradient w.r.t. the image is computed); detach the input")
         ctx.plan = plan
         plan.run_forward(x)
         ctx.generation = plan.fwd_generation
         return tuple(o.clone() for o in plan.outputs)
 
     @staticmethod
+    @torch.autograd.function.once_differentiable
     def backward(ctx, *grads):
         plan: TrainPlan = ctx.plan
         if ctx.generation != plan.fwd_generation:
@@ -603,7 +631,17 @@ class _DenseFunction(torch.autograd.Function):
                 "backward of a stale forward: another train-mode forward of the same input shape and outputs ran in "
                 "between and overwrote the saved activations of this one (call backward before the next forward)")
         plan.run_backward([None if g is None else g.contiguous().float() for g in grads])
-        return (None, None, *plan.grad_views_on_path())
+        return (None, _train_dx(ctx, plan), *plan.grad_views_on_path())
+
+
+def _train_dx(ctx, plan: TrainPlan):
+    """the image gradient of a train-mode step: a copy of the plan's static buffer (local to this rank: the gradient
+    all-reduce covers parameters only), or None when the plan was built for an input without a gradient"""
+    if not ctx.needs_input_grad[1]:
+        return None
+    if not plan.want_dx:
+        raise L.FvitError("the input requires grad but this train plan was built without the image gradient")
+    return plan.dx.clone()
 
 
 class _EvalGradFunction(torch.autograd.Function):
@@ -611,7 +649,9 @@ class _EvalGradFunction(torch.autograd.Function):
     forward runs the inference launch list unchanged -- bitwise the output of the same call under no_grad, at its speed
     and memory -- and keeps x. backward recomputes: the eval-grad plan (Engine.eval_grad_plan) runs a saving forward on
     x with every BatchNorm on its running statistics, then its backward from the output gradient, which yields the
-    parameter gradients and the image gradient. Each node recomputes on its own, so several forwards may feed one
+    parameter gradients and the image gradient. Which of them autograd asks for (ctx.needs_input_grad) selects the plan:
+    a stage none of whose parameters needs a gradient runs the data-only backward, and is skipped when x needs none
+    either. Each node recomputes on its own, so several forwards may feed one
     backward; nothing is built until the first backward. First order only: the gradients come from raw kernel buffers
     and carry no graph, so a backward through them (create_graph=True, then differentiating dx) raises."""
 
@@ -639,7 +679,8 @@ class _EvalGradFunction(torch.autograd.Function):
         engine, plan = ctx.engine, ctx.plan
         _check_eval_backward(engine.model, plan.weights_key() != ctx.weights_key)
         with torch.cuda.device(x.device):
-            gp = engine.eval_grad_plan(x)
+            needs = dict(zip(map(id, engine._params), ctx.needs_input_grad[3:]))
+            gp = engine.eval_grad_plan(x, ctx.needs_input_grad[2], stage_mask(engine.model, lambda p: needs[id(p)]))
             gp.run_forward(x)
             g = gout.contiguous().float()
             gp.run_backward(g if gp.kind is None else [g])
@@ -675,10 +716,9 @@ class _EvalDenseGradFunction(torch.autograd.Function):
     forward_raw. forward runs the inference extraction unchanged (bitwise the no_grad outputs) and keeps x. backward
     recomputes through the eval levels plan (Engine.eval_dense_plan: a levels-mode TrainPlan with every BatchNorm, the
     level norms included, on running statistics and no stochastic depth), loads the output gradients (an unused output
-    is a zero gradient) and runs its backward. When x needs a gradient the plan is built without a frozen prefix
-    (frozen = -1): in eval mode the prefix computes the same arithmetic, and its weight gradients are computed and then
-    dropped (None for parameters that do not require grad) -- the price of the image gradient through it. Guards and
-    first-order restriction as _EvalGradFunction."""
+    is a zero gradient) and runs its backward. The frozen prefix, and every stage none of whose parameters needs a
+    gradient, is data-only: crossed by the activation gradient alone when x needs one, not emitted otherwise. Guards
+    and first-order restriction as _EvalGradFunction."""
 
     @staticmethod
     def forward(ctx, engine, plan, spec, x: torch.Tensor, *params):
@@ -698,7 +738,8 @@ class _EvalDenseGradFunction(torch.autograd.Function):
         _check_eval_backward(engine.model, (plan.weights_key(), _norm_versions(ctx.outs)) != ctx.weights_key)
         want_dx = ctx.needs_input_grad[3]
         with torch.cuda.device(x.device):
-            gp = engine.eval_dense_plan(x, ctx.outs, -1 if want_dx else ctx.frozen)
+            needs = dict(zip(map(id, ctx.params), ctx.needs_input_grad[4:]))
+            gp = engine.eval_dense_plan(x, ctx.outs, ctx.frozen, want_dx, stage_mask(engine.model, lambda p: needs[id(p)]))
             if len(gp.params) != len(ctx.params) or any(a is not b for a, b in zip(gp.params, ctx.params)):
                 raise L.FvitError("the model's parameters changed between an eval-mode forward and its backward")
             gp.run_forward(x)

@@ -264,10 +264,15 @@ def _emit_downsample_train(self, i: int, src: dict, dst: dict) -> None:
 
 # ====================================================================================== backward
 def _bn_bwd(self, d: dict, gin, g_is_f16: int, ldg: int, g_rows, raw, ldr: int, r_rows, nrows: int, act: int, out,
-            ldo: int, o_rows, row_scale=None) -> None:
+            ldo: int, o_rows, row_scale=None, data_only=False) -> None:
     """BatchNorm2d backward of d (_bn_train) into fp16 rows `out`: batch statistics (fvit_bn_bwd), or the running
-    statistics of an eval-mode plan (fvit_bn_eval_bwd: no mean(dy) terms, one pass)"""
+    statistics of an eval-mode plan (fvit_bn_eval_bwd: no mean(dy) terms, one pass). data_only (running statistics,
+    no stochastic depth: a frozen or eval stage): the streaming fvit_bn_eval_dgrad, dy times the forward's folded scale"""
     bn = d["bn"]
+    if data_only:
+        self._op(self.bwd_ops, "fvit_bn_eval_dgrad", gin, g_is_f16, ldg, g_rows, raw, ldr, r_rows, nrows, bn.num_features,
+                 d["sc"].data_ptr(), d["sh"].data_ptr(), act, None, None, out, ldo, o_rows)
+        return
     if self.eval_grad:
         self._op(self.bwd_ops, "fvit_bn_eval_bwd", gin, g_is_f16, ldg, g_rows, raw, ldr, r_rows, nrows, bn.num_features,
                  bn.running_mean.data_ptr(), bn.running_var.data_ptr(), float(bn.eps), bn.weight.data_ptr(),
@@ -299,21 +304,30 @@ def _conv_wgrad(self, *, dz, lddz, x, ldx, x_rows, rows, cout, cin, shifts, conv
 
 
 def _emit_downsample_bwd(self, ds: dict, src: dict, dst: dict) -> None:
+    """Downsample backward; data-only (with the level in front of it, stage 1 + i): no weight gradient, LayerNorm dx only"""
     ops = self.bwd_ops
+    data_only = self.data_only[1 + ds["i"]]
     Cs, ld, pl_rows, npix = ds["Cs"], ds["ld"], ds["pl_rows"], ds["npix"]
     mod = ds["mod"]
     # gradient of the conv output in plane space (border rows read the buffer's zero row)
     self._op(ops, "fvit_cast_scale_f16", dst["g"].data_ptr(), 2 * Cs, ds["rmap_g"].data_ptr(), pl_rows, 2 * Cs, None, None,
              ds["dY"].data_ptr(), 2 * Cs, None)
     shifts = [p * pl_rows + s for (s, p) in ds["taps"]]
-    _conv_wgrad(self, dz=ds["dY"].data_ptr(), lddz=2 * Cs, x=ds["planes"].data_ptr(), ldx=ld, x_rows=4 * pl_rows,
-                rows=pl_rows, cout=2 * Cs, cin=Cs, shifts=shifts, conv_weight=mod.reduction[0].weight, name=f"ds{ds['i']}")
+    if not data_only:
+        _conv_wgrad(self, dz=ds["dY"].data_ptr(), lddz=2 * Cs, x=ds["planes"].data_ptr(), ldx=ld, x_rows=4 * pl_rows,
+                    rows=pl_rows, cout=2 * Cs, cin=Cs, shifts=shifts, conv_weight=mod.reduction[0].weight,
+                    name=f"ds{ds['i']}")
     for p, tl_ in ds["plane_taps"].items():
         self._bgemm(a=ds["dY"].data_ptr(), a_rows=pl_rows, lda=2 * Cs, b=ds["wT"][p].data_ptr(), b_rows=Cs,
                     ldb=len(tl_) * ds["co_pad"], m=pl_rows, n=Cs, kc=2 * Cs, taps=[(-ds["taps"][t][0], 0) for t in tl_],
                     out_f16=ds["dplanes"].data_ptr() + 2 * p * pl_rows * ld, ld_o16=ld,
                     flops=2.0 * self.B * ds["Ho"] * ds["Wo"] * Cs * 2 * Cs * len(tl_))
     # LayerNorm2d backward: writes the source level's output gradient
+    if data_only:
+        self._op(ops, "fvit_ln_dgrad", ds["dplanes"].data_ptr(), ld, ds["omap"].data_ptr(), ds["xh"].data_ptr(), Cs,
+                 ds["rs"].data_ptr(), mod.norm.weight.data_ptr(), npix, Cs, src["g"].data_ptr(), Cs,
+                 ds["src_rows"].data_ptr(), 0, 0)
+        return
     self._op(ops, "fvit_ln_bwd", ds["dplanes"].data_ptr(), ld, ds["omap"].data_ptr(), ds["xh"].data_ptr(), Cs,
              ds["rs"].data_ptr(), mod.norm.weight.data_ptr(), npix, Cs, src["g"].data_ptr(), Cs, ds["src_rows"].data_ptr(), 0, 0,
              ("scal", 1), self.G(mod.norm.weight), self.G(mod.norm.bias))
@@ -321,8 +335,10 @@ def _emit_downsample_bwd(self, ds: dict, src: dict, dst: dict) -> None:
 
 def _emit_conv_blocks_bwd(self, lv: dict, input_grad: bool = True) -> None:
     """input_grad=False: nothing below reads the gradient of the level's input (the frozen prefix ends here), so the
-    first block's conv1 data-gradient GEMM is not emitted"""
+    first block's conv1 data-gradient GEMM is not emitted. A data-only level: the two BatchNorm passes without their
+    reductions and the two data-gradient GEMMs per block."""
     Cc, rows, ld, npix = lv["C"], lv["rows"], lv["ld"], lv["npix"]
+    data_only = self.data_only[1 + lv["level_index"]]
     g = lv["g"].data_ptr()
     pix, interior = lv["pix"].data_ptr(), lv["interior"].data_ptr()
     shifts = [s for (s, _) in lv["taps"]]
@@ -331,7 +347,7 @@ def _emit_conv_blocks_bwd(self, lv: dict, input_grad: bool = True) -> None:
         # x_out = x_in + BN2(conv2(h)); h = GELU(BN1(conv1(x_in)))
         self._before_write(lv["dzB"].data_ptr())
         _bn_bwd(self, bnB, g, 0, Cc, pix, sv["rawB"].data_ptr(), ld, pix, npix, L.ACT_NONE, lv["dzB"].data_ptr(), ld, pix,
-                sv["rs"])
+                sv["rs"], data_only)
         # h = GELU(BN1(rawA)) was kept by the forward; the pre-activation BN1(rawA) is re-derived inside the dgrad
         # epilogue from rawA and the BatchNorm affine (aux_scale / aux_shift).
         # conv biases sit in front of a batch-statistics BatchNorm: their gradient sum_rows(dz) is identically zero
@@ -339,19 +355,21 @@ def _emit_conv_blocks_bwd(self, lv: dict, input_grad: bool = True) -> None:
         # statistics (eval-mode plan) remove nothing: there it is a column sum of dz.
         bias_b = blk.conv2.bias if self.eval_grad else None
         bias_a = blk.conv1.bias if self.eval_grad else None
-        _conv_wgrad(self, dz=lv["dzB"].data_ptr(), lddz=ld, x=sv["h16"].data_ptr(), ldx=ld, x_rows=rows, rows=rows, cout=Cc,
-                    cin=Cc, shifts=shifts, conv_weight=blk.conv2.weight, name="convB", bias=bias_b, bias_rows=pix,
-                    bias_nrows=npix)
+        if not data_only:
+            _conv_wgrad(self, dz=lv["dzB"].data_ptr(), lddz=ld, x=sv["h16"].data_ptr(), ldx=ld, x_rows=rows, rows=rows,
+                        cout=Cc, cin=Cc, shifts=shifts, conv_weight=blk.conv2.weight, name="convB", bias=bias_b,
+                        bias_rows=pix, bias_nrows=npix)
         self._bgemm(a=lv["dzB"].data_ptr(), a_rows=rows, lda=ld, b=sv["wT2"].data_ptr(), b_rows=Cc, ldb=9 * _ru(Cc, 64),
                     m=rows, n=Cc, kc=Cc, taps=lv["taps"], act=L.ACT_GELU_BWD, aux=sv["rawA"].data_ptr(), ld_aux=ld,
                     aux_scale=bnA["sc"].data_ptr(), aux_shift=bnA["sh"].data_ptr(),
                     row_map=interior, out_f16=lv["dyA"].data_ptr(), ld_o16=ld, flops=2.0 * npix * Cc * Cc * 9)
         self._before_write(lv["dzA"].data_ptr())
         _bn_bwd(self, bnA, lv["dyA"].data_ptr(), 1, ld, pix, sv["rawA"].data_ptr(), ld, pix, npix, L.ACT_NONE,
-                lv["dzA"].data_ptr(), ld, pix)
-        _conv_wgrad(self, dz=lv["dzA"].data_ptr(), lddz=ld, x=sv["xin"].data_ptr(), ldx=ld, x_rows=rows, rows=rows, cout=Cc,
-                    cin=Cc, shifts=shifts, conv_weight=blk.conv1.weight, name="convA", bias=bias_a, bias_rows=pix,
-                    bias_nrows=npix)
+                lv["dzA"].data_ptr(), ld, pix, None, data_only)
+        if not data_only:
+            _conv_wgrad(self, dz=lv["dzA"].data_ptr(), lddz=ld, x=sv["xin"].data_ptr(), ldx=ld, x_rows=rows, rows=rows,
+                        cout=Cc, cin=Cc, shifts=shifts, conv_weight=blk.conv1.weight, name="convA", bias=bias_a,
+                        bias_rows=pix, bias_nrows=npix)
         if sv is lv["blocks_sv"][0] and not input_grad:
             continue
         # g += conv1 data gradient
@@ -365,18 +383,19 @@ def _emit_conv_part_bwd(self) -> None:
     m, B = self.model, self.B
     for idx in range(len(self.conv_lv) - 1, -1, -1):
         lv = self.conv_lv[idx]
-        if idx < self.n_frozen_lv:    # frozen prefix: no dgrad / wgrad / BatchNorm backward below this point
+        if not self._needed(1 + idx):  # nothing below reads a gradient: no dgrad / wgrad / BatchNorm backward from here
             return
         if lv is self.feat:           # levels mode with a conv top level: its output gradient enters here
             self._inject(idx)
-        _emit_conv_blocks_bwd(self, lv, input_grad=(idx - 1 >= self.n_frozen_lv) if idx > 0 else not self.stem_frozen)
+        _emit_conv_blocks_bwd(self, lv, input_grad=self._needed(idx))
         if idx > 0:
-            if idx - 1 < self.n_frozen_lv:
+            if not self._needed(idx):
                 return
             _emit_downsample_bwd(self, lv["ds"], self.conv_lv[idx - 1], lv)
             self._inject(idx - 1)
-    if self.stem_frozen:
+    if not self._needed(0):
         return
+    data_only = self.data_only[0]
     # PatchEmbed
     st, lv0 = self.stem_sv, self.conv_lv[0]
     pe = m.patch_embed.conv_down
@@ -389,11 +408,12 @@ def _emit_conv_part_bwd(self) -> None:
     dY2 = nb.new("stem.dY2", (pl_rows, lv0["ld"]), torch.float16)
     bn2, bn1 = st["bn2"], st["bn1"]
     _bn_bwd(self, bn2, lv0["g"].data_ptr(), 0, dim, lv0["pix"].data_ptr(), st["raw2"].data_ptr(), lv0["ld"],
-            lv0["pix"].data_ptr(), B * H0 * W0, L.ACT_RELU, dY2.data_ptr(), lv0["ld"], q_of_pix.data_ptr())
+            lv0["pix"].data_ptr(), B * H0 * W0, L.ACT_RELU, dY2.data_ptr(), lv0["ld"], q_of_pix.data_ptr(), None, data_only)
     taps = self._s2_taps(W0)
     shifts = [p * pl_rows + s for (s, p) in taps]
-    _conv_wgrad(self, dz=dY2.data_ptr(), lddz=lv0["ld"], x=st["planes"].data_ptr(), ldx=ld_in, x_rows=4 * pl_rows,
-                rows=pl_rows, cout=dim, cin=in_dim, shifts=shifts, conv_weight=pe[3].weight, name="stem2")
+    if not data_only:
+        _conv_wgrad(self, dz=dY2.data_ptr(), lddz=lv0["ld"], x=st["planes"].data_ptr(), ldx=ld_in, x_rows=4 * pl_rows,
+                    rows=pl_rows, cout=dim, cin=in_dim, shifts=shifts, conv_weight=pe[3].weight, name="stem2")
     co_pad = _ru(dim, 64)
     dplanes = nb.new("stem.dplanes16", (4 * pl_rows, ld_in), torch.float16)
     for p in range(4):
@@ -408,12 +428,13 @@ def _emit_conv_part_bwd(self) -> None:
                     flops=2.0 * B * H0 * W0 * in_dim * dim * len(tl_))
     dz1 = nb.new("stem.dz1", (npix1, ld_in), torch.float16)
     _bn_bwd(self, bn1, dplanes.data_ptr(), 1, ld_in, st["stem_map"].data_ptr(), st["raw1"].data_ptr(), ld_in,
-            st["stem_map"].data_ptr(), npix1, L.ACT_RELU, dz1.data_ptr(), ld_in, None)
+            st["stem_map"].data_ptr(), npix1, L.ACT_RELU, dz1.data_ptr(), ld_in, None, None, data_only)
     k1, sld = st["k1"], st["sld"]
-    self._bgemm(a=dz1.data_ptr(), a_rows=npix1, lda=ld_in, a_mn=True, b=st["col16"].data_ptr(), b_rows=npix1, ldb=sld,
-                b_mn=True, m=in_dim, n=k1, kc=npix1, split_k=self._split_k(in_dim, k1, npix1), alpha_ptr=inv,
-                out_f32=self.G(pe[0].weight), ld_o32=k1, flops=2.0 * npix1 * in_dim * k1)
-    if self.eval_grad:
+    if not data_only:
+        self._bgemm(a=dz1.data_ptr(), a_rows=npix1, lda=ld_in, a_mn=True, b=st["col16"].data_ptr(), b_rows=npix1, ldb=sld,
+                    b_mn=True, m=in_dim, n=k1, kc=npix1, split_k=self._split_k(in_dim, k1, npix1), alpha_ptr=inv,
+                    out_f32=self.G(pe[0].weight), ld_o32=k1, flops=2.0 * npix1 * in_dim * k1)
+    if self.want_dx:
         # the image gradient (fp32 NCHW, like x): the backward of conv1, 3x3 / stride 2 / pad 1, as a gather
         cin = m.cfg["in_chans"]
         self.dx = nb.new("stem.dx", (B, cin, self.H, self.W), torch.float32)

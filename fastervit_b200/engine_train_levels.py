@@ -477,7 +477,7 @@ def _build_backward(self) -> None:
     import os
     first = {}
     for name, p in m.named_parameters():
-        if name.startswith("levels."):
+        if name.startswith("levels.") and id(p) in self._goff:
             first.setdefault(int(name.split(".")[1]), self._goff[id(p)])
     # (level norms outside the model have slices after [0, total): they are final once every injection ran, a bucket
     # point of their own at the end)
@@ -495,17 +495,25 @@ def _build_backward(self) -> None:
     elif self.kind == "pooled":
         self._emit_pooled_bwd(self.feat)
     else:
-        for d in self.dense:      # outputs inside the frozen prefix: their norm's weight / bias gradients only
-            if d["level"] < self.n_frozen_lv:
+        for d in self.dense:      # outputs of levels the backward does not reach: their norm's weight / bias gradients only
+            if not self._needed(1 + d["level"]):
                 self._inject(d["level"], g=False)
-        if self.feat["kind"] == "tok" and self.feat["level_index"] >= self.n_frozen_lv:
+        if self.feat["kind"] == "tok" and self._needed(1 + self.feat["level_index"]):
             self._inject(self.feat["level_index"])   # (a conv top level: _emit_conv_part_bwd)
     toks = [lv for lv in self.lv]
     hi = total
     for idx in range(len(toks) - 1, -1, -1):
         tl = toks[idx]
-        if tl["level_index"] < self.n_frozen_lv:
+        if not self._needed(1 + tl["level_index"]):
             break
+        src = toks[idx - 1] if idx > 0 else self.conv_out
+        if self.data_only[1 + tl["level_index"]]:   # no parameter gradient, so no bucket point: the data gradient alone
+            self._emit_token_level_bwd(tl, None)
+            if not self._needed(tl["level_index"]):
+                break
+            self._emit_downsample_bwd(tl["ds"], src, tl)
+            self._inject(tl["level_index"] - 1)
+            continue
         lo = first.get(tl["level_index"], hi)
         # offsets of the level's blocks in the flat buffer (module order = offset order, contiguous)
         spans = []
@@ -526,9 +534,8 @@ def _build_backward(self) -> None:
         else:
             point(lo, hi)
         hi = lo
-        src = toks[idx - 1] if idx > 0 else self.conv_out
-        if tl["level_index"] - 1 < self.n_frozen_lv:
-            break     # the Downsample in front of this level belongs to the frozen prefix: the backward ends here
+        if not self._needed(tl["level_index"]):
+            break     # the Downsample in front of this level belongs to a stage nobody needs a gradient from: the end
         self._emit_downsample_bwd(tl["ds"], src, tl)
         self._inject(tl["level_index"] - 1)
     else:
@@ -590,13 +597,14 @@ def _emit_head_bwd(self, feat: dict) -> None:
     _pool_bn_bwd(self, feat, dpool)
 
 
-def _emit_attn_core_bwd(self, at: dict, dao, dqkv, groups: int, S: int) -> None:
+def _emit_attn_core_bwd(self, at: dict, dao, dqkv, groups: int, S: int, want_dbias: bool = True) -> None:
     """backward of the attention core: the wgmma tile kernel (S <= 64), the wgmma key-loop kernel (S > 64: needs the
     forward's output and log-sum-exp; per-pair partial dQ reduced into an fp32 scratch matrix -- any-res S = 148, the
     14 x 14 ... 48 x 48 windows of the 21k models) or the generic SIMT kernel."""
     attn = at["attn"]
     h, hd, hdp, Cp = attn.num_heads, at["hd"], at["hdp"], at["Cp"]
     ops = self.bwd_ops
+    dbias = at["bias"]["dbias"] if want_dbias else None   # (NULL: every kernel skips the accumulation, fvit.h)
     self._before_write(dqkv.data_ptr())
     if at.get("kind") == "loop":
         # one scratch matrix per plan, sized for the largest attention of the model (the blocks' backward passes run
@@ -608,10 +616,10 @@ def _emit_attn_core_bwd(self, at: dict, dao, dqkv, groups: int, S: int) -> None:
             self._dq_scratch = scr                                                  # launches keep their pointer)
         self._op(ops, "fvit_attn_loop_bwd_long", at["qkv"].data_ptr(), 3 * Cp, dao.data_ptr(), Cp, at["ao"].data_ptr(), Cp,
                  at["lse"].data_ptr(), groups, S, h, hdp, at["bias"]["out"].data_ptr(), at["scale"], dqkv.data_ptr(), 3 * Cp,
-                 at["bias"]["dbias"], scr.data_ptr(), Cp)
+                 dbias, scr.data_ptr(), Cp)
     else:
         self._op(ops, _attn_bwd_entry(S, hdp, at["use_tc"]), at["qkv"].data_ptr(), 3 * Cp, dao.data_ptr(), Cp, groups, S, h, hd,
-                 hdp, at["bias"]["out"].data_ptr(), at["scale"], dqkv.data_ptr(), 3 * Cp, at["bias"]["dbias"])
+                 hdp, at["bias"]["out"].data_ptr(), at["scale"], dqkv.data_ptr(), 3 * Cp, dbias)
     self.bwd_flops[len(ops) - 1] = 10.0 * groups * h * S * S * hd
 
 
@@ -647,13 +655,35 @@ def _bias_bwd(self, bs: dict) -> None:
     self._bwd_side.update(range(n0, len(self.bwd_ops)))
 
 
-def _mlp_bwd(self, tl: dict, ms: dict, gamma, g_ptr: int, rows: int, ln: nn.LayerNorm, xh, rs, in_map=None) -> None:
+_ONE = dict(gamma=None, s=None, inv_s=("scal", 2), w_alpha=("scal", 1))
+
+
+def _data_only_entry(self, tl: dict, br: dict, g_ptr: int, rows: int, Cc: int, rs) -> None:
+    """entry of a data-only residual branch: tl["dz"] = fp16 operand copy of g (layer scale and its normaliser folded
+    in) -- fvit_branch_grad without the bias and layer-scale sums"""
+    self._before_write(tl["dz"].data_ptr())
+    self._op(self.bwd_ops, "fvit_cast_scale_f16", g_ptr, Cc, None, rows, Cc, P(br["gamma"]), br["s"], tl["dz"].data_ptr(), Cc,
+             rs)
+
+
+def _mlp_bwd(self, tl: dict, ms: dict, gamma, g_ptr: int, rows: int, ln: nn.LayerNorm, xh, rs, in_map=None,
+             data_only: bool = False) -> None:
     """Backward of x += gamma * fc2(gelu(fc1(LN(x)))) on gradient rows g_ptr[0:rows]."""
     ops = self.bwd_ops
     mlp = ms["mlp"]
     Cc, hid = mlp.fc1.weight.shape[1], mlp.fc1.weight.shape[0]
     br = self._branch(gamma)
     dz, dp, dy = tl["dz"], tl["dp"], tl["dy"]
+    if data_only:
+        _data_only_entry(self, tl, br, g_ptr, rows, Cc, ms["rs"])
+        self._linear_bwd(lin=mlp.fc2, w16=ms["w2"].data_ptr(), ldw=ms["ld2"], x16=None, ldx=0, dz16=dz.data_ptr(), lddz=Cc,
+                         rows=rows, n_out=Cc, k_in=hid, br=br, dx16=dp.data_ptr(), lddx=hid, dx_act=L.ACT_MUL_AUX,
+                         dx_aux=ms["p16"].data_ptr(), ld_aux=hid, data_only=True)
+        self._linear_bwd(lin=mlp.fc1, w16=ms["w1"].data_ptr(), ldw=ms["ld1"], x16=None, ldx=0, dz16=dp.data_ptr(), lddz=hid,
+                         rows=rows, n_out=hid, k_in=Cc, br=_ONE, dx16=dy.data_ptr(), lddx=Cc, data_only=True)
+        self._op(ops, "fvit_ln_dgrad", dy.data_ptr(), Cc, None, xh.data_ptr(), Cc, rs.data_ptr(), ln.weight.data_ptr(), rows,
+                 Cc, g_ptr, Cc, in_map, 1, 0)
+        return
     fused = Cc % 8 == 0 and mlp.fc2.bias is not None
     self._before_write(dz.data_ptr())
     if fused:   # operand cast + fc2 bias gradient + layer-scale gradient in one pass over g
@@ -680,8 +710,22 @@ def _mlp_bwd(self, tl: dict, ms: dict, gamma, g_ptr: int, rows: int, ln: nn.Laye
              g_ptr, Cc, in_map, 1, 0, ("scal", 1), self.G(ln.weight), self.G(ln.bias))
 
 
+def _attn_data_only(self, tl: dict, at: dict, br: dict, g_ptr: int) -> None:
+    """proj / attention core / qkv data gradients of a data-only level's attention branch, from g into tl["dy"]"""
+    attn = at["attn"]
+    Cc, Cp, rows = attn.qkv.in_features, at["Cp"], at["rows"]
+    dz, dy, dao, dqkv = tl["dz"], tl["dy"], tl["dao"], tl["dqkv"]
+    _data_only_entry(self, tl, br, g_ptr, rows, Cc, at["rs"])
+    self._linear_bwd(lin=attn.proj, w16=at["wp"].data_ptr(), ldw=at["ldp"], x16=None, ldx=0, dz16=dz.data_ptr(), lddz=Cc,
+                     rows=rows, n_out=Cc, k_in=Cp, br=br, dx16=dao.data_ptr(), lddx=Cp, flops_k=Cc, data_only=True)
+    _emit_attn_core_bwd(self, at, dao, dqkv, at["groups"], at["S"], want_dbias=False)
+    self._linear_bwd(lin=attn.qkv, w16=at["wq"].data_ptr(), ldw=at["ldq"], x16=None, ldx=0, dz16=dqkv.data_ptr(),
+                     lddz=3 * Cp, rows=rows, n_out=3 * Cp, k_in=Cc, br=_ONE, dx16=dy.data_ptr(), lddx=Cc,
+                     flops_k=Cc * (3 * Cc) / (3 * Cp), data_only=True)
+
+
 def _attn_bwd(self, tl: dict, at: dict, gamma, g_ptr: int, ln: nn.LayerNorm, xh, rs, in_map, g_base: int,
-              clear_moved: bool) -> None:
+              clear_moved: bool, data_only: bool = False) -> None:
     """Backward of x += gamma * proj(attn(qkv(LN(x)))); g_base = pointer the in_map row indices refer to."""
     ops = self.bwd_ops
     attn = at["attn"]
@@ -689,6 +733,11 @@ def _attn_bwd(self, tl: dict, at: dict, gamma, g_ptr: int, ln: nn.LayerNorm, xh,
     rows, S, groups = at["rows"], at["S"], at["groups"]
     br = self._branch(gamma)
     dz, dy, dao, dqkv = tl["dz"], tl["dy"], tl["dao"], tl["dqkv"]
+    if data_only:
+        _attn_data_only(self, tl, at, br, g_ptr)
+        self._op(ops, "fvit_ln_dgrad", dy.data_ptr(), Cc, None, xh.data_ptr(), Cc, rs.data_ptr(), ln.weight.data_ptr(), rows,
+                 Cc, g_ptr, Cc, in_map, 1, 1 if clear_moved else 0)
+        return
     padded = hdp != hd
     fused = Cc % 8 == 0 and attn.proj.bias is not None
     self._before_write(dz.data_ptr())
@@ -748,46 +797,54 @@ def _unpad_row_map(self, heads3: int, hd: int, hdp: int) -> int:
 
 
 def _emit_token_level_bwd(self, tl: dict, after_block=None) -> None:
+    """A data-only level (TrainPlan.data_only): the data-gradient GEMMs, the attention core without dbias, LayerNorm dx
+    and the carrier-token routing -- no weight-gradient GEMM, no bias / layer-scale / positional-MLP gradient."""
     B, Cc, S, ncw, ws = self.B, tl["C"], tl["S"], tl["ncw"], tl["ws"]
     nW, n_ct = tl["nW"], tl["n_ct"]
     ops = self.bwd_ops
     g_ptr = tl["g"].data_ptr()
     has_ct = ncw > 0
     rows = nW * S
+    do = self.data_only[1 + tl["level_index"]]
     for sv in reversed(tl["blocks_sv"]):
         blk = sv["blk"]
         w = sv["w"]
         if sv.get("prop"):
             g1 = blk.gamma1 if isinstance(blk.gamma1, torch.Tensor) else None
             self._op(ops, "fvit_propagate_bwd", g_ptr, Cc, tl["xs"].data_ptr(), Cc, tl["prop_src"].data_ptr(), rows, Cc,
-                     P(g1), ("scal", 1), self.G(g1) if g1 is not None else None)
+                     P(g1), ("scal", 1), self.G(g1) if g1 is not None and not do else None)
         # window branch (reverse order): MLP, attention + norm1 (routes carrier-slot gradients to the raster buffer)
-        _mlp_bwd(self, tl, sv["w_mlp"], blk.gamma4, g_ptr, rows, blk.norm2, w["xh2"], w["rs2"])
+        _mlp_bwd(self, tl, sv["w_mlp"], blk.gamma4, g_ptr, rows, blk.norm2, w["xh2"], w["rs2"], data_only=do)
         _attn_bwd(self, tl, sv["w_attn"], blk.gamma3, g_ptr, blk.norm1, w["xh1"], w["rs1"],
-                  tl["norm1_gather"].data_ptr() if has_ct else None, g_ptr, True)
-        # positional embedding of the window tokens: sum over windows of the gradient at (x + pe)
-        self._op(ops, "fvit_group_sum", g_ptr, Cc, nW, S, ncw, Cc, ("scal", 1), sv["pe"]["dout"])
-        _posemb_bwd(self, sv["pe"])
+                  tl["norm1_gather"].data_ptr() if has_ct else None, g_ptr, True, data_only=do)
+        if not do:
+            # positional embedding of the window tokens: sum over windows of the gradient at (x + pe)
+            self._op(ops, "fvit_group_sum", g_ptr, Cc, nW, S, ncw, Cc, ("scal", 1), sv["pe"]["dout"])
+            _posemb_bwd(self, sv["pe"])
         if has_ct:
             c = sv["c"]
             gc_ptr = g_ptr + tl["ctr0"] * Cc * 4
             rows_c = B * n_ct
-            _mlp_bwd(self, tl, sv["c_mlp"], blk.gamma2, gc_ptr, rows_c, blk.hat_norm2, c["xh2"], c["rs2"])
+            _mlp_bwd(self, tl, sv["c_mlp"], blk.gamma2, gc_ptr, rows_c, blk.hat_norm2, c["xh2"], c["rs2"], data_only=do)
             # carrier attention; its LayerNorm gathered from the xs carrier rows (ct_dewindow): the
             # gradient goes back there (row indices are relative to the level's g buffer)
-            _attn_bwd_carrier(self, tl, sv, blk, gc_ptr, g_ptr)
+            _attn_bwd_carrier(self, tl, sv, blk, gc_ptr, g_ptr, data_only=do)
         if after_block is not None:
             after_block(tl["blocks_sv"].index(sv))   # this block's parameter gradients are final
     level = self.model.levels[tl["level_index"]]
     if level.do_gt and has_ct:
         tk = level.global_tokenizer
         (kh, sh_, oh), (kw, sw_, ow) = tk.pool
+        if do:
+            self._op(ops, "fvit_token_init_dgrad", g_ptr, Cc, tl["pix_map"].data_ptr(), tl["ct_rows"].data_ptr(), B, tl["Hp"],
+                     tl["Wp"], Cc, tk.pos_embed.weight.data_ptr(), kh, kw, sh_, sw_, oh, ow, g_ptr, Cc)
+            return
         self._op(ops, "fvit_token_init_bwd", g_ptr, Cc, tl["x0_16"].data_ptr(), Cc, tl["pix_map"].data_ptr(),
                  tl["ct_rows"].data_ptr(), B, tl["Hp"], tl["Wp"], Cc, tk.pos_embed.weight.data_ptr(), kh, kw, sh_, sw_, oh, ow,
                  ("scal", 1), g_ptr, Cc, self.G(tk.pos_embed.weight), self.G(tk.pos_embed.bias))
 
 
-def _attn_bwd_carrier(self, tl: dict, sv: dict, blk, gc_ptr: int, g_ptr: int) -> None:
+def _attn_bwd_carrier(self, tl: dict, sv: dict, blk, gc_ptr: int, g_ptr: int, data_only: bool = False) -> None:
     """hat_attn + hat_norm1 backward. ln_bwd works on row indices of one buffer, so the raster rows are
     addressed as rows of the level buffer (offset ctr0) and in_map = ct_gather (xs carrier rows)."""
     ops = self.bwd_ops
@@ -800,6 +857,13 @@ def _attn_bwd_carrier(self, tl: dict, sv: dict, blk, gc_ptr: int, g_ptr: int) ->
     h, hd, hdp, Cp = attn.num_heads, at["hd"], at["hdp"], at["Cp"]
     br = self._branch(blk.gamma1)
     dz, dy, dao, dqkv = tl["dz"], tl["dy"], tl["dao"], tl["dqkv"]
+    if data_only:
+        # the same three data gradients; hat_norm1's dx accumulated in place, then moved to the xs carrier rows
+        _attn_data_only(self, tl, at, br, gc_ptr)
+        self._op(ops, "fvit_ln_dgrad", dy.data_ptr(), Cc, None, c["xh1"].data_ptr(), Cc, c["rs1"].data_ptr(),
+                 blk.hat_norm1.weight.data_ptr(), rows_c, Cc, gc_ptr, Cc, None, 1, 0)
+        self._op(ops, "fvit_scatter_add_rows", gc_ptr, Cc, g_ptr, Cc, tl["ct_gather"].data_ptr(), rows_c, Cc)
+        return
     padded = hdp != hd
     fused = Cc % 8 == 0 and attn.proj.bias is not None
     self._before_write(dz.data_ptr())

@@ -148,6 +148,10 @@ _OP_SIGS: dict[str, list] = {
     "fvit_pool_bn_eval_bwd": [_P, _L, _P, _I, _I, _I, _P, _P, _F, _P, _P, _L, _P, _P, _L, _P, _P, _P],
     "fvit_stem_conv_dgrad": [_P, _L, _I, _I, _I, _P, _I, _P, _P, _P],
     "fvit_stem_col2im": [_P, _L, _I, _I, _I, _I, _P, _P],
+    # data-only backward stages (include/fvit.h "Data-only backward")
+    "fvit_bn_eval_dgrad": [_P, _I, _L, _P, _P, _L, _P, _I, _I, _P, _P, _I, _P, _P, _P, _L, _P, _P],
+    "fvit_ln_dgrad": [_P, _L, _P, _P, _L, _P, _P, _I, _I, _P, _L, _P, _I, _I, _P],
+    "fvit_token_init_dgrad": [_P, _L, _P, _P, _I, _I, _I, _I, _P, _I, _I, _I, _I, _I, _I, _P, _L, _P],
     # optimizer step (include/fvit.h "optimizer step on the flat gradient buffer")
     "fvit_optim_gather_f32": [_P, _I, _P, _P, _P, _P],
     "fvit_optim_sqnorm": [_P, _I, _P, _P, _P, _P],

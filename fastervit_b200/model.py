@@ -252,6 +252,7 @@ class FasterViT(nn.Module):
         self.apply(self._init_weights)
         self._engine = None
         self._grad_allreduce = None
+        self._train_input_grad = False
 
     # fv.py:930-943: Linear trunc_normal(.02)/zero bias, norms to identity, convs keep torch default
     def _init_weights(self, m):
@@ -290,6 +291,15 @@ class FasterViT(nn.Module):
         gradient buffer is averaged over `group` (default: the world) with a single NCCL all-reduce — the one
         collective of the path (train.py:551). Parameters must start identical on all ranks."""
         self._grad_allreduce = True if group is None else group
+
+    def enable_input_grad(self, enabled: bool = True):
+        """Train-mode image gradients: after this, an input with requires_grad under .train() gets its gradient
+        (x.grad, fp32, local to the rank) from model(x), forward_features, forward_levels and the pooled features of a
+        num_classes = 0 model -- a trainable front end, pixel-space prompts, adversarial training. Without it such an
+        input raises, as it always did: the plan for it is a second one per input shape, and a caller that merely forgot
+        to detach should hear about it. Eval mode needs no switch."""
+        self._train_input_grad = bool(enabled)
+        return self
 
     def switch_to_deploy(self):
         """Put every positional-embedding module into deploy mode (the reference exposes `switch_to_deploy` per module,

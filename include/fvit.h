@@ -479,6 +479,30 @@ int fvit_token_init_bwd(const float* g, int64_t ldg, const void* x16, int64_t ld
 int fvit_propagate_bwd(float* g, int64_t ldg, const float* xs, int64_t ldx, const int32_t* src_map, int32_t rows, int32_t C,
                        const float* gamma, const float* scalar, float* dgamma, void* stream);
 
+/* ---- Data-only backward: the activation gradient through a stage whose parameters get no gradient ----
+ * (a frozen prefix that an image gradient crosses; an eval-mode input gradient with the parameters frozen). The plans
+ * then emit the data-gradient GEMMs and the attention-core backward (dbias = NULL) as they are, fvit_cast_scale_f16
+ * for the branch entry, fvit_propagate_bwd with dgamma = NULL, and the three entry points below in place of
+ * fvit_bn_eval_bwd / fvit_ln_bwd / fvit_token_init_bwd: the same arithmetic for the data gradient, no parameter sums. */
+/* Running-statistics BatchNorm2d, data gradient alone: out16[o_rows[r]][c] = scale[c] * colmul[c] * *scalar * dy with
+ * dy = gin[g_rows[r]][c] (fp32 or fp16), zeroed where act == FVIT_ACT_RELU and raw16[r_rows[r]][c] * scale[c] +
+ * shift[c] <= 0. scale / shift are the forward's folded BatchNorm (fvit_affine_fold: w * rsqrt(var + eps) and
+ * b - mean * scale); colmul, scalar, the row maps optional; raw16 / shift only read for the ReLU mask. A row whose map
+ * entry is negative is skipped. One streaming pass, no reductions, no atomics; 16-byte accesses and zeroed padding
+ * columns under the layout conditions of fvit_bn_eval_bwd. */
+int fvit_bn_eval_dgrad(const void* gin, int32_t g_is_f16, int64_t ldg, const int32_t* g_rows, const void* raw16,
+                       int64_t ldr, const int32_t* r_rows, int32_t nrows, int32_t C, const float* scale,
+                       const float* shift, int32_t act, const float* colmul, const float* scalar, void* out16,
+                       int64_t ldo, const int32_t* o_rows, void* stream);
+/* The g update of fvit_ln_bwd without dgamma / dbeta (same dy_map / in_map / use_g / clear_moved conventions). */
+int fvit_ln_dgrad(const void* dy16, int64_t lddy, const int32_t* dy_map, const void* xhat16, int64_t ldxh,
+                  const float* rstd, const float* gamma, int32_t rows, int32_t C, float* g, int64_t ldg,
+                  const int32_t* in_map, int32_t use_g, int32_t clear_moved, void* stream);
+/* The gx update of fvit_token_init_bwd without dw / dbias (and so without the fp16 copy of the level input). */
+int fvit_token_init_dgrad(const float* g, int64_t ldg, const int32_t* pix_map, const int32_t* ct_row_map, int32_t B,
+                          int32_t Hp, int32_t Wp, int32_t C, const float* w, int32_t kh, int32_t kw, int32_t sh,
+                          int32_t sw, int32_t oh, int32_t ow, float* gx, int64_t ldgx, void* stream);
+
 /* ---- optimizer step on the flat gradient buffer (SURVEY §8 f.1; train.py:879-899) -----------------------
  * Replaces, for the training loop either side of loss.backward(): GradScaler.unscale_ + the non-finite check,
  * dispatch_clip_grad(..., mode='norm') (`--clip-grad 5.0`), optimizer.step() for `--opt adamw` / `--opt lamb`
