@@ -31,6 +31,11 @@ def _ru(x: int, m: int) -> int:
     return (x + m - 1) // m * m
 
 
+def P(t):
+    """device pointer of an optional tensor"""
+    return None if t is None else t.data_ptr()
+
+
 # ---------------------------------------------------------------------------------- index maps
 def _ct_dewindow_perm(cs: int, sr: list[int]) -> torch.Tensor:
     """raster position r -> window-major carrier index it is read from; the literal index algebra of
@@ -172,28 +177,49 @@ class Plan:
     def _op(self, target: list, name: str, *args) -> None:
         target.append((getattr(self.lib, name), args, name))
 
-    def _gemm(self, *, a, a_rows, lda, b, ldb, m, n, kc, taps=None, a_planes=1, a_plane_stride=0,
-              b_rows=0, col_scale=None, col_shift=None, col_scale2=None, act=L.ACT_NONE, resid=None,
-              ld_resid=0, row_map=None, out_f32=None, ld_o32=0, out_f16=None, ld_o16=0,
-              col_sum=None, col_sumsq=None, alpha=1.0, tile_n=0, m_alg=None) -> None:
-        """Emit one fvit_gemm launch. m_alg = number of output rows that are real work (pixels / tokens,
-        without layout padding) for the algorithmic FLOP count 2*m_alg*n*kc*ntaps."""
+    def _gemm(self, *, a, a_rows, lda, b, ldb, m, n, kc, b_rows=0, taps=None, a_planes=1, a_plane_stride=0,
+              a_mn=False, b_mn=False, b_taps=None, split_k=1, alpha_ptr=None, act=L.ACT_NONE, col_scale=None, col_shift=None, col_scale2=None, row_scale=None, aux=None, ld_aux=0,
+              aux_scale=None, aux_shift=None, resid=None, ld_resid=0, row_map=None, out_f32=None, ld_o32=0,
+              out_f16=None, ld_o16=0, out_pre16=None, ld_pre16=0, pre_is_grad=False, col_sum=None, col_sumsq=None,
+              out_colsum=None, out_colsum_alpha=None, target=None, m_alg=None, flops=None) -> None:
+        """Emit one fvit_gemm launch (fields: GemmArgs, include/fvit.h) into `target` (default: the forward list) and
+        record its algorithmic FLOPs in op_flops / bwd_flops: `flops`, else 2*m_alg*n*kc*ntaps with m_alg = the number
+        of output rows that are real work (pixels / tokens, without layout padding). A pointer may be symbolic,
+        ("scal" | "scr", i): TrainPlan._finish_train resolves it once its device scalars and scratch exist."""
         g = L.GemmArgs()
-        g.a, g.a_rows, g.lda, g.a_plane_stride, g.a_planes = a, a_rows, lda, a_plane_stride, a_planes
-        g.b, g.b_rows, g.ldb = b, b_rows or n, ldb
+        g.a_rows, g.lda, g.a_plane_stride, g.a_planes, g.a_mn_major = a_rows, lda, a_plane_stride, a_planes, int(a_mn)
+        g.b_rows, g.ldb, g.b_mn_major = b_rows or n, ldb, int(b_mn)
         g.m, g.n, g.kc = m, n, kc
         taps = taps or [(0, 0)]
         g.ntaps = len(taps)
         for i, (s, p) in enumerate(taps):
             g.tap_shift[i], g.tap_plane[i] = s, p
-        g.split_k, g.tile_n, g.alpha, g.act = 1, tile_n, alpha, act
-        g.col_scale, g.col_shift, g.col_scale2 = col_scale, col_shift, col_scale2
-        g.resid, g.ld_resid, g.row_map = resid, ld_resid, row_map
-        g.out_f32, g.ld_out_f32, g.out_f16, g.ld_out_f16 = out_f32, ld_o32, out_f16, ld_o16
-        g.col_sum, g.col_sumsq = col_sum, col_sumsq
+        if b_taps is not None:   # conv weight gradient: taps folded into N (include/fvit.h: b_ntaps)
+            assert len(taps) == 1 and a_mn and b_mn
+            g.b_ntaps = len(b_taps)
+            for i, sft in enumerate(b_taps):
+                g.tap_shift[i] = sft
+        g.split_k, g.alpha, g.act, g.pre_is_grad = split_k, 1.0, act, int(pre_is_grad)
+        g.ld_aux, g.ld_resid, g.ld_out_f32, g.ld_out_f16, g.ld_out_pre16 = ld_aux, ld_resid, ld_o32, ld_o16, ld_pre16
+        g._sym = {}
+        for f, v in (("a", a), ("b", b), ("alpha_ptr", alpha_ptr), ("col_scale", col_scale), ("col_shift", col_shift),
+                     ("col_scale2", col_scale2), ("row_scale", row_scale), ("aux", aux), ("aux_scale", aux_scale),
+                     ("aux_shift", aux_shift), ("resid", resid), ("row_map", row_map), ("out_f32", out_f32),
+                     ("out_f16", out_f16), ("out_pre16", out_pre16), ("col_sum", col_sum), ("col_sumsq", col_sumsq),
+                     ("out_colsum", out_colsum), ("out_colsum_alpha", out_colsum_alpha)):
+            if isinstance(v, tuple):
+                g._sym[f] = v
+            else:
+                setattr(g, f, v)
         self._gemm_keep.append(g)
-        self.ops.append((self.lib.fvit_gemm, (C.byref(g),), "fvit_gemm"))
-        self.op_flops[len(self.ops) - 1] = 2.0 * (m_alg if m_alg is not None else m) * n * kc * len(taps)
+        lst = self.ops if target is None else target
+        lst.append((self.lib.fvit_gemm, (C.byref(g),), "fvit_gemm"))
+        if flops is None:
+            flops = 2.0 * (m_alg if m_alg is not None else m) * n * kc * len(taps)
+        if lst is self.ops:
+            self.op_flops[len(lst) - 1] = flops
+        elif lst is getattr(self, "bwd_ops", None):
+            self.bwd_flops[len(lst) - 1] = flops
 
     # ---- weight preparation emitters ------------------------------------------------------------
     def _pack_linear(self, name: str, lin: nn.Linear) -> tuple[torch.Tensor, int]:
@@ -215,12 +241,11 @@ class Plan:
         """(scale, shift) device vectors for the GEMM epilogue; see fvit_affine_fold."""
         sc = self.bufs.new(name + ".scale", (n,), torch.float32)
         sh = self.bufs.new(name + ".shift", (n,), torch.float32)
-        p = lambda t: None if t is None else t.data_ptr()
         self._op(self.prep_ops, "fvit_affine_fold", sc.data_ptr(), sh.data_ptr(), n,
-                 p(bn.weight) if bn is not None else None, p(bn.bias) if bn is not None else None,
-                 p(bn.running_mean) if bn is not None else None,
-                 p(bn.running_var) if bn is not None else None,
-                 float(bn.eps) if bn is not None else 0.0, p(bias), p(ls))
+                 P(bn.weight) if bn is not None else None, P(bn.bias) if bn is not None else None,
+                 P(bn.running_mean) if bn is not None else None,
+                 P(bn.running_var) if bn is not None else None,
+                 float(bn.eps) if bn is not None else 0.0, P(bias), P(ls))
         return sc, sh
 
     # ---- plan construction ----------------------------------------------------------------------
@@ -238,10 +263,7 @@ class Plan:
         ld_in = _ru(in_dim, 8)
         pl_rows = B * (H0 + 1) * (W0 + 1)
         stem_planes = nb.new("stem.planes", (4 * pl_rows, ld_in), torch.float16)
-        bi, yi, xi = torch.meshgrid(torch.arange(B), torch.arange(H1), torch.arange(W1), indexing="ij")
-        plane = (yi & 1) * 2 + (xi & 1)
-        stem_map = nb.i32("stem.map", (plane * pl_rows + bi * (H0 + 1) * (W0 + 1)
-                                       + ((yi >> 1) + 1) * (W0 + 1) + (xi >> 1) + 1).reshape(-1))
+        stem_map = self._parity_plane_map("stem.map", H1, W1)
         pe = m.patch_embed.conv_down
         s1, t1 = self._fold("stem.bn1", in_dim, pe[1])
         # conv1 (fv.py:458-460) on tensor cores: im2col rows [pixel, 9*in_chans -> stem_ld] (one HBM-bound
@@ -254,8 +276,8 @@ class Plan:
         self._op(self.prep_ops, "fvit_cast_pad_f16", pe[0].weight.data_ptr(), k1, w1.data_ptr(), sld, in_dim, k1, sld)
         self._gemm(a=col16.data_ptr(), a_rows=B * H1 * W1, lda=sld, b=w1.data_ptr(), ldb=sld,
                    m=B * H1 * W1, n=in_dim, kc=sld, col_scale=s1.data_ptr(), col_shift=t1.data_ptr(),
-                   act=L.ACT_RELU, row_map=stem_map.data_ptr(), out_f16=stem_planes.data_ptr(), ld_o16=ld_in)
-        self.op_flops[len(self.ops) - 1] = 2.0 * B * H1 * W1 * in_dim * k1
+                   act=L.ACT_RELU, row_map=stem_map.data_ptr(), out_f16=stem_planes.data_ptr(), ld_o16=ld_in,
+                   flops=2.0 * B * H1 * W1 * in_dim * k1)
 
         lvl = self._conv_level_buffers(0, dim, H0, W0)
         w16, ldw = self._pack_conv("stem.conv2", pe[3])
@@ -263,8 +285,7 @@ class Plan:
         self._gemm(a=stem_planes.data_ptr(), a_rows=pl_rows, lda=ld_in, a_planes=4,
                    a_plane_stride=pl_rows * ld_in, b=w16.data_ptr(), ldb=ldw, m=pl_rows, n=dim, kc=in_dim,
                    taps=self._s2_taps(W0), col_scale=s2.data_ptr(), col_shift=t2.data_ptr(), act=L.ACT_RELU,
-                   m_alg=B * H0 * W0,
-                   row_map=self._plane_to_padded_map("stem.to_l0", B, H0, W0).data_ptr(),
+                   m_alg=lvl["npix"], row_map=self._plane_to_padded_map("stem.to_l0", B, H0, W0).data_ptr(),
                    out_f32=lvl["x32"].data_ptr(), ld_o32=lvl["C"], out_f16=lvl["x16"].data_ptr(),
                    ld_o16=lvl["ld"])
 
@@ -335,6 +356,16 @@ class Plan:
                 taps.append((da * (Wo + 1) + db, ph * 2 + pw))
         return taps
 
+    def _parity_plane_map(self, name: str, H: int, W: int) -> torch.Tensor:
+        """pixel (b, y, x) of an H x W map -> its row in the four parity planes that feed a 3x3 stride-2 convolution:
+        plane (y&1)*2 + (x&1), plane row (y>>1)+1 and column (x>>1)+1 behind the zero top row / left column."""
+        B = self.B
+        Ho, Wo = (H + 1) // 2, (W + 1) // 2
+        pl_rows = B * (Ho + 1) * (Wo + 1)
+        bi, yi, xi = torch.meshgrid(torch.arange(B), torch.arange(H), torch.arange(W), indexing="ij")
+        return self.bufs.i32(name, (((yi & 1) * 2 + (xi & 1)) * pl_rows + bi * (Ho + 1) * (Wo + 1)
+                                    + ((yi >> 1) + 1) * (Wo + 1) + (xi >> 1) + 1).reshape(-1))
+
     def _plane_to_padded_map(self, name: str, B: int, Ho: int, Wo: int) -> torch.Tensor:
         """plane-space output row (b, a+1, c+1) -> zero-bordered level row; border rows -> -1."""
         bi, ai, ci = torch.meshgrid(torch.arange(B), torch.arange(Ho + 1), torch.arange(Wo + 1), indexing="ij")
@@ -342,7 +373,18 @@ class Plan:
         dst = torch.where((ai >= 1) & (ci >= 1), dst, torch.full_like(dst, -1))
         return self.bufs.i32(name, dst.reshape(-1))
 
-    def _conv_level_buffers(self, i: int, Cc: int, Hc: int, Wc: int) -> dict:
+    def _downsample_row_map(self, i: int, dst: dict, Ho: int, Wo: int) -> torch.Tensor:
+        """plane-space output row (b, a+1, c+1) of Downsample i -> the row of pixel (a, c) in the next level: its
+        zero-bordered conv map, or its window-major token buffer (dst["pix_map_host"]); border rows -> -1."""
+        if "pix_map_host" not in dst:
+            return self._plane_to_padded_map(f"ds{i}.rmap", self.B, Ho, Wo)
+        full = torch.full((self.B, Ho + 1, Wo + 1), -1, dtype=torch.int64)
+        full[:, 1:, 1:] = dst["pix_map_host"][:, :Ho, :Wo]
+        return self.bufs.i32(f"ds{i}.rmap", full.reshape(-1))
+
+    def _conv_level_buffers(self, i: int, Cc: int, Hc: int, Wc: int, f16=("x16", "h16")) -> dict:
+        """geometry, row maps and buffers of a conv level's zero-bordered map: the fp32 residual stream x32 and one
+        [rows, ld] fp16 matrix per name in f16"""
         B, nb = self.B, self.bufs
         rows = B * (Hc + 2) * (Wc + 2)
         ld = _ru(Cc, 8)
@@ -351,10 +393,11 @@ class Plan:
         ident = torch.arange(rows).view(B, Hc + 2, Wc + 2)
         interior = nb.i32(f"l{i}.interior", torch.where(inside, ident, torch.full_like(ident, -1)).reshape(-1))
         pix = nb.i32(f"l{i}.pix", ident[:, 1:-1, 1:-1].reshape(-1))  # pixel (b,y,x) -> padded row
-        return dict(C=Cc, H=Hc, W=Wc, ld=ld, rows=rows, interior=interior, pix=pix,
-                    x32=nb.new(f"l{i}.x32", (rows, Cc), torch.float32),
-                    x16=nb.new(f"l{i}.x16", (rows, ld), torch.float16),
-                    h16=nb.new(f"l{i}.h16", (rows, ld), torch.float16))
+        d = dict(C=Cc, H=Hc, W=Wc, ld=ld, rows=rows, npix=B * Hc * Wc, interior=interior, pix=pix,
+                 x32=nb.new(f"l{i}.x32", (rows, Cc), torch.float32))
+        for k in f16:
+            d[k] = nb.new(f"l{i}.{k}", (rows, ld), torch.float16)
+        return d
 
     # ---- conv levels ------------------------------------------------------------------------------
     def _emit_conv_blocks(self, i: int, level, lv: dict) -> None:
@@ -369,12 +412,12 @@ class Plan:
             # h = GELU(BN(conv1(x)))                                        (fv.py:504-506)
             self._gemm(a=lv["x16"].data_ptr(), a_rows=lv["rows"], lda=lv["ld"], b=w1.data_ptr(), ldb=ld1,
                        m=lv["rows"], n=Cc, kc=Cc, taps=taps, col_scale=s1.data_ptr(), col_shift=t1.data_ptr(),
-                       m_alg=self.B * lv["H"] * lv["W"], act=L.ACT_GELU, row_map=lv["interior"].data_ptr(), out_f16=lv["h16"].data_ptr(),
+                       m_alg=lv["npix"],act=L.ACT_GELU, row_map=lv["interior"].data_ptr(), out_f16=lv["h16"].data_ptr(),
                        ld_o16=lv["ld"])
             # x = x + gamma * BN(conv2(h))                                   (fv.py:507-511)
             self._gemm(a=lv["h16"].data_ptr(), a_rows=lv["rows"], lda=lv["ld"], b=w2.data_ptr(), ldb=ld2,
                        m=lv["rows"], n=Cc, kc=Cc, taps=taps, col_scale=s2.data_ptr(), col_shift=t2.data_ptr(),
-                       m_alg=self.B * lv["H"] * lv["W"], resid=lv["x32"].data_ptr(), ld_resid=Cc, row_map=lv["interior"].data_ptr(),
+                       m_alg=lv["npix"],resid=lv["x32"].data_ptr(), ld_resid=Cc, row_map=lv["interior"].data_ptr(),
                        out_f32=lv["x32"].data_ptr(), ld_o32=Cc, out_f16=lv["x16"].data_ptr(), ld_o16=lv["ld"])
             self._mark(f"levels.{i}.blocks.{j}", kind="conv", lv=lv)
 
@@ -388,9 +431,7 @@ class Plan:
         ld = _ru(Cs, 8)
         pl_rows = B * (Ho + 1) * (Wo + 1)
         planes = nb.new(f"ds{i}.planes", (4 * pl_rows, ld), torch.float16)
-        bi, yi, xi = torch.meshgrid(torch.arange(B), torch.arange(Hs), torch.arange(Ws), indexing="ij")
-        omap = nb.i32(f"ds{i}.omap", (((yi & 1) * 2 + (xi & 1)) * pl_rows + bi * (Ho + 1) * (Wo + 1)
-                                      + ((yi >> 1) + 1) * (Wo + 1) + (xi >> 1) + 1).reshape(-1))
+        omap = self._parity_plane_map(f"ds{i}.omap", Hs, Ws)
         src_rows = src["pix"] if src["kind"] == "conv" else src["crop_map"]
         src_x = src["x32"] if src["kind"] == "conv" else src["xs"]
         self._op(self.ops, "fvit_ln_fwd", src_x.data_ptr(), Cs, src_rows.data_ptr(), B * Hs * Ws, Cs,
@@ -398,20 +439,13 @@ class Plan:
                  planes.data_ptr(), ld, omap.data_ptr(), None, None, None, 0)
         w16, ldw = self._pack_conv(f"ds{i}.conv", ds.reduction[0])
         if to_conv:
-            rmap = self._plane_to_padded_map(f"ds{i}.rmap", B, Ho, Wo)
-            self._gemm(a=planes.data_ptr(), a_rows=pl_rows, lda=ld, a_planes=4, a_plane_stride=pl_rows * ld,
-                       b=w16.data_ptr(), ldb=ldw, m=pl_rows, n=2 * Cs, kc=Cs, taps=self._s2_taps(Wo),
-                       m_alg=B * Ho * Wo, row_map=rmap.data_ptr(), out_f32=dst["x32"].data_ptr(), ld_o32=dst["C"],
-                       out_f16=dst["x16"].data_ptr(), ld_o16=dst["ld"])
+            out = dict(out_f32=dst["x32"].data_ptr(), out_f16=dst["x16"].data_ptr(), ld_o16=dst["ld"])
         else:
-            # plane-space row (b, a+1, c+1) -> token row of pixel (a, c) in the window-major buffer
-            pm = dst["pix_map_host"]  # [B, Hp, Wp]
-            full = torch.full((B, Ho + 1, Wo + 1), -1, dtype=torch.int64)
-            full[:, 1:, 1:] = pm[:, :Ho, :Wo]
-            rmap = nb.i32(f"ds{i}.rmap", full.reshape(-1))
-            self._gemm(a=planes.data_ptr(), a_rows=pl_rows, lda=ld, a_planes=4, a_plane_stride=pl_rows * ld,
-                       b=w16.data_ptr(), ldb=ldw, m=pl_rows, n=2 * Cs, kc=Cs, taps=self._s2_taps(Wo),
-                       m_alg=B * Ho * Wo, row_map=rmap.data_ptr(), out_f32=dst["xs"].data_ptr(), ld_o32=dst["C"])
+            out = dict(out_f32=dst["xs"].data_ptr())
+        rmap = self._downsample_row_map(i, dst, Ho, Wo)
+        self._gemm(a=planes.data_ptr(), a_rows=pl_rows, lda=ld, a_planes=4, a_plane_stride=pl_rows * ld,
+                   b=w16.data_ptr(), ldb=ldw, m=pl_rows, n=2 * Cs, kc=Cs, taps=self._s2_taps(Wo),
+                   m_alg=B * Ho * Wo, row_map=rmap.data_ptr(), ld_o32=dst["C"], **out)
 
     # ---- transformer levels -----------------------------------------------------------------------
     def _token_level_buffers(self, i: int, level, Cc: int, Hc: int, Wc: int) -> dict:
@@ -502,20 +536,7 @@ class Plan:
         if not use_tc:
             hdp = hd
         Cp = h * hdp
-        qb = attn.qkv.bias
-        if hdp == hd:
-            wq, ldq = self._pack_linear(nm + ".qkv", attn.qkv)
-            qb_ptr = qb.data_ptr() if qb is not None else None
-        else:
-            ldq = _ru(Cc, 8)
-            wq = self.bufs.new(nm + ".qkv.w16", (3 * Cp, ldq), torch.float16)
-            self._op(self.prep_ops, "fvit_cast_headpad_f16", attn.qkv.weight.data_ptr(), Cc, wq.data_ptr(), ldq,
-                     3 * Cp, Cc, hd, hdp, 1, 0)
-            qb_ptr = None
-            if qb is not None:
-                qbp = self.bufs.new(nm + ".qkv.bias_pad", (3 * Cp,), torch.float32)
-                self._op(self.prep_ops, "fvit_vec_headpad_f32", qb.data_ptr(), qbp.data_ptr(), 3 * Cp, hd, hdp)
-                qb_ptr = qbp.data_ptr()
+        wq, ldq, qb_ptr, wp, ldp = self._pack_attention(nm, attn, hdp)
         scale = float(getattr(attn, "scale", hd ** -0.5))   # qk_scale or head_dim ** -0.5 (fv.py:544)
         fused = (self._attn_kind(S, hdp) == "tile" and self.fused_hat != "0"
                  and (self.fused_hat == "1" or hdp == 64))
@@ -544,55 +565,77 @@ class Plan:
         # proj: K dimension is the (head-padded) attention output
         lin = attn.proj
         n = lin.weight.shape[0]
-        if hdp == hd:
-            wp, ldp = self._pack_linear(nm + ".proj", lin)
-        else:
-            ldp = Cp
-            wp = self.bufs.new(nm + ".proj.w16", (n, Cp), torch.float16)
-            self._op(self.prep_ops, "fvit_cast_headpad_f16", lin.weight.data_ptr(), Cc, wp.data_ptr(), Cp, n, Cp,
-                     hd, hdp, 0, 1)
         if isinstance(gamma, torch.Tensor):
             sc, sh = self._fold(nm + ".proj.ls", n, bias=lin.bias, ls=gamma)
             cs_, sh_ = sc.data_ptr(), sh.data_ptr()
         else:
             cs_, sh_ = None, lin.bias.data_ptr()
         self._gemm(a=ao.data_ptr(), a_rows=rows, lda=Cp, b=wp.data_ptr(), ldb=ldp, m=rows, n=n, kc=Cp,
-                   col_scale=cs_, col_shift=sh_, resid=stream_buf, ld_resid=n, out_f32=stream_buf, ld_o32=n)
-        self.op_flops[len(self.ops) - 1] = 2.0 * rows * n * Cc
+                   col_scale=cs_, col_shift=sh_, resid=stream_buf, ld_resid=n, out_f32=stream_buf, ld_o32=n,
+                   flops=2.0 * rows * n * Cc)
 
-    def _emit_bias(self, nm: str, rpb, S: int) -> torch.Tensor:
+    def _pack_attention(self, nm: str, attn, hdp: int) -> tuple:
+        """fp16 operands of an attention's qkv and proj Linears with every head zero-padded from head_dim to hdp (the
+        rows of qkv, the columns of proj), and qkv's bias padded alike: (wq, ldq, qkv bias pointer, wp, ldp)"""
+        Cc, hd = attn.qkv.in_features, attn.head_dim
+        if hdp == hd:
+            wq, ldq = self._pack_linear(nm + ".qkv", attn.qkv)
+            wp, ldp = self._pack_linear(nm + ".proj", attn.proj)
+            return wq, ldq, P(attn.qkv.bias), wp, ldp
+        Cp = attn.num_heads * hdp
+        ldq = _ru(Cc, 8)
+        wq = self.bufs.new(nm + ".qkv.w16", (3 * Cp, ldq), torch.float16)
+        self._op(self.prep_ops, "fvit_cast_headpad_f16", attn.qkv.weight.data_ptr(), Cc, wq.data_ptr(), ldq, 3 * Cp, Cc,
+                 hd, hdp, 1, 0)
+        qb_ptr = None
+        if attn.qkv.bias is not None:
+            qbp = self.bufs.new(nm + ".qkv.bias_pad", (3 * Cp,), torch.float32)
+            self._op(self.prep_ops, "fvit_vec_headpad_f32", attn.qkv.bias.data_ptr(), qbp.data_ptr(), 3 * Cp, hd, hdp)
+            qb_ptr = qbp.data_ptr()
+        n = attn.proj.weight.shape[0]
+        wp = self.bufs.new(nm + ".proj.w16", (n, Cp), torch.float16)
+        self._op(self.prep_ops, "fvit_cast_headpad_f16", attn.proj.weight.data_ptr(), Cc, wp.data_ptr(), Cp, n, Cp, hd,
+                 hdp, 0, 1)
+        return wq, ldq, qb_ptr, wp, Cp
+
+    def _emit_bias(self, nm: str, rpb, S: int, hidden=None) -> dict:
         """PosEmbMLPSwinv2D (fv.py:276-307): table MLP + gather + 16*sigmoid, written straight into the
-        module's `relative_bias` buffer (which the reference also overwrites every forward)."""
-        P = rpb.relative_coords_table.shape[1] * rpb.relative_coords_table.shape[2]
-        table = self.bufs.new(nm + ".table", (P, rpb.num_heads), torch.float32)
+        module's `relative_bias` buffer (which the reference also overwrites every forward). With a `hidden` buffer
+        (training) the MLP also saves its hidden activations for the backward, and so runs in deploy mode too."""
+        npts = rpb.relative_coords_table.shape[1] * rpb.relative_coords_table.shape[2]
+        table = self.bufs.new(nm + ".table", (npts, rpb.num_heads), torch.float32)
         if tuple(rpb.relative_bias.shape) != (1, rpb.num_heads, S, S):
             rpb.relative_bias = torch.zeros(1, rpb.num_heads, S, S, device=self.device)
         tgt = self.prep_ops  # batch independent: recomputed only when the weights change
         n0 = len(tgt)
-        self._op(tgt, "fvit_cpb_mlp_fwd", rpb.relative_coords_table.data_ptr(), P, rpb.cpb_mlp[0].weight.data_ptr(),
+        self._op(tgt, "fvit_cpb_mlp_fwd", rpb.relative_coords_table.data_ptr(), npts, rpb.cpb_mlp[0].weight.data_ptr(),
                  rpb.cpb_mlp[0].bias.data_ptr(), rpb.cpb_mlp[2].weight.data_ptr(), rpb.num_heads,
-                 table.data_ptr(), None)
+                 table.data_ptr(), P(hidden))
         self._op(tgt, "fvit_attn_bias_fwd", table.data_ptr(), rpb.relative_position_index.data_ptr(),
                  rpb.num_heads, S, rpb.window ** 2, rpb.relative_bias.data_ptr())
-        self._deploy_guard(tgt, n0, rpb)
-        return rpb.relative_bias
+        if hidden is None:
+            self._deploy_guard(tgt, n0, rpb)
+        return dict(mod=rpb, out=rpb.relative_bias, hidden=hidden, npts=npts, S=S)
 
-    def _emit_pos_embed(self, nm: str, tpe, n_side: int, Cc: int) -> torch.Tensor:
+    def _emit_pos_embed(self, nm: str, tpe, n_side: int, Cc: int, hidden=None) -> dict:
         """PosEmbMLPSwinv1D rank 2 (fv.py:355-365): MLP over the centred n x n grid, written into the
-        module's `relative_bias` buffer; the add itself is fused into the following LayerNorm."""
+        module's `relative_bias` buffer; the add itself is fused into the following LayerNorm. `hidden`: as
+        _emit_bias."""
         r = torch.arange(n_side, dtype=torch.float32)
         grid = torch.stack(torch.meshgrid(r, r, indexing="ij"))          # 2, n, n
         grid = (grid - n_side // 2) / (n_side // 2)
-        coords = self.bufs.new(nm + ".coords", (n_side * n_side, 2), torch.float32)
+        npts = n_side * n_side
+        coords = self.bufs.new(nm + ".coords", (npts, 2), torch.float32)
         coords.copy_(grid.flatten(1).t())
-        if tuple(tpe.relative_bias.shape) != (1, n_side * n_side, Cc):
-            tpe.relative_bias = torch.zeros(1, n_side * n_side, Cc, device=self.device)
+        if tuple(tpe.relative_bias.shape) != (1, npts, Cc):
+            tpe.relative_bias = torch.zeros(1, npts, Cc, device=self.device)
         n0 = len(self.prep_ops)
-        self._op(self.prep_ops, "fvit_cpb_mlp_fwd", coords.data_ptr(), n_side * n_side,
-                 tpe.cpb_mlp[0].weight.data_ptr(), tpe.cpb_mlp[0].bias.data_ptr(),
-                 tpe.cpb_mlp[2].weight.data_ptr(), Cc, tpe.relative_bias.data_ptr(), None)
-        self._deploy_guard(self.prep_ops, n0, tpe)
-        return tpe.relative_bias
+        self._op(self.prep_ops, "fvit_cpb_mlp_fwd", coords.data_ptr(), npts, tpe.cpb_mlp[0].weight.data_ptr(),
+                 tpe.cpb_mlp[0].bias.data_ptr(), tpe.cpb_mlp[2].weight.data_ptr(), Cc, tpe.relative_bias.data_ptr(),
+                 P(hidden))
+        if hidden is None:
+            self._deploy_guard(self.prep_ops, n0, tpe)
+        return dict(mod=tpe, out=tpe.relative_bias, hidden=hidden, coords=coords, npts=npts, D=Cc)
 
     def _emit_branch_out(self, nm: str, lin: nn.Linear, gamma, a, lda, rows, stream_buf, act=L.ACT_NONE,
                          out16=None, ld16=0) -> None:
@@ -628,19 +671,19 @@ class Plan:
                      tl["ct_rows"].data_ptr(), xs_ptr, Cc)
         for j, blk in enumerate(level.blocks):
             nm = f"l{i}.b{j}"
-            pe = self._emit_pos_embed(nm + ".pe", blk.pos_embed, ws, Cc)
+            pe = self._emit_pos_embed(nm + ".pe", blk.pos_embed, ws, Cc)["out"]
             if has_ct:
                 ctr_ptr = xs_ptr + tl["ctr0"] * Cc * 4
                 rows_c = B * n_ct
                 hat_pe = None
                 if hasattr(blk, "hat_pos_embed"):
-                    hat_pe = self._emit_pos_embed(nm + ".hat_pe", blk.hat_pos_embed, int(n_ct ** 0.5), Cc)
+                    hat_pe = self._emit_pos_embed(nm + ".hat_pe", blk.hat_pos_embed, int(n_ct ** 0.5), Cc)["out"]
                 # ct = dewindow(ct) + hat_pos_embed ; LN -> fp16                 (fv.py:673-679)
                 self._op(self.ops, "fvit_ln_fwd", xs_ptr, Cc, tl["ct_gather"].data_ptr(), rows_c, Cc,
                          hat_pe.data_ptr() if hat_pe is not None else None, n_ct, 0, ctr_ptr, Cc,
                          blk.hat_norm1.weight.data_ptr(), blk.hat_norm1.bias.data_ptr(), float(blk.hat_norm1.eps),
                          tl["ctn16"].data_ptr(), Cc, None, None, None, None, 0)
-                hb = self._emit_bias(nm + ".hat_bias", blk.hat_attn.pos_emb_funct, n_ct)
+                hb = self._emit_bias(nm + ".hat_bias", blk.hat_attn.pos_emb_funct, n_ct)["out"]
                 self._emit_attention(nm + ".hat_attn", blk.hat_attn, blk.gamma1, rows_c, B, n_ct, tl["ctn16"], Cc,
                                      tl["ctqkv16"], tl["ctao16"], hb, ctr_ptr)
                 self._op(self.ops, "fvit_ln_fwd", ctr_ptr, Cc, None, rows_c, Cc, None, 1, 0, None, 0,
@@ -654,7 +697,7 @@ class Plan:
             self._op(self.ops, "fvit_ln_fwd", xs_ptr, Cc, tl["norm1_gather"].data_ptr() if has_ct else None, rows,
                      Cc, pe.data_ptr(), S, ncw, xs_ptr, Cc, blk.norm1.weight.data_ptr(), blk.norm1.bias.data_ptr(),
                      float(blk.norm1.eps), tl["xn16"].data_ptr(), Cc, None, None, None, None, 0)
-            ab = self._emit_bias(nm + ".bias", blk.attn.pos_emb_funct, S)
+            ab = self._emit_bias(nm + ".bias", blk.attn.pos_emb_funct, S)["out"]
             self._emit_attention(nm + ".attn", blk.attn, blk.gamma3, rows, nW, S, tl["xn16"], Cc, tl["qkv16"],
                                  tl["ao16"], ab, xs_ptr)
             self._op(self.ops, "fvit_ln_fwd", xs_ptr, Cc, None, rows, Cc, None, 1, 0, None, 0,

@@ -14,8 +14,6 @@ so no fp16 product underflows. Parameter gradients are fp32 and exact in scale.
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import os
 
 import torch
@@ -23,7 +21,7 @@ import torch
 from . import lib as L
 from .engine import Plan, _ru
 from .engine_train_conv import ConvPartEmitters
-from .engine_train_levels import TokenLevelEmitters
+from .engine_train_levels import _ONE, TokenLevelEmitters
 
 
 def levels_path(model, outs) -> set[int]:
@@ -198,7 +196,7 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
     def _branch(self, gamma) -> dict:
         """device-scalar pointers of a residual branch: dgrad alpha (1/s_b) and wgrad alpha (1/(S s_b))"""
         if not isinstance(gamma, torch.Tensor):
-            return dict(gamma=None, s=None, inv_s=("scal", 2), w_alpha=("scal", 1))
+            return _ONE
         slot = self._nscal
         self._nscal += 3
         self._branch_slots.append((slot, gamma))
@@ -224,10 +222,8 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
                 if isinstance(args, tuple):
                     lst[i] = (fn, tuple(res(a) for a in args), name)
         for g in self._gemm_keep:
-            for f in ("alpha_ptr", "out_f32", "col_sum", "col_sumsq", "out_colsum", "out_colsum_alpha"):
-                v = getattr(g, "_sym_" + f, None)
-                if v is not None:
-                    setattr(g, f, res(v))
+            for f, v in g._sym.items():
+                setattr(g, f, res(v))
         # per-backward prologue: zero accumulators, pick the gradient scale, per-branch wgrad alphas
         pro: list[tuple] = [("zero", self.gflat, "memset"), ("zero", self.scr, "memset")]
         for lv in self.lv:
@@ -241,42 +237,6 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         for slot, _ in self._branch_slots:
             self._branch_alpha_ops.append((self.lib.fvit_vec_mul, (sp + 4, 0, sp + 4 * (slot + 1), 0, sp + 4 * (slot + 2), 1),
                                            "fvit_vec_mul"))
-
-    # symbolic-pointer aware GEMM emitter for the backward list
-    def _bgemm(self, *, a, a_rows, lda, b, b_rows, ldb, m, n, kc, a_mn=False, b_mn=False, taps=None, a_planes=1,
-               a_plane_stride=0, b_row_off=0, b_taps=None, split_k=1, alpha_ptr=None, act=L.ACT_NONE, aux=None, ld_aux=0,
-               out_f32=None, ld_o32=0, out_f16=None, ld_o16=0, row_map=None, resid=None, ld_resid=0, target=None,
-               flops=None, out_colsum=None, out_colsum_alpha=None, aux_scale=None, aux_shift=None) -> None:
-        g = L.GemmArgs()
-        g.a, g.a_rows, g.lda, g.a_plane_stride, g.a_planes, g.a_mn_major = a, a_rows, lda, a_plane_stride, a_planes, int(a_mn)
-        g.b, g.b_rows, g.ldb, g.b_mn_major = b, b_rows, ldb, int(b_mn)
-        g.m, g.n, g.kc = m, n, kc
-        taps = taps or [(0, 0)]
-        g.ntaps = len(taps)
-        for i, (s, p) in enumerate(taps):
-            g.tap_shift[i], g.tap_plane[i] = s, p
-        g.b_row_off = b_row_off
-        if b_taps is not None:   # conv weight gradient: taps folded into N (include/fvit.h: b_ntaps)
-            assert len(taps) == 1 and a_mn and b_mn
-            g.b_ntaps = len(b_taps)
-            for i, sft in enumerate(b_taps):
-                g.tap_shift[i] = sft
-        g.split_k, g.alpha, g.act = split_k, 1.0, act
-        g.aux, g.ld_aux, g.row_map = aux, ld_aux, row_map
-        g.aux_scale, g.aux_shift = aux_scale, aux_shift
-        g.resid, g.ld_resid = resid, ld_resid
-        g.out_f16, g.ld_out_f16, g.ld_out_f32 = out_f16, ld_o16, ld_o32
-        for f, v in (("alpha_ptr", alpha_ptr), ("out_f32", out_f32), ("out_colsum", out_colsum),
-                     ("out_colsum_alpha", out_colsum_alpha)):
-            if isinstance(v, tuple):
-                setattr(g, "_sym_" + f, v)
-            elif v is not None:
-                setattr(g, f, v)
-        self._gemm_keep.append(g)
-        lst = self.bwd_ops if target is None else target
-        lst.append((self.lib.fvit_gemm, (C.byref(g),), "fvit_gemm"))
-        if lst is self.bwd_ops:
-            self.bwd_flops[len(lst) - 1] = flops if flops is not None else 2.0 * m * n * kc * len(taps)
 
     # ------------------------------------------------------------------------------ weight gradients as a side branch
     # A weight-gradient GEMM reads an activation gradient (a per-level buffer every block reuses) and a saved
@@ -332,9 +292,9 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
             gW = self.G(lin.weight) if gW is None else gW
             gW_ld = k_in if gW_ld is None else gW_ld
             n0 = len(self.bwd_ops)
-            self._bgemm(a=dz16, a_rows=rows, lda=lddz, a_mn=True, b=x16, b_rows=rows, ldb=ldx, b_mn=True, m=n_out, n=k_in,
-                        kc=rows, split_k=self._split_k(n_out, k_in, rows), alpha_ptr=br["w_alpha"], out_f32=gW,
-                        ld_o32=gW_ld, row_map=gW_row_map, flops=2.0 * rows * n_out * fk)
+            self._gemm(a=dz16, a_rows=rows, lda=lddz, a_mn=True, b=x16, b_rows=rows, ldb=ldx, b_mn=True, m=n_out, n=k_in,
+                       kc=rows, split_k=self._split_k(n_out, k_in, rows), alpha_ptr=br["w_alpha"], out_f32=gW,
+                       ld_o32=gW_ld, row_map=gW_row_map, target=self.bwd_ops, flops=2.0 * rows * n_out * fk)
             if (lin.bias is not None or bias_to is not None) and not bias_done:
                 dst = bias_to if bias_to is not None else self.G(lin.bias)
                 self._op(self.bwd_ops, "fvit_colsum", dz16, 1, lddz, None, None, 0, rows, n_out, None, br["w_alpha"], dst,
@@ -342,11 +302,21 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
             self._side_from(n0, dz16)   # (weight gradient + bias column sums: both only read dz16)
         if want_dgrad:
             self._before_write(dx16)
-            self._bgemm(a=dz16, a_rows=rows, lda=lddz, b=w16, b_rows=n_out, ldb=ldw, b_mn=True, m=rows, n=k_in, kc=n_out,
-                        alpha_ptr=dx_alpha if dx_alpha is not None else br["inv_s"], act=dx_act, aux=dx_aux,
-                        ld_aux=ld_aux, out_f16=dx16, ld_o16=lddx, flops=2.0 * rows * n_out * fk,
-                        out_colsum=dx_colsum[0] if dx_colsum else None,
-                        out_colsum_alpha=dx_colsum[1] if dx_colsum else None)
+            self._gemm(a=dz16, a_rows=rows, lda=lddz, b=w16, b_rows=n_out, ldb=ldw, b_mn=True, m=rows, n=k_in, kc=n_out,
+                       alpha_ptr=dx_alpha if dx_alpha is not None else br["inv_s"], act=dx_act, aux=dx_aux, ld_aux=ld_aux,
+                       out_f16=dx16, ld_o16=lddx, out_colsum=dx_colsum[0] if dx_colsum else None,
+                       out_colsum_alpha=dx_colsum[1] if dx_colsum else None, target=self.bwd_ops,
+                       flops=2.0 * rows * n_out * fk)
+
+    def _ln_bwd(self, ln, dy, lddy: int, dy_map, xh, rs, rows: int, C: int, g, g_map, use_g: int, clear_moved: int,
+                data_only: bool) -> None:
+        """LayerNorm backward into the gradient rows g (through g_map; fvit_ln_bwd in include/fvit.h): with the weight /
+        bias gradients (fvit_ln_bwd), or the input gradient alone in a data-only stage (fvit_ln_dgrad)"""
+        args = (dy, lddy, dy_map, xh, C, rs, ln.weight.data_ptr(), rows, C, g, C, g_map, use_g, clear_moved)
+        if data_only:
+            self._op(self.bwd_ops, "fvit_ln_dgrad", *args)
+        else:
+            self._op(self.bwd_ops, "fvit_ln_bwd", *args, ("scal", 1), self.G(ln.weight), self.G(ln.bias))
 
     # ------------------------------------------------------------------------------ plan construction
     def _build(self) -> None:

@@ -14,11 +14,7 @@ import torch
 import torch.nn as nn
 
 from . import lib as L
-from .engine import _ru
-
-
-def P(t):
-    return None if t is None else t.data_ptr()
+from .engine import P, _ru
 
 
 def _bn_train(self, name: str, bn: nn.BatchNorm2d, count: int, ls=None) -> dict:
@@ -80,10 +76,7 @@ def _emit_conv_part_train(self) -> dict:
     ld_in = _ru(in_dim, 8)
     pl_rows = B * (H0 + 1) * (W0 + 1)
     npix1 = B * H1 * W1
-    bi, yi, xi = torch.meshgrid(torch.arange(B), torch.arange(H1), torch.arange(W1), indexing="ij")
-    plane = (yi & 1) * 2 + (xi & 1)
-    stem_map = nb.i32("stem.map", (plane * pl_rows + bi * (H0 + 1) * (W0 + 1) + ((yi >> 1) + 1) * (W0 + 1)
-                                   + (xi >> 1) + 1).reshape(-1))
+    stem_map = self._parity_plane_map("stem.map", H1, W1)
     pe = m.patch_embed.conv_down
     st = dict(H1=H1, W1=W1, H0=H0, W0=W0, pl_rows=pl_rows, ld_in=ld_in, npix1=npix1, stem_map=stem_map)
     # conv1: im2col + GEMM -> raw1 (plane layout) + statistics
@@ -99,9 +92,7 @@ def _emit_conv_part_train(self) -> dict:
     bn1 = _bn_train(self, "stem.bn1", pe[1], npix1)
     self._gemm(a=col16.data_ptr(), a_rows=npix1, lda=sld, b=w1.data_ptr(), ldb=sld, m=npix1, n=in_dim,
                kc=sld, col_shift=_bn_col_shift(self, bn1, None), row_map=stem_map.data_ptr(), out_f16=raw1.data_ptr(),
-               ld_o16=ld_in, col_sum=bn1["col_sum"],
-               col_sumsq=bn1["col_sumsq"])
-    self.op_flops[len(self.ops) - 1] = 2.0 * npix1 * in_dim * k1
+               ld_o16=ld_in, col_sum=bn1["col_sum"], col_sumsq=bn1["col_sumsq"], flops=2.0 * npix1 * in_dim * k1)
     _bn_finalize(self, bn1)
     self._op(self.ops, "fvit_affine_rows", raw1.data_ptr(), ld_in, stem_map.data_ptr(), npix1, in_dim, bn1["sc"].data_ptr(),
              bn1["sh"].data_ptr(), L.ACT_RELU, None, 0, None, 0, planes.data_ptr(), ld_in, None)
@@ -143,20 +134,14 @@ def _emit_conv_part_train(self) -> dict:
 
 
 def _conv_level_train_buffers(self, i: int, Cc: int, Hc: int, Wc: int, depth: int) -> dict:
-    B, nb = self.B, self.bufs
-    rows = B * (Hc + 2) * (Wc + 2)
-    ld = _ru(Cc, 8)
-    bi, yi, xi = torch.meshgrid(torch.arange(B), torch.arange(Hc + 2), torch.arange(Wc + 2), indexing="ij")
-    inside = (yi >= 1) & (yi <= Hc) & (xi >= 1) & (xi <= Wc)
-    ident = torch.arange(rows).view(B, Hc + 2, Wc + 2)
-    d = dict(C=Cc, H=Hc, W=Wc, ld=ld, rows=rows, npix=B * Hc * Wc, kind="conv",
-             interior=nb.i32(f"l{i}.interior", torch.where(inside, ident, torch.full_like(ident, -1)).reshape(-1)),
-             pix=nb.i32(f"l{i}.pix", ident[:, 1:-1, 1:-1].reshape(-1)),
-             x32=nb.new(f"l{i}.x32", (rows, Cc), torch.float32),
-             x16s=[nb.new(f"l{i}.x16.{j}", (rows, ld), torch.float16) for j in range(depth + 1)],
-             dzA=nb.new(f"l{i}.dzA", (rows, ld), torch.float16), dzB=nb.new(f"l{i}.dzB", (rows, ld), torch.float16),
-             dyA=nb.new(f"l{i}.dyA", (rows, ld), torch.float16),
-             g=nb.new(f"l{i}.g", (rows + 1, Cc), torch.float32), zero_row=rows)
+    """Plan._conv_level_buffers with the backward's fp16 gradient operands (dzA, dzB, dyA), one fp16 operand copy of
+    the map per block boundary (x16s: every block's saved input, then the level output) and the fp32 gradient g with
+    one guaranteed-zero row at the end"""
+    nb = self.bufs
+    d = self._conv_level_buffers(i, Cc, Hc, Wc, f16=("dzA", "dzB", "dyA"))
+    rows = d["rows"]
+    d.update(kind="conv", zero_row=rows, g=nb.new(f"l{i}.g", (rows + 1, Cc), torch.float32),
+             x16s=[nb.new(f"l{i}.x16.{j}", (rows, d["ld"]), torch.float16) for j in range(depth + 1)])
     d["x16"] = d["x16s"][-1]  # level output operand (input of the downsample LayerNorm is x32)
     return d
 
@@ -214,9 +199,7 @@ def _emit_downsample_train(self, i: int, src: dict, dst: dict) -> None:
     pl_rows = B * (Ho + 1) * (Wo + 1)
     npix = B * Hs * Ws
     planes = nb.new(f"ds{i}.planes", (4 * pl_rows, ld), torch.float16)
-    bi, yi, xi = torch.meshgrid(torch.arange(B), torch.arange(Hs), torch.arange(Ws), indexing="ij")
-    omap = nb.i32(f"ds{i}.omap", (((yi & 1) * 2 + (xi & 1)) * pl_rows + bi * (Ho + 1) * (Wo + 1)
-                                  + ((yi >> 1) + 1) * (Wo + 1) + (xi >> 1) + 1).reshape(-1))
+    omap = self._parity_plane_map(f"ds{i}.omap", Hs, Ws)
     src_rows = src["pix"] if src["kind"] == "conv" else src["crop_map"]
     src_x = src["x32"] if src["kind"] == "conv" else src["xs"]
     xh = nb.new(f"ds{i}.xhat", (npix, Cs), torch.float16)
@@ -226,40 +209,38 @@ def _emit_downsample_train(self, i: int, src: dict, dst: dict) -> None:
              ds_mod.norm.weight.data_ptr(), ds_mod.norm.bias.data_ptr(), float(ds_mod.norm.eps), planes.data_ptr(), ld,
              omap.data_ptr(), mu.data_ptr(), rs.data_ptr(), xh.data_ptr(), Cs)
     w16, ldw = self._pack_conv(f"ds{i}.conv", ds_mod.reduction[0])
-    taps = self._s2_taps(Wo)
-    if dst.get("kind", "tok") == "conv" or "x16s" in dst:
-        rmap_t = torch.full((B, Ho + 1, Wo + 1), -1, dtype=torch.int64)
-        bb, aa, cc = torch.meshgrid(torch.arange(B), torch.arange(Ho), torch.arange(Wo), indexing="ij")
-        rmap_t[:, 1:, 1:] = bb * (Ho + 2) * (Wo + 2) + (aa + 1) * (Wo + 2) + cc + 1
-        rmap = nb.i32(f"ds{i}.rmap", rmap_t.reshape(-1))
-        self._gemm(a=planes.data_ptr(), a_rows=pl_rows, lda=ld, a_planes=4, a_plane_stride=pl_rows * ld, b=w16.data_ptr(),
-                   ldb=ldw, m=pl_rows, n=2 * Cs, kc=Cs, taps=taps, m_alg=B * Ho * Wo, row_map=rmap.data_ptr(),
-                   out_f32=dst["x32"].data_ptr(), ld_o32=dst["C"], out_f16=dst["x16s"][0].data_ptr(), ld_o16=dst["ld"])
-    else:
-        pm = dst["pix_map_host"]
-        rmap_t = torch.full((B, Ho + 1, Wo + 1), -1, dtype=torch.int64)
-        rmap_t[:, 1:, 1:] = pm[:, :Ho, :Wo]
-        rmap = nb.i32(f"ds{i}.rmap", rmap_t.reshape(-1))
-        dst["x0_16"] = nb.new(f"ds{i}.x0_16", (dst["xs"].shape[0], 2 * Cs), torch.float16)
-        self._gemm(a=planes.data_ptr(), a_rows=pl_rows, lda=ld, a_planes=4, a_plane_stride=pl_rows * ld, b=w16.data_ptr(),
-                   ldb=ldw, m=pl_rows, n=2 * Cs, kc=Cs, taps=taps, m_alg=B * Ho * Wo, row_map=rmap.data_ptr(),
-                   out_f32=dst["xs"].data_ptr(), ld_o32=dst["C"], out_f16=dst["x0_16"].data_ptr(), ld_o16=2 * Cs)
-    # backward-side maps / packed operands
-    zero_row = dst["zero_row"]
-    rmap_g = nb.i32(f"ds{i}.rmap_g", torch.where(rmap_t >= 0, rmap_t, torch.full_like(rmap_t, zero_row)).reshape(-1))
-    plane_taps = {p: [t for t in range(9) if taps[t][1] == p] for p in range(4)}
-    co_pad = _ru(2 * Cs, 64)
-    wT = {}
-    for p, tl_ in plane_taps.items():
-        buf = nb.new(f"ds{i}.wT.{p}", (Cs, len(tl_) * co_pad), torch.float16)
-        t9 = tl_ + [0] * (9 - len(tl_))
-        self._op(self.prep_ops, "fvit_pack_conv3x3_taps_f16", ds_mod.reduction[0].weight.data_ptr(), buf.data_ptr(), 2 * Cs,
-                 Cs, co_pad, 1, len(tl_), *t9)
-        wT[p] = buf
-    dst["ds"] = dict(i=i, mod=ds_mod, Cs=Cs, Hs=Hs, Ws=Ws, Ho=Ho, Wo=Wo, ld=ld, pl_rows=pl_rows, npix=npix, planes=planes,
-                     omap=omap, src_rows=src_rows, xh=xh, rs=rs, taps=taps, rmap_g=rmap_g, plane_taps=plane_taps, wT=wT,
-                     co_pad=co_pad, dY=nb.new(f"ds{i}.dY16", (pl_rows, 2 * Cs), torch.float16),
+    if "x16s" in dst:   # a conv level: its residual stream and first block's input operand
+        out32, out16, ld16 = dst["x32"], dst["x16s"][0], dst["ld"]
+    else:               # a token level: its residual stream and x0, the tokenizer's weight-gradient operand
+        out32, ld16 = dst["xs"], 2 * Cs
+        out16 = dst["x0_16"] = nb.new(f"ds{i}.x0_16", (dst["xs"].shape[0], 2 * Cs), torch.float16)
+    rmap = self._downsample_row_map(i, dst, Ho, Wo)
+    self._gemm(a=planes.data_ptr(), a_rows=pl_rows, lda=ld, a_planes=4, a_plane_stride=pl_rows * ld, b=w16.data_ptr(),
+               ldb=ldw, m=pl_rows, n=2 * Cs, kc=Cs, taps=self._s2_taps(Wo), m_alg=B * Ho * Wo, row_map=rmap.data_ptr(),
+               out_f32=out32.data_ptr(), ld_o32=dst["C"], out_f16=out16.data_ptr(), ld_o16=ld16)
+    # backward-side maps / packed operands: the border rows of the plane-space output read the gradient's zero row
+    rmap_g = nb.i32(f"ds{i}.rmap_g", torch.where(rmap >= 0, rmap, torch.full_like(rmap, dst["zero_row"])))
+    wT = _s2_dgrad_operands(self, f"ds{i}", ds_mod.reduction[0], Wo)
+    dst["ds"] = dict(i=i, mod=ds_mod, Cs=Cs, Ho=Ho, Wo=Wo, ld=ld, pl_rows=pl_rows, npix=npix, planes=planes, omap=omap,
+                     src_rows=src_rows, xh=xh, rs=rs, rmap_g=rmap_g, wT=wT,
+                     dY=nb.new(f"ds{i}.dY16", (pl_rows, 2 * Cs), torch.float16),
                      dplanes=nb.new(f"ds{i}.dplanes16", (4 * pl_rows, ld), torch.float16))
+
+
+def _s2_dgrad_operands(self, name: str, conv: nn.Conv2d, Wo: int) -> list:
+    """data-gradient operands of a 3x3 stride-2 convolution over parity planes (Plan._s2_taps): for each input plane,
+    the flipped / transposed weights of the taps that read it, [(packed fp16 buffer, tap indices)] * 4"""
+    cout, cin = conv.weight.shape[:2]
+    taps = self._s2_taps(Wo)
+    co_pad = _ru(cout, 64)
+    wT = []
+    for p in range(4):
+        tl_ = [t for t in range(9) if taps[t][1] == p]
+        buf = self.bufs.new(f"{name}.wT.{p}", (cin, len(tl_) * co_pad), torch.float16)
+        self._op(self.prep_ops, "fvit_pack_conv3x3_taps_f16", conv.weight.data_ptr(), buf.data_ptr(), cout, cin, co_pad, 1,
+                 len(tl_), *(tl_ + [0] * (9 - len(tl_))))
+        wT.append((buf, tl_))
+    return wT
 
 
 # ====================================================================================== backward
@@ -293,9 +274,9 @@ def _conv_wgrad(self, *, dz, lddz, x, ldx, x_rows, rows, cout, cin, shifts, conv
     scr = ("scr", self._scratch(name + ".dWtaps", nt * cout * cin))
     sk = self._split_k(cout, cin, rows, nt)
     n0 = len(self.bwd_ops)
-    self._bgemm(a=dz, a_rows=rows, lda=lddz, a_mn=True, b=x, b_rows=x_rows, ldb=ldx, b_mn=True, b_taps=list(shifts), m=cout,
-                n=cin, kc=rows, split_k=sk, alpha_ptr=("scal", 1), out_f32=scr, ld_o32=nt * cin,
-                flops=2.0 * rows * cout * cin * nt)
+    self._gemm(a=dz, a_rows=rows, lda=lddz, a_mn=True, b=x, b_rows=x_rows, ldb=ldx, b_mn=True, b_taps=list(shifts), m=cout,
+               n=cin, kc=rows, split_k=sk, alpha_ptr=("scal", 1), out_f32=scr, ld_o32=nt * cin, target=self.bwd_ops,
+               flops=2.0 * rows * cout * cin * nt)
     self._op(self.bwd_ops, "fvit_unpack_conv_grad", scr, nt * cin, self.G(conv_weight), cout, cin)
     if bias is not None:
         self._op(self.bwd_ops, "fvit_colsum", dz, 1, lddz, bias_rows, None, 0, bias_nrows, cout, None, ("scal", 1),
@@ -303,34 +284,35 @@ def _conv_wgrad(self, *, dz, lddz, x, ldx, x_rows, rows, cout, cin, shifts, conv
     self._side_from(n0, dz)   # (its own zeroed scratch slice in, a parameter gradient out: a leaf pair)
 
 
-def _emit_downsample_bwd(self, ds: dict, src: dict, dst: dict) -> None:
-    """Downsample backward; data-only (with the level in front of it, stage 1 + i): no weight gradient, LayerNorm dx only"""
-    ops = self.bwd_ops
-    data_only = self.data_only[1 + ds["i"]]
-    Cs, ld, pl_rows, npix = ds["Cs"], ds["ld"], ds["pl_rows"], ds["npix"]
-    mod = ds["mod"]
-    # gradient of the conv output in plane space (border rows read the buffer's zero row)
-    self._op(ops, "fvit_cast_scale_f16", dst["g"].data_ptr(), 2 * Cs, ds["rmap_g"].data_ptr(), pl_rows, 2 * Cs, None, None,
-             ds["dY"].data_ptr(), 2 * Cs, None)
-    shifts = [p * pl_rows + s for (s, p) in ds["taps"]]
+def _s2_conv_bwd(self, *, conv: nn.Conv2d, wT: list, dY, lddy: int, planes, dplanes, ld: int, pl_rows: int, Wo: int,
+                 npix: int, name: str, data_only: bool) -> None:
+    """Backward of a 3x3 stride-2 convolution over the parity planes `planes` (ld wide) from the gradient dY of its
+    pl_rows plane-space output rows (npix of them real pixels): the weight gradient unless data_only, then the gradient
+    of the planes into dplanes, one GEMM per plane over the taps that read it (wT: _s2_dgrad_operands)"""
+    cout, cin = conv.weight.shape[:2]
+    taps = self._s2_taps(Wo)
     if not data_only:
-        _conv_wgrad(self, dz=ds["dY"].data_ptr(), lddz=2 * Cs, x=ds["planes"].data_ptr(), ldx=ld, x_rows=4 * pl_rows,
-                    rows=pl_rows, cout=2 * Cs, cin=Cs, shifts=shifts, conv_weight=mod.reduction[0].weight,
-                    name=f"ds{ds['i']}")
-    for p, tl_ in ds["plane_taps"].items():
-        self._bgemm(a=ds["dY"].data_ptr(), a_rows=pl_rows, lda=2 * Cs, b=ds["wT"][p].data_ptr(), b_rows=Cs,
-                    ldb=len(tl_) * ds["co_pad"], m=pl_rows, n=Cs, kc=2 * Cs, taps=[(-ds["taps"][t][0], 0) for t in tl_],
-                    out_f16=ds["dplanes"].data_ptr() + 2 * p * pl_rows * ld, ld_o16=ld,
-                    flops=2.0 * self.B * ds["Ho"] * ds["Wo"] * Cs * 2 * Cs * len(tl_))
-    # LayerNorm2d backward: writes the source level's output gradient
-    if data_only:
-        self._op(ops, "fvit_ln_dgrad", ds["dplanes"].data_ptr(), ld, ds["omap"].data_ptr(), ds["xh"].data_ptr(), Cs,
-                 ds["rs"].data_ptr(), mod.norm.weight.data_ptr(), npix, Cs, src["g"].data_ptr(), Cs,
-                 ds["src_rows"].data_ptr(), 0, 0)
-        return
-    self._op(ops, "fvit_ln_bwd", ds["dplanes"].data_ptr(), ld, ds["omap"].data_ptr(), ds["xh"].data_ptr(), Cs,
-             ds["rs"].data_ptr(), mod.norm.weight.data_ptr(), npix, Cs, src["g"].data_ptr(), Cs, ds["src_rows"].data_ptr(), 0, 0,
-             ("scal", 1), self.G(mod.norm.weight), self.G(mod.norm.bias))
+        _conv_wgrad(self, dz=dY, lddz=lddy, x=planes, ldx=ld, x_rows=4 * pl_rows, rows=pl_rows, cout=cout, cin=cin,
+                    shifts=[p * pl_rows + s for (s, p) in taps], conv_weight=conv.weight, name=name)
+    for p, (buf, tl_) in enumerate(wT):
+        self._gemm(a=dY, a_rows=pl_rows, lda=lddy, b=buf.data_ptr(), b_rows=cin, ldb=buf.shape[1], m=pl_rows, n=cin,
+                   kc=cout, taps=[(-taps[t][0], 0) for t in tl_], out_f16=dplanes + 2 * p * pl_rows * ld, ld_o16=ld,
+                   target=self.bwd_ops, flops=2.0 * npix * cin * cout * len(tl_))
+
+
+def _emit_downsample_bwd(self, ds: dict, src: dict, dst: dict) -> None:
+    """Downsample backward into the source level's output gradient; data-only (with the level in front of it, stage
+    1 + i): no weight gradient, LayerNorm dx only"""
+    data_only = self.data_only[1 + ds["i"]]
+    Cs, ld, pl_rows = ds["Cs"], ds["ld"], ds["pl_rows"]
+    # gradient of the conv output in plane space (border rows read the buffer's zero row)
+    self._op(self.bwd_ops, "fvit_cast_scale_f16", dst["g"].data_ptr(), 2 * Cs, ds["rmap_g"].data_ptr(), pl_rows, 2 * Cs,
+             None, None, ds["dY"].data_ptr(), 2 * Cs, None)
+    _s2_conv_bwd(self, conv=ds["mod"].reduction[0], wT=ds["wT"], dY=ds["dY"].data_ptr(), lddy=2 * Cs,
+                 planes=ds["planes"].data_ptr(), dplanes=ds["dplanes"].data_ptr(), ld=ld, pl_rows=pl_rows, Wo=ds["Wo"],
+                 npix=self.B * ds["Ho"] * ds["Wo"], name=f"ds{ds['i']}", data_only=data_only)
+    self._ln_bwd(ds["mod"].norm, ds["dplanes"].data_ptr(), ld, ds["omap"].data_ptr(), ds["xh"].data_ptr(),
+                 ds["rs"].data_ptr(), ds["npix"], Cs, src["g"].data_ptr(), ds["src_rows"].data_ptr(), 0, 0, data_only)
 
 
 def _emit_conv_blocks_bwd(self, lv: dict, input_grad: bool = True) -> None:
@@ -359,10 +341,10 @@ def _emit_conv_blocks_bwd(self, lv: dict, input_grad: bool = True) -> None:
             _conv_wgrad(self, dz=lv["dzB"].data_ptr(), lddz=ld, x=sv["h16"].data_ptr(), ldx=ld, x_rows=rows, rows=rows,
                         cout=Cc, cin=Cc, shifts=shifts, conv_weight=blk.conv2.weight, name="convB", bias=bias_b,
                         bias_rows=pix, bias_nrows=npix)
-        self._bgemm(a=lv["dzB"].data_ptr(), a_rows=rows, lda=ld, b=sv["wT2"].data_ptr(), b_rows=Cc, ldb=9 * _ru(Cc, 64),
-                    m=rows, n=Cc, kc=Cc, taps=lv["taps"], act=L.ACT_GELU_BWD, aux=sv["rawA"].data_ptr(), ld_aux=ld,
-                    aux_scale=bnA["sc"].data_ptr(), aux_shift=bnA["sh"].data_ptr(),
-                    row_map=interior, out_f16=lv["dyA"].data_ptr(), ld_o16=ld, flops=2.0 * npix * Cc * Cc * 9)
+        self._gemm(a=lv["dzB"].data_ptr(), a_rows=rows, lda=ld, b=sv["wT2"].data_ptr(), b_rows=Cc, ldb=9 * _ru(Cc, 64),
+                   m=rows, n=Cc, kc=Cc, taps=lv["taps"], act=L.ACT_GELU_BWD, aux=sv["rawA"].data_ptr(), ld_aux=ld,
+                   aux_scale=bnA["sc"].data_ptr(), aux_shift=bnA["sh"].data_ptr(), row_map=interior,
+                   out_f16=lv["dyA"].data_ptr(), ld_o16=ld, target=self.bwd_ops, m_alg=npix)
         self._before_write(lv["dzA"].data_ptr())
         _bn_bwd(self, bnA, lv["dyA"].data_ptr(), 1, ld, pix, sv["rawA"].data_ptr(), ld, pix, npix, L.ACT_NONE,
                 lv["dzA"].data_ptr(), ld, pix, None, data_only)
@@ -373,9 +355,9 @@ def _emit_conv_blocks_bwd(self, lv: dict, input_grad: bool = True) -> None:
         if sv is lv["blocks_sv"][0] and not input_grad:
             continue
         # g += conv1 data gradient
-        self._bgemm(a=lv["dzA"].data_ptr(), a_rows=rows, lda=ld, b=sv["wT1"].data_ptr(), b_rows=Cc, ldb=9 * _ru(Cc, 64),
-                    m=rows, n=Cc, kc=Cc, taps=lv["taps"], row_map=interior, resid=g, ld_resid=Cc, out_f32=g, ld_o32=Cc,
-                    flops=2.0 * npix * Cc * Cc * 9)
+        self._gemm(a=lv["dzA"].data_ptr(), a_rows=rows, lda=ld, b=sv["wT1"].data_ptr(), b_rows=Cc, ldb=9 * _ru(Cc, 64),
+                   m=rows, n=Cc, kc=Cc, taps=lv["taps"], row_map=interior, resid=g, ld_resid=Cc, out_f32=g, ld_o32=Cc,
+                   target=self.bwd_ops, m_alg=npix)
 
 
 def _emit_conv_part_bwd(self) -> None:
@@ -409,31 +391,18 @@ def _emit_conv_part_bwd(self) -> None:
     bn2, bn1 = st["bn2"], st["bn1"]
     _bn_bwd(self, bn2, lv0["g"].data_ptr(), 0, dim, lv0["pix"].data_ptr(), st["raw2"].data_ptr(), lv0["ld"],
             lv0["pix"].data_ptr(), B * H0 * W0, L.ACT_RELU, dY2.data_ptr(), lv0["ld"], q_of_pix.data_ptr(), None, data_only)
-    taps = self._s2_taps(W0)
-    shifts = [p * pl_rows + s for (s, p) in taps]
-    if not data_only:
-        _conv_wgrad(self, dz=dY2.data_ptr(), lddz=lv0["ld"], x=st["planes"].data_ptr(), ldx=ld_in, x_rows=4 * pl_rows,
-                    rows=pl_rows, cout=dim, cin=in_dim, shifts=shifts, conv_weight=pe[3].weight, name="stem2")
-    co_pad = _ru(dim, 64)
     dplanes = nb.new("stem.dplanes16", (4 * pl_rows, ld_in), torch.float16)
-    for p in range(4):
-        tl_ = [t for t in range(9) if taps[t][1] == p]
-        buf = nb.new(f"stem.wT.{p}", (in_dim, len(tl_) * co_pad), torch.float16)
-        t9 = tl_ + [0] * (9 - len(tl_))
-        self._op(self.prep_ops, "fvit_pack_conv3x3_taps_f16", pe[3].weight.data_ptr(), buf.data_ptr(), dim, in_dim, co_pad, 1,
-                 len(tl_), *t9)
-        self._bgemm(a=dY2.data_ptr(), a_rows=pl_rows, lda=lv0["ld"], b=buf.data_ptr(), b_rows=in_dim, ldb=len(tl_) * co_pad,
-                    m=pl_rows, n=in_dim, kc=dim, taps=[(-taps[t][0], 0) for t in tl_],
-                    out_f16=dplanes.data_ptr() + 2 * p * pl_rows * ld_in, ld_o16=ld_in,
-                    flops=2.0 * B * H0 * W0 * in_dim * dim * len(tl_))
+    _s2_conv_bwd(self, conv=pe[3], wT=_s2_dgrad_operands(self, "stem", pe[3], W0), dY=dY2.data_ptr(), lddy=lv0["ld"],
+                 planes=st["planes"].data_ptr(), dplanes=dplanes.data_ptr(), ld=ld_in, pl_rows=pl_rows, Wo=W0,
+                 npix=B * H0 * W0, name="stem2", data_only=data_only)
     dz1 = nb.new("stem.dz1", (npix1, ld_in), torch.float16)
     _bn_bwd(self, bn1, dplanes.data_ptr(), 1, ld_in, st["stem_map"].data_ptr(), st["raw1"].data_ptr(), ld_in,
             st["stem_map"].data_ptr(), npix1, L.ACT_RELU, dz1.data_ptr(), ld_in, None, None, data_only)
     k1, sld = st["k1"], st["sld"]
     if not data_only:
-        self._bgemm(a=dz1.data_ptr(), a_rows=npix1, lda=ld_in, a_mn=True, b=st["col16"].data_ptr(), b_rows=npix1, ldb=sld,
-                    b_mn=True, m=in_dim, n=k1, kc=npix1, split_k=self._split_k(in_dim, k1, npix1), alpha_ptr=inv,
-                    out_f32=self.G(pe[0].weight), ld_o32=k1, flops=2.0 * npix1 * in_dim * k1)
+        self._gemm(a=dz1.data_ptr(), a_rows=npix1, lda=ld_in, a_mn=True, b=st["col16"].data_ptr(), b_rows=npix1, ldb=sld,
+                   b_mn=True, m=in_dim, n=k1, kc=npix1, split_k=self._split_k(in_dim, k1, npix1), alpha_ptr=inv,
+                   out_f32=self.G(pe[0].weight), ld_o32=k1, target=self.bwd_ops)
     if self.want_dx:
         # the image gradient (fp32 NCHW, like x): the backward of conv1, 3x3 / stride 2 / pad 1, as a gather
         cin = m.cfg["in_chans"]
@@ -445,8 +414,8 @@ def _emit_conv_part_bwd(self) -> None:
             # any other channel count: the tap products dcol = dz1 . W1 / S on tensor cores, then a gather of them
             ldc = _ru(k1, 4)
             dcol = nb.new("stem.dcol", (npix1, ldc), torch.float32)
-            self._bgemm(a=dz1.data_ptr(), a_rows=npix1, lda=ld_in, b=st["w1"].data_ptr(), b_rows=in_dim, ldb=sld, b_mn=True,
-                        m=npix1, n=k1, kc=in_dim, alpha_ptr=inv, out_f32=dcol.data_ptr(), ld_o32=ldc)
+            self._gemm(a=dz1.data_ptr(), a_rows=npix1, lda=ld_in, b=st["w1"].data_ptr(), b_rows=in_dim, ldb=sld, b_mn=True,
+                       m=npix1, n=k1, kc=in_dim, alpha_ptr=inv, out_f32=dcol.data_ptr(), ld_o32=ldc, target=self.bwd_ops)
             self._op(ops, "fvit_stem_col2im", dcol.data_ptr(), ldc, B, cin, self.H, self.W, self.dx.data_ptr())
 
 

@@ -9,11 +9,7 @@ import torch
 import torch.nn as nn
 
 from . import lib as L
-from .engine import _ru
-
-
-def P(t):
-    return None if t is None else t.data_ptr()
+from .engine import P, _ru
 
 
 def _drop_buf(self, name: str, rate: float, groups: int, group_size: int):
@@ -182,44 +178,28 @@ def _inject(self, level: int, g=True) -> None:
 
 
 def _posemb_train(self, nm: str, tpe, n_side: int, Cc: int) -> dict:
-    """PosEmbMLPSwinv1D in training: same launch as eval plus the saved hidden activations."""
-    r = torch.arange(n_side, dtype=torch.float32)
-    grid = torch.stack(torch.meshgrid(r, r, indexing="ij"))
-    grid = (grid - n_side // 2) / (n_side // 2)
-    npts = n_side * n_side
-    coords = self.bufs.new(nm + ".coords", (npts, 2), torch.float32)
-    coords.copy_(grid.flatten(1).t())
-    hidden = self.bufs.new(nm + ".hidden", (npts, 512), torch.float32)
-    if tuple(tpe.relative_bias.shape) != (1, npts, Cc):
-        tpe.relative_bias = torch.zeros(1, npts, Cc, device=self.device)
-    self._op(self.prep_ops, "fvit_cpb_mlp_fwd", coords.data_ptr(), npts, tpe.cpb_mlp[0].weight.data_ptr(),
-             tpe.cpb_mlp[0].bias.data_ptr(), tpe.cpb_mlp[2].weight.data_ptr(), Cc, tpe.relative_bias.data_ptr(),
-             hidden.data_ptr())
-    return dict(mod=tpe, coords=coords, hidden=hidden, out=tpe.relative_bias, npts=npts, D=Cc,
-                dout=("scr", self._scratch(nm + ".dpe", npts * Cc)))
+    """Plan._emit_pos_embed saving the MLP's hidden activations, plus the scratch slice of its output gradient"""
+    hidden = self.bufs.new(nm + ".hidden", (n_side ** 2, 512), torch.float32)
+    pe = self._emit_pos_embed(nm, tpe, n_side, Cc, hidden=hidden)
+    pe["dout"] = ("scr", self._scratch(nm + ".dpe", pe["npts"] * Cc))
+    return pe
 
 
 def _bias_train(self, nm: str, rpb, S: int) -> dict:
-    """PosEmbMLPSwinv2D in training: table MLP (hidden saved) + gather/sigmoid into relative_bias."""
+    """Plan._emit_bias saving the table MLP's hidden activations, plus the scratch slices of the bias and table
+    gradients"""
     npts = rpb.relative_coords_table.shape[1] * rpb.relative_coords_table.shape[2]
-    table = self.bufs.new(nm + ".table", (npts, rpb.num_heads), torch.float32)
     hidden = self.bufs.new(nm + ".hidden", (npts, 512), torch.float32)
-    if tuple(rpb.relative_bias.shape) != (1, rpb.num_heads, S, S):
-        rpb.relative_bias = torch.zeros(1, rpb.num_heads, S, S, device=self.device)
-    self._op(self.prep_ops, "fvit_cpb_mlp_fwd", rpb.relative_coords_table.data_ptr(), npts,
-             rpb.cpb_mlp[0].weight.data_ptr(), rpb.cpb_mlp[0].bias.data_ptr(), rpb.cpb_mlp[2].weight.data_ptr(),
-             rpb.num_heads, table.data_ptr(), hidden.data_ptr())
-    self._op(self.prep_ops, "fvit_attn_bias_fwd", table.data_ptr(), rpb.relative_position_index.data_ptr(),
-             rpb.num_heads, S, rpb.window ** 2, rpb.relative_bias.data_ptr())
-    return dict(mod=rpb, hidden=hidden, out=rpb.relative_bias, npts=npts, S=S,
-                dbias=("scr", self._scratch(nm + ".dbias", rpb.num_heads * S * S)),
-                dtable=("scr", self._scratch(nm + ".dtable", npts * rpb.num_heads)))
+    bs = self._emit_bias(nm, rpb, S, hidden=hidden)
+    bs["dbias"] = ("scr", self._scratch(nm + ".dbias", rpb.num_heads * S * S))
+    bs["dtable"] = ("scr", self._scratch(nm + ".dtable", npts * rpb.num_heads))
+    return bs
 
 
 def _attn_fwd_train(self, nm: str, attn, gamma, rows: int, groups: int, S: int, y16, qkv, ao, bias, stream_buf,
                     u16, rs=None) -> dict:
-    """Train-mode copy of Plan._emit_attention: same three launches, un-folded layer scale so that the
-    branch output u = proj(...) + b can be saved (u16) for the layer-scale gradient."""
+    """Train-mode Plan._emit_attention: the three-launch attention with the layer scale un-folded, so that the branch
+    output u = proj(...) + b can be saved (u16) for the layer-scale gradient."""
     Cc, h, hd = attn.qkv.in_features, attn.num_heads, attn.head_dim
     hdp = self._head_pad(hd)
     kind = self._attn_kind(S, hdp)
@@ -232,23 +212,9 @@ def _attn_fwd_train(self, nm: str, attn, gamma, rows: int, groups: int, S: int, 
     if not use_tc:
         hdp = hd
     Cp = h * hdp
-    qb = attn.qkv.bias
-    if hdp == hd:
-        wq, ldq = self._pack_linear(nm + ".qkv", attn.qkv)
-        qb_ptr = P(qb)
-    else:
-        ldq = _ru(Cc, 8)
-        wq = self.bufs.new(nm + ".qkv.w16", (3 * Cp, ldq), torch.float16)
-        self._op(self.prep_ops, "fvit_cast_headpad_f16", attn.qkv.weight.data_ptr(), Cc, wq.data_ptr(), ldq, 3 * Cp,
-                 Cc, hd, hdp, 1, 0)
-        qb_ptr = None
-        if qb is not None:
-            qbp = self.bufs.new(nm + ".qkv.bias_pad", (3 * Cp,), torch.float32)
-            self._op(self.prep_ops, "fvit_vec_headpad_f32", qb.data_ptr(), qbp.data_ptr(), 3 * Cp, hd, hdp)
-            qb_ptr = qbp.data_ptr()
+    wq, ldq, qb_ptr, wp, ldp = self._pack_attention(nm, attn, hdp)
     self._gemm(a=y16.data_ptr(), a_rows=rows, lda=Cc, b=wq.data_ptr(), ldb=ldq, m=rows, n=3 * Cp, kc=Cc,
-               col_shift=qb_ptr, out_f16=qkv.data_ptr(), ld_o16=3 * Cp)
-    self.op_flops[len(self.ops) - 1] = 2.0 * rows * 3 * Cc * Cc
+               col_shift=qb_ptr, out_f16=qkv.data_ptr(), ld_o16=3 * Cp, flops=2.0 * rows * 3 * Cc * Cc)
     scale = float(getattr(attn, "scale", hd ** -0.5))   # qk_scale or head_dim ** -0.5 (fv.py:544)
     lse = None
     if kind == "loop":
@@ -262,41 +228,16 @@ def _attn_fwd_train(self, nm: str, attn, gamma, rows: int, groups: int, S: int, 
         self._op(self.ops, "fvit_attn_core_fwd", qkv.data_ptr(), 3 * Cp, groups, S, h, hd, bias["out"].data_ptr(),
                  scale, ao.data_ptr(), Cp, None)
     self.op_flops[len(self.ops) - 1] = 4.0 * groups * h * S * S * hd
-    lin = attn.proj
-    n = lin.weight.shape[0]
-    if hdp == hd:
-        wp, ldp = self._pack_linear(nm + ".proj", lin)
-    else:
-        ldp = Cp
-        wp = self.bufs.new(nm + ".proj.w16", (n, Cp), torch.float16)
-        self._op(self.prep_ops, "fvit_cast_headpad_f16", lin.weight.data_ptr(), Cc, wp.data_ptr(), Cp, n, Cp, hd, hdp,
-                 0, 1)
-    has_ls = isinstance(gamma, torch.Tensor)
-    self._gemm_train_branch(a=ao.data_ptr(), lda=Cp, w=wp.data_ptr(), ldw=ldp, rows=rows, n=n, k=Cp, bias=lin.bias,
-                            gamma=gamma if has_ls else None, stream_buf=stream_buf, u16=u16 if has_ls else None, rs=rs)
-    self.op_flops[len(self.ops) - 1] = 2.0 * rows * n * Cc
+    # x += droppath_row * gamma * u, u = proj(...) + b saved (u16) when gamma is a layer-scale parameter
+    ls = gamma if isinstance(gamma, torch.Tensor) else None
+    u16 = u16 if ls is not None else None
+    n = attn.proj.weight.shape[0]
+    self._gemm(a=ao.data_ptr(), a_rows=rows, lda=Cp, b=wp.data_ptr(), ldb=ldp, m=rows, n=n, kc=Cp,
+               col_shift=P(attn.proj.bias), col_scale2=P(ls), row_scale=rs, out_pre16=P(u16),
+               ld_pre16=n if ls is not None else 0, resid=stream_buf, ld_resid=n, out_f32=stream_buf, ld_o32=n,
+               flops=2.0 * rows * n * Cc)
     return dict(rs=rs, attn=attn, wq=wq, ldq=ldq, wp=wp, ldp=ldp, hd=hd, hdp=hdp, Cp=Cp, use_tc=use_tc, kind=kind, lse=lse,
-                scale=scale, S=S,
-                groups=groups, rows=rows, qkv=qkv, ao=ao, y16=y16, bias=bias, u16=u16 if has_ls else None)
-
-
-def _gemm_train_branch(self, *, a, lda, w, ldw, rows, n, k, bias, gamma, stream_buf, u16, rs=None) -> None:
-    """x += droppath_row * gamma * (a @ W^T + b), saving u = a @ W^T + b (fp16) when gamma is a parameter."""
-    g = L.GemmArgs()
-    g.a, g.a_rows, g.lda, g.a_planes = a, rows, lda, 1
-    g.b, g.b_rows, g.ldb = w, n, ldw
-    g.m, g.n, g.kc, g.ntaps = rows, n, k, 1
-    g.split_k, g.alpha = 1, 1.0
-    g.col_shift = P(bias)
-    if gamma is not None:
-        g.col_scale2 = gamma.data_ptr()
-        g.out_pre16, g.ld_out_pre16 = u16.data_ptr(), n
-    g.row_scale = rs
-    g.resid, g.ld_resid, g.out_f32, g.ld_out_f32 = stream_buf, n, stream_buf, n
-    self._gemm_keep.append(g)
-    import ctypes as C
-    self.ops.append((self.lib.fvit_gemm, (C.byref(g),), "fvit_gemm"))
-    self.op_flops[len(self.ops) - 1] = 2.0 * rows * n * k
+                scale=scale, S=S, groups=groups, rows=rows, qkv=qkv, ao=ao, y16=y16, bias=bias, u16=u16)
 
 
 def _emit_token_level_train(self, i: int, level, tl: dict) -> None:
@@ -396,26 +337,18 @@ def _mlp_fwd_train(self, nm: str, mlp, gamma, rows: int, y16, p16, h16, stream_b
     w1, ld1 = self._pack_linear(nm + ".fc1", mlp.fc1)
     # fc1: gelu'(pre-activation) saved through out_pre16 (one erf evaluation yields GELU and its derivative, so the
     # fc2 data-gradient epilogue is a plain multiply: FVIT_ACT_MUL_AUX), GELU output is the fc2 operand
-    g = L.GemmArgs()
-    g.a, g.a_rows, g.lda, g.a_planes = y16.data_ptr(), rows, k1, 1
-    g.b, g.b_rows, g.ldb = w1.data_ptr(), n1, ld1
-    g.m, g.n, g.kc, g.ntaps, g.split_k, g.alpha = rows, n1, k1, 1, 1, 1.0
-    g.col_shift, g.act = mlp.fc1.bias.data_ptr(), L.ACT_GELU
-    g.out_f16, g.ld_out_f16 = h16.data_ptr(), n1
-    g.out_pre16, g.ld_out_pre16 = p16.data_ptr(), n1
-    g.pre_is_grad = 1
-    self._gemm_keep.append(g)
-    import ctypes as C
-    self.ops.append((self.lib.fvit_gemm, (C.byref(g),), "fvit_gemm"))
-    self.op_flops[len(self.ops) - 1] = 2.0 * rows * n1 * k1
+    self._gemm(a=y16.data_ptr(), a_rows=rows, lda=k1, b=w1.data_ptr(), ldb=ld1, m=rows, n=n1, kc=k1,
+               col_shift=mlp.fc1.bias.data_ptr(), act=L.ACT_GELU, out_f16=h16.data_ptr(), ld_o16=n1,
+               out_pre16=p16.data_ptr(), ld_pre16=n1, pre_is_grad=True)
+    # fc2: x += droppath_row * gamma * u, u = fc2(h) saved (u16) when gamma is a layer-scale parameter
     n2, k2 = mlp.fc2.weight.shape
     w2, ld2 = self._pack_linear(nm + ".fc2", mlp.fc2)
-    has_ls = isinstance(gamma, torch.Tensor)
-    self._gemm_train_branch(a=h16.data_ptr(), lda=k2, w=w2.data_ptr(), ldw=ld2, rows=rows, n=n2, k=k2,
-                            bias=mlp.fc2.bias, gamma=gamma if has_ls else None, stream_buf=stream_buf,
-                            u16=u16 if has_ls else None, rs=rs)
-    return dict(rs=rs, mlp=mlp, w1=w1, ld1=ld1, w2=w2, ld2=ld2, rows=rows, y16=y16, p16=p16, h16=h16,
-                u16=u16 if has_ls else None)
+    ls = gamma if isinstance(gamma, torch.Tensor) else None
+    u16 = u16 if ls is not None else None
+    self._gemm(a=h16.data_ptr(), a_rows=rows, lda=k2, b=w2.data_ptr(), ldb=ld2, m=rows, n=n2, kc=k2,
+               col_shift=P(mlp.fc2.bias), col_scale2=P(ls), row_scale=rs, out_pre16=P(u16),
+               ld_pre16=n2 if ls is not None else 0, resid=stream_buf, ld_resid=n2, out_f32=stream_buf, ld_o32=n2)
+    return dict(rs=rs, mlp=mlp, w1=w1, ld1=ld1, w2=w2, ld2=ld2, rows=rows, y16=y16, p16=p16, h16=h16, u16=u16)
 
 
 def _emit_head_train(self, prev: dict) -> None:
@@ -589,11 +522,11 @@ def _emit_head_bwd(self, feat: dict) -> None:
     self._op(ops, "fvit_colsum", self._dlogits.data_ptr(), 0, ncp, None, None, 0, B, ncls, None, None,
              self.G(m.head.bias), None)
     # dW_head = dl^T pooled ; dpooled = dl W_head
-    self._bgemm(a=dl16.data_ptr(), a_rows=B, lda=ldl, a_mn=True, b=hs["pooled"].data_ptr(), b_rows=B,
-                ldb=hs["pooled"].stride(0), b_mn=True, m=ncls, n=nf, kc=B, alpha_ptr=inv, out_f32=self.G(m.head.weight),
-                ld_o32=nf)
-    self._bgemm(a=dl16.data_ptr(), a_rows=B, lda=ldl, b=hs["hw16"].data_ptr(), b_rows=ncls, ldb=hs["ldh"], b_mn=True,
-                m=B, n=nf, kc=ncls, out_f32=dpool.data_ptr(), ld_o32=nf)
+    self._gemm(a=dl16.data_ptr(), a_rows=B, lda=ldl, a_mn=True, b=hs["pooled"].data_ptr(), b_rows=B,
+               ldb=hs["pooled"].stride(0), b_mn=True, m=ncls, n=nf, kc=B, alpha_ptr=inv, out_f32=self.G(m.head.weight),
+               ld_o32=nf, target=ops)
+    self._gemm(a=dl16.data_ptr(), a_rows=B, lda=ldl, b=hs["hw16"].data_ptr(), b_rows=ncls, ldb=hs["ldh"], b_mn=True,
+               m=B, n=nf, kc=ncls, out_f32=dpool.data_ptr(), ld_o32=nf, target=ops)
     _pool_bn_bwd(self, feat, dpool)
 
 
@@ -655,132 +588,97 @@ def _bias_bwd(self, bs: dict) -> None:
     self._bwd_side.update(range(n0, len(self.bwd_ops)))
 
 
+# TrainPlan._branch of a branch without layer scale
 _ONE = dict(gamma=None, s=None, inv_s=("scal", 2), w_alpha=("scal", 1))
 
 
-def _data_only_entry(self, tl: dict, br: dict, g_ptr: int, rows: int, Cc: int, rs) -> None:
-    """entry of a data-only residual branch: tl["dz"] = fp16 operand copy of g (layer scale and its normaliser folded
-    in) -- fvit_branch_grad without the bias and layer-scale sums"""
-    self._before_write(tl["dz"].data_ptr())
-    self._op(self.bwd_ops, "fvit_cast_scale_f16", g_ptr, Cc, None, rows, Cc, P(br["gamma"]), br["s"], tl["dz"].data_ptr(), Cc,
-             rs)
+def _branch_entry(self, tl: dict, br: dict, g_ptr: int, rows: int, Cc: int, rs, u16, bias, data_only: bool) -> bool:
+    """Entry of the backward of a residual branch x += gamma * (... + bias) on gradient rows g_ptr[0:rows]: tl["dz"] =
+    fp16 operand copy of g (layer scale, its normaliser and the drop-path row scale folded in), and unless data_only the
+    layer-scale gradient from the saved branch output u16 -- in one pass with the bias gradient (fvit_branch_grad)
+    where that kernel applies. Returns whether the bias gradient was taken."""
+    ops, dz = self.bwd_ops, tl["dz"].data_ptr()
+    self._before_write(dz)
+    if not data_only and Cc % 8 == 0 and bias is not None:
+        has_g = br["gamma"] is not None
+        self._op(ops, "fvit_branch_grad", g_ptr, Cc, rows, Cc, P(br["gamma"]), br["s"], rs, dz, Cc, br["w_alpha"],
+                 self.G(bias), P(u16), Cc, ("scal", 1), self.G(br["gamma"]) if has_g else None)
+        return True
+    self._op(ops, "fvit_cast_scale_f16", g_ptr, Cc, None, rows, Cc, P(br["gamma"]), br["s"], dz, Cc, rs)
+    if br["gamma"] is not None and not data_only:
+        self._op(ops, "fvit_colsum", g_ptr, 0, Cc, None, u16.data_ptr(), Cc, rows, Cc, None, ("scal", 1),
+                 self.G(br["gamma"]), rs)
+    return False
 
 
-def _mlp_bwd(self, tl: dict, ms: dict, gamma, g_ptr: int, rows: int, ln: nn.LayerNorm, xh, rs, in_map=None,
-             data_only: bool = False) -> None:
-    """Backward of x += gamma * fc2(gelu(fc1(LN(x)))) on gradient rows g_ptr[0:rows]."""
-    ops = self.bwd_ops
+def _mlp_bwd(self, tl: dict, ms: dict, gamma, g_ptr: int, rows: int, ln: nn.LayerNorm, xh, rs, data_only: bool) -> None:
+    """Backward of x += gamma * fc2(gelu(fc1(LN(x)))) on gradient rows g_ptr[0:rows]; data_only: the data gradient
+    alone (no weight-gradient GEMM, no bias / layer-scale / LayerNorm parameter gradient)."""
     mlp = ms["mlp"]
     Cc, hid = mlp.fc1.weight.shape[1], mlp.fc1.weight.shape[0]
     br = self._branch(gamma)
-    dz, dp, dy = tl["dz"], tl["dp"], tl["dy"]
-    if data_only:
-        _data_only_entry(self, tl, br, g_ptr, rows, Cc, ms["rs"])
-        self._linear_bwd(lin=mlp.fc2, w16=ms["w2"].data_ptr(), ldw=ms["ld2"], x16=None, ldx=0, dz16=dz.data_ptr(), lddz=Cc,
-                         rows=rows, n_out=Cc, k_in=hid, br=br, dx16=dp.data_ptr(), lddx=hid, dx_act=L.ACT_MUL_AUX,
-                         dx_aux=ms["p16"].data_ptr(), ld_aux=hid, data_only=True)
-        self._linear_bwd(lin=mlp.fc1, w16=ms["w1"].data_ptr(), ldw=ms["ld1"], x16=None, ldx=0, dz16=dp.data_ptr(), lddz=hid,
-                         rows=rows, n_out=hid, k_in=Cc, br=_ONE, dx16=dy.data_ptr(), lddx=Cc, data_only=True)
-        self._op(ops, "fvit_ln_dgrad", dy.data_ptr(), Cc, None, xh.data_ptr(), Cc, rs.data_ptr(), ln.weight.data_ptr(), rows,
-                 Cc, g_ptr, Cc, in_map, 1, 0)
-        return
-    fused = Cc % 8 == 0 and mlp.fc2.bias is not None
-    self._before_write(dz.data_ptr())
-    if fused:   # operand cast + fc2 bias gradient + layer-scale gradient in one pass over g
-        has_g = br["gamma"] is not None
-        self._op(ops, "fvit_branch_grad", g_ptr, Cc, rows, Cc, P(br["gamma"]), br["s"], ms["rs"], dz.data_ptr(), Cc,
-                 br["w_alpha"], self.G(mlp.fc2.bias), ms["u16"].data_ptr() if has_g else None, Cc, ("scal", 1),
-                 self.G(gamma) if has_g else None)
-    else:
-        self._op(ops, "fvit_cast_scale_f16", g_ptr, Cc, None, rows, Cc, P(br["gamma"]), br["s"], dz.data_ptr(), Cc, ms["rs"])
-        if br["gamma"] is not None:
-            self._op(ops, "fvit_colsum", g_ptr, 0, Cc, None, ms["u16"].data_ptr(), Cc, rows, Cc, None, ("scal", 1),
-                     self.G(gamma), ms["rs"])
-    # fc2: dW2, db2, dp = (dz W2) o gelu'(p)   (p16 holds gelu'(p), saved by the forward epilogue)
-    self._linear_bwd(lin=mlp.fc2, w16=ms["w2"].data_ptr(), ldw=ms["ld2"], x16=ms["h16"].data_ptr(), ldx=hid,
-                     dz16=dz.data_ptr(), lddz=Cc, rows=rows, n_out=Cc, k_in=hid, br=br, dx16=dp.data_ptr(), lddx=hid,
-                     dx_act=L.ACT_MUL_AUX, dx_aux=ms["p16"].data_ptr(), ld_aux=hid, bias_done=fused,
-                     dx_colsum=(self.G(mlp.fc1.bias), ("scal", 1)) if mlp.fc1.bias is not None else None)
-    one = dict(gamma=None, s=None, inv_s=("scal", 2), w_alpha=("scal", 1))
-    # (fc1's bias gradient = column sums of dp, taken in the epilogue of the GEMM that produced dp)
-    self._linear_bwd(lin=mlp.fc1, w16=ms["w1"].data_ptr(), ldw=ms["ld1"], x16=ms["y16"].data_ptr(), ldx=Cc,
-                     dz16=dp.data_ptr(), lddz=hid, rows=rows, n_out=hid, k_in=Cc, br=one, dx16=dy.data_ptr(), lddx=Cc,
-                     bias_done=mlp.fc1.bias is not None)
-    self._op(ops, "fvit_ln_bwd", dy.data_ptr(), Cc, None, xh.data_ptr(), Cc, rs.data_ptr(), ln.weight.data_ptr(), rows, Cc,
-             g_ptr, Cc, in_map, 1, 0, ("scal", 1), self.G(ln.weight), self.G(ln.bias))
+    dz, dp, dy = tl["dz"].data_ptr(), tl["dp"].data_ptr(), tl["dy"].data_ptr()
+    bias_done = _branch_entry(self, tl, br, g_ptr, rows, Cc, ms["rs"], ms["u16"], mlp.fc2.bias, data_only)
+    # fc2: dW2, db2, dp = (dz W2) o gelu'(p)   (p16 holds gelu'(p), saved by the forward epilogue); fc1's bias gradient =
+    # column sums of dp, taken in the epilogue of the GEMM that produces dp
+    fc1_db = (self.G(mlp.fc1.bias), ("scal", 1)) if mlp.fc1.bias is not None and not data_only else None
+    self._linear_bwd(lin=mlp.fc2, w16=ms["w2"].data_ptr(), ldw=ms["ld2"], x16=ms["h16"].data_ptr(), ldx=hid, dz16=dz,
+                     lddz=Cc, rows=rows, n_out=Cc, k_in=hid, br=br, dx16=dp, lddx=hid, dx_act=L.ACT_MUL_AUX,
+                     dx_aux=ms["p16"].data_ptr(), ld_aux=hid, bias_done=bias_done, dx_colsum=fc1_db, data_only=data_only)
+    self._linear_bwd(lin=mlp.fc1, w16=ms["w1"].data_ptr(), ldw=ms["ld1"], x16=ms["y16"].data_ptr(), ldx=Cc, dz16=dp,
+                     lddz=hid, rows=rows, n_out=hid, k_in=Cc, br=_ONE, dx16=dy, lddx=Cc,
+                     bias_done=mlp.fc1.bias is not None, data_only=data_only)
+    self._ln_bwd(ln, dy, Cc, None, xh.data_ptr(), rs.data_ptr(), rows, Cc, g_ptr, None, 1, 0, data_only)
 
 
-def _attn_data_only(self, tl: dict, at: dict, br: dict, g_ptr: int) -> None:
-    """proj / attention core / qkv data gradients of a data-only level's attention branch, from g into tl["dy"]"""
-    attn = at["attn"]
-    Cc, Cp, rows = attn.qkv.in_features, at["Cp"], at["rows"]
-    dz, dy, dao, dqkv = tl["dz"], tl["dy"], tl["dao"], tl["dqkv"]
-    _data_only_entry(self, tl, br, g_ptr, rows, Cc, at["rs"])
-    self._linear_bwd(lin=attn.proj, w16=at["wp"].data_ptr(), ldw=at["ldp"], x16=None, ldx=0, dz16=dz.data_ptr(), lddz=Cc,
-                     rows=rows, n_out=Cc, k_in=Cp, br=br, dx16=dao.data_ptr(), lddx=Cp, flops_k=Cc, data_only=True)
-    _emit_attn_core_bwd(self, at, dao, dqkv, at["groups"], at["S"], want_dbias=False)
-    self._linear_bwd(lin=attn.qkv, w16=at["wq"].data_ptr(), ldw=at["ldq"], x16=None, ldx=0, dz16=dqkv.data_ptr(),
-                     lddz=3 * Cp, rows=rows, n_out=3 * Cp, k_in=Cc, br=_ONE, dx16=dy.data_ptr(), lddx=Cc,
-                     flops_k=Cc * (3 * Cc) / (3 * Cp), data_only=True)
-
-
-def _attn_bwd(self, tl: dict, at: dict, gamma, g_ptr: int, ln: nn.LayerNorm, xh, rs, in_map, g_base: int,
-              clear_moved: bool, data_only: bool = False) -> None:
-    """Backward of x += gamma * proj(attn(qkv(LN(x)))); g_base = pointer the in_map row indices refer to."""
+def _attn_bwd(self, tl: dict, at: dict, gamma, g_ptr: int, ln: nn.LayerNorm, xh, rs, pe, data_only: bool,
+              in_map=None, carrier: bool = False) -> None:
+    """Backward of x += gamma * proj(attn(qkv(LN(x + pe)))) on gradient rows g_ptr[0:rows], then of the positional
+    embedding pe (_posemb_train, or None) added at the LayerNorm's input.
+    Window tokens: the LayerNorm backward routes the gradient of the rows it gathered back through in_map
+    (norm1_gather: the carrier slots to the raster carrier rows). Carrier tokens (carrier=True): g_ptr addresses the
+    raster carrier rows of the level's gradient; hat_norm1's input gradient is accumulated there in place, then moved
+    to the xs carrier rows hat_norm1 gathered from (ct_gather).
+    data_only: the data gradient alone (no weight-gradient GEMM, no bias / layer-scale / attention-bias / positional-MLP
+    / LayerNorm parameter gradient)."""
     ops = self.bwd_ops
     attn = at["attn"]
     Cc, h, hd, hdp, Cp = attn.qkv.in_features, attn.num_heads, at["hd"], at["hdp"], at["Cp"]
     rows, S, groups = at["rows"], at["S"], at["groups"]
+    unpad = hdp != hd and not data_only   # parameter gradients of head-padded operands are un-padded
     br = self._branch(gamma)
-    dz, dy, dao, dqkv = tl["dz"], tl["dy"], tl["dao"], tl["dqkv"]
-    if data_only:
-        _attn_data_only(self, tl, at, br, g_ptr)
-        self._op(ops, "fvit_ln_dgrad", dy.data_ptr(), Cc, None, xh.data_ptr(), Cc, rs.data_ptr(), ln.weight.data_ptr(), rows,
-                 Cc, g_ptr, Cc, in_map, 1, 1 if clear_moved else 0)
-        return
-    padded = hdp != hd
-    fused = Cc % 8 == 0 and attn.proj.bias is not None
-    self._before_write(dz.data_ptr())
-    if fused:   # operand cast + proj bias gradient + layer-scale gradient in one pass over g
-        has_g = br["gamma"] is not None
-        self._op(ops, "fvit_branch_grad", g_ptr, Cc, rows, Cc, P(br["gamma"]), br["s"], at["rs"], dz.data_ptr(), Cc,
-                 br["w_alpha"], self.G(attn.proj.bias), at["u16"].data_ptr() if has_g else None, Cc, ("scal", 1),
-                 self.G(gamma) if has_g else None)
-    else:
-        self._op(ops, "fvit_cast_scale_f16", g_ptr, Cc, None, rows, Cc, P(br["gamma"]), br["s"], dz.data_ptr(), Cc, at["rs"])
-        if br["gamma"] is not None:
-            self._op(ops, "fvit_colsum", g_ptr, 0, Cc, None, at["u16"].data_ptr(), Cc, rows, Cc, None, ("scal", 1),
-                     self.G(gamma), at["rs"])
+    dz, dy, dao, dqkv = tl["dz"].data_ptr(), tl["dy"].data_ptr(), tl["dao"], tl["dqkv"]
+    bias_done = _branch_entry(self, tl, br, g_ptr, rows, Cc, at["rs"], at["u16"], attn.proj.bias, data_only)
     # proj
-    if padded:
-        gWp = ("scr", self._scratch("dWproj_pad", Cc * Cp))
-    else:
-        gWp = self.G(attn.proj.weight)
-    self._linear_bwd(lin=attn.proj, w16=at["wp"].data_ptr(), ldw=at["ldp"], x16=at["ao"].data_ptr(), ldx=Cp,
-                     dz16=dz.data_ptr(), lddz=Cc, rows=rows, n_out=Cc, k_in=Cp, br=br, gW=gWp, gW_ld=Cp,
-                     dx16=dao.data_ptr(), lddx=Cp, flops_k=Cc, bias_done=fused)
-    if padded:
+    gWp = ("scr", self._scratch("dWproj_pad", Cc * Cp)) if unpad else None
+    self._linear_bwd(lin=attn.proj, w16=at["wp"].data_ptr(), ldw=at["ldp"], x16=at["ao"].data_ptr(), ldx=Cp, dz16=dz,
+                     lddz=Cc, rows=rows, n_out=Cc, k_in=Cp, br=br, gW=gWp, dx16=dao.data_ptr(), lddx=Cp, flops_k=Cc,
+                     bias_done=bias_done, data_only=data_only)
+    if unpad:
         self._op(ops, "fvit_unpad_heads_f32", gWp, Cp, self.G(attn.proj.weight), Cc, Cc, Cp, hd, hdp, 0, 1, None)
         self._bwd_side.add(len(ops) - 1)   # fresh scratch in, parameter gradient out: leaf launch
     # attention core
-    _emit_attn_core_bwd(self, at, dao, dqkv, groups, S)
-    _bias_bwd(self, at["bias"])
-    # qkv
-    one = dict(gamma=None, s=None, inv_s=("scal", 2), w_alpha=("scal", 1))
-    gWq, gbq = self.G(attn.qkv.weight), (self.G(attn.qkv.bias) if attn.qkv.bias is not None else None)
-    if padded:   # dW rows are head-padded: the GEMM epilogue scatters them through a row map, only the bias is un-padded
-        gbq = ("scr", self._scratch("dbqkv_pad", 3 * Cp))
+    _emit_attn_core_bwd(self, at, dao, dqkv, groups, S, want_dbias=not data_only)
+    if not data_only:
+        _bias_bwd(self, at["bias"])
+    # qkv: with padded heads the weight-gradient GEMM scatters its rows through a row map, only the bias is un-padded
+    gbq = ("scr", self._scratch("dbqkv_pad", 3 * Cp)) if unpad else None
     self._linear_bwd(lin=attn.qkv, w16=at["wq"].data_ptr(), ldw=at["ldq"], x16=at["y16"].data_ptr(), ldx=Cc,
-                     dz16=dqkv.data_ptr(), lddz=3 * Cp, rows=rows, n_out=3 * Cp, k_in=Cc, br=one, gW=gWq, gW_ld=Cc,
-                     gW_row_map=_unpad_row_map(self, 3 * h, hd, hdp) if padded else None,
-                     bias_to=gbq, dx16=dy.data_ptr(), lddx=Cc, flops_k=Cc * (3 * Cc) / (3 * Cp))
-    if padded:
-        if attn.qkv.bias is not None:
-            self._op(ops, "fvit_unpad_heads_f32", gbq, 1, self.G(attn.qkv.bias), 1, 3 * Cp, 1, hd, hdp, 1, 0, None)
-            self._bwd_side.add(len(ops) - 1)   # fresh scratch in, parameter gradient out: leaf launch
-    # LayerNorm (with the gather routing of the forward)
-    self._op(ops, "fvit_ln_bwd", dy.data_ptr(), Cc, None, xh.data_ptr(), Cc, rs.data_ptr(), ln.weight.data_ptr(), rows, Cc,
-             g_ptr, Cc, in_map, 1, 1 if clear_moved else 0, ("scal", 1), self.G(ln.weight), self.G(ln.bias))
+                     dz16=dqkv.data_ptr(), lddz=3 * Cp, rows=rows, n_out=3 * Cp, k_in=Cc, br=_ONE,
+                     gW_row_map=_unpad_row_map(self, 3 * h, hd, hdp) if unpad else None, bias_to=gbq, dx16=dy,
+                     lddx=Cc, flops_k=Cc * (3 * Cc) / (3 * Cp), data_only=data_only)
+    if unpad and attn.qkv.bias is not None:
+        self._op(ops, "fvit_unpad_heads_f32", gbq, 1, self.G(attn.qkv.bias), 1, 3 * Cp, 1, hd, hdp, 1, 0, None)
+        self._bwd_side.add(len(ops) - 1)   # fresh scratch in, parameter gradient out: leaf launch
+    # LayerNorm (with the gather routing of the forward), then the positional embedding: its gradient summed over the
+    # windows (over the images for the carriers)
+    self._ln_bwd(ln, dy, Cc, None, xh.data_ptr(), rs.data_ptr(), rows, Cc, g_ptr, in_map, 1, int(not carrier),
+                 data_only)
+    if pe is not None and not data_only:
+        self._op(ops, "fvit_group_sum", g_ptr, Cc, groups, S, 0 if carrier else tl["ncw"], Cc, ("scal", 1), pe["dout"])
+        _posemb_bwd(self, pe)
+    if carrier:
+        self._op(ops, "fvit_scatter_add_rows", g_ptr, Cc, tl["g"].data_ptr(), Cc, tl["ct_gather"].data_ptr(), rows, Cc)
 
 
 def _unpad_row_map(self, heads3: int, hd: int, hdp: int) -> int:
@@ -797,9 +695,12 @@ def _unpad_row_map(self, heads3: int, hd: int, hdp: int) -> int:
 
 
 def _emit_token_level_bwd(self, tl: dict, after_block=None) -> None:
-    """A data-only level (TrainPlan.data_only): the data-gradient GEMMs, the attention core without dbias, LayerNorm dx
-    and the carrier-token routing -- no weight-gradient GEMM, no bias / layer-scale / positional-MLP gradient."""
-    B, Cc, S, ncw, ws = self.B, tl["C"], tl["S"], tl["ncw"], tl["ws"]
+    """Backward of a transformer level from its gradient rows tl["g"], the blocks in reverse order -- per block the
+    carrier propagation, the window tokens' MLP and attention branches, then the carrier tokens' -- and then the global
+    tokenizer. after_block(k) runs once block k's parameter gradients are final. A data-only level
+    (TrainPlan.data_only): the data-gradient GEMMs, the attention core without dbias, LayerNorm dx and the carrier-token
+    routing -- no weight-gradient GEMM, no bias / layer-scale / positional-MLP gradient."""
+    B, Cc, S, ncw = self.B, tl["C"], tl["S"], tl["ncw"]
     nW, n_ct = tl["nW"], tl["n_ct"]
     ops = self.bwd_ops
     g_ptr = tl["g"].data_ptr()
@@ -814,21 +715,15 @@ def _emit_token_level_bwd(self, tl: dict, after_block=None) -> None:
             self._op(ops, "fvit_propagate_bwd", g_ptr, Cc, tl["xs"].data_ptr(), Cc, tl["prop_src"].data_ptr(), rows, Cc,
                      P(g1), ("scal", 1), self.G(g1) if g1 is not None and not do else None)
         # window branch (reverse order): MLP, attention + norm1 (routes carrier-slot gradients to the raster buffer)
-        _mlp_bwd(self, tl, sv["w_mlp"], blk.gamma4, g_ptr, rows, blk.norm2, w["xh2"], w["rs2"], data_only=do)
-        _attn_bwd(self, tl, sv["w_attn"], blk.gamma3, g_ptr, blk.norm1, w["xh1"], w["rs1"],
-                  tl["norm1_gather"].data_ptr() if has_ct else None, g_ptr, True, data_only=do)
-        if not do:
-            # positional embedding of the window tokens: sum over windows of the gradient at (x + pe)
-            self._op(ops, "fvit_group_sum", g_ptr, Cc, nW, S, ncw, Cc, ("scal", 1), sv["pe"]["dout"])
-            _posemb_bwd(self, sv["pe"])
+        _mlp_bwd(self, tl, sv["w_mlp"], blk.gamma4, g_ptr, rows, blk.norm2, w["xh2"], w["rs2"], do)
+        _attn_bwd(self, tl, sv["w_attn"], blk.gamma3, g_ptr, blk.norm1, w["xh1"], w["rs1"], sv["pe"], do,
+                  in_map=tl["norm1_gather"].data_ptr() if has_ct else None)
         if has_ct:
             c = sv["c"]
-            gc_ptr = g_ptr + tl["ctr0"] * Cc * 4
-            rows_c = B * n_ct
-            _mlp_bwd(self, tl, sv["c_mlp"], blk.gamma2, gc_ptr, rows_c, blk.hat_norm2, c["xh2"], c["rs2"], data_only=do)
-            # carrier attention; its LayerNorm gathered from the xs carrier rows (ct_dewindow): the
-            # gradient goes back there (row indices are relative to the level's g buffer)
-            _attn_bwd_carrier(self, tl, sv, blk, gc_ptr, g_ptr, data_only=do)
+            gc_ptr = g_ptr + tl["ctr0"] * Cc * 4   # the raster carrier rows
+            _mlp_bwd(self, tl, sv["c_mlp"], blk.gamma2, gc_ptr, B * n_ct, blk.hat_norm2, c["xh2"], c["rs2"], do)
+            _attn_bwd(self, tl, sv["c_attn"], blk.gamma1, gc_ptr, blk.hat_norm1, c["xh1"], c["rs1"], sv["hat_pe"], do,
+                      carrier=True)
         if after_block is not None:
             after_block(tl["blocks_sv"].index(sv))   # this block's parameter gradients are final
     level = self.model.levels[tl["level_index"]]
@@ -844,73 +739,6 @@ def _emit_token_level_bwd(self, tl: dict, after_block=None) -> None:
                  ("scal", 1), g_ptr, Cc, self.G(tk.pos_embed.weight), self.G(tk.pos_embed.bias))
 
 
-def _attn_bwd_carrier(self, tl: dict, sv: dict, blk, gc_ptr: int, g_ptr: int, data_only: bool = False) -> None:
-    """hat_attn + hat_norm1 backward. ln_bwd works on row indices of one buffer, so the raster rows are
-    addressed as rows of the level buffer (offset ctr0) and in_map = ct_gather (xs carrier rows)."""
-    ops = self.bwd_ops
-    B, Cc, n_ct = self.B, tl["C"], tl["n_ct"]
-    c = sv["c"]
-    at = sv["c_attn"]
-    rows_c = B * n_ct
-    # everything except the final LayerNorm backward is identical to the window case
-    attn = at["attn"]
-    h, hd, hdp, Cp = attn.num_heads, at["hd"], at["hdp"], at["Cp"]
-    br = self._branch(blk.gamma1)
-    dz, dy, dao, dqkv = tl["dz"], tl["dy"], tl["dao"], tl["dqkv"]
-    if data_only:
-        # the same three data gradients; hat_norm1's dx accumulated in place, then moved to the xs carrier rows
-        _attn_data_only(self, tl, at, br, gc_ptr)
-        self._op(ops, "fvit_ln_dgrad", dy.data_ptr(), Cc, None, c["xh1"].data_ptr(), Cc, c["rs1"].data_ptr(),
-                 blk.hat_norm1.weight.data_ptr(), rows_c, Cc, gc_ptr, Cc, None, 1, 0)
-        self._op(ops, "fvit_scatter_add_rows", gc_ptr, Cc, g_ptr, Cc, tl["ct_gather"].data_ptr(), rows_c, Cc)
-        return
-    padded = hdp != hd
-    fused = Cc % 8 == 0 and attn.proj.bias is not None
-    self._before_write(dz.data_ptr())
-    if fused:
-        has_g = br["gamma"] is not None
-        self._op(ops, "fvit_branch_grad", gc_ptr, Cc, rows_c, Cc, P(br["gamma"]), br["s"], at["rs"], dz.data_ptr(), Cc,
-                 br["w_alpha"], self.G(attn.proj.bias), at["u16"].data_ptr() if has_g else None, Cc, ("scal", 1),
-                 self.G(blk.gamma1) if has_g else None)
-    else:
-        self._op(ops, "fvit_cast_scale_f16", gc_ptr, Cc, None, rows_c, Cc, P(br["gamma"]), br["s"], dz.data_ptr(), Cc,
-                 at["rs"])
-        if br["gamma"] is not None:
-            self._op(ops, "fvit_colsum", gc_ptr, 0, Cc, None, at["u16"].data_ptr(), Cc, rows_c, Cc, None, ("scal", 1),
-                     self.G(blk.gamma1), at["rs"])
-    gWp = ("scr", self._scratch("dWproj_pad_c", Cc * Cp)) if padded else self.G(attn.proj.weight)
-    self._linear_bwd(lin=attn.proj, w16=at["wp"].data_ptr(), ldw=at["ldp"], x16=at["ao"].data_ptr(), ldx=Cp,
-                     dz16=dz.data_ptr(), lddz=Cc, rows=rows_c, n_out=Cc, k_in=Cp, br=br, gW=gWp, gW_ld=Cp,
-                     dx16=dao.data_ptr(), lddx=Cp, flops_k=Cc, bias_done=fused)
-    if padded:
-        self._op(ops, "fvit_unpad_heads_f32", gWp, Cp, self.G(attn.proj.weight), Cc, Cc, Cp, hd, hdp, 0, 1, None)
-        self._bwd_side.add(len(ops) - 1)   # fresh scratch in, parameter gradient out: leaf launch
-    _emit_attn_core_bwd(self, at, dao, dqkv, B, n_ct)
-    _bias_bwd(self, at["bias"])
-    one = dict(gamma=None, s=None, inv_s=("scal", 2), w_alpha=("scal", 1))
-    gWq, gbq = self.G(attn.qkv.weight), (self.G(attn.qkv.bias) if attn.qkv.bias is not None else None)
-    if padded:
-        gbq = ("scr", self._scratch("dbqkv_pad_c", 3 * Cp))
-    self._linear_bwd(lin=attn.qkv, w16=at["wq"].data_ptr(), ldw=at["ldq"], x16=at["y16"].data_ptr(), ldx=Cc,
-                     dz16=dqkv.data_ptr(), lddz=3 * Cp, rows=rows_c, n_out=3 * Cp, k_in=Cc, br=one, gW=gWq, gW_ld=Cc,
-                     gW_row_map=_unpad_row_map(self, 3 * h, hd, hdp) if padded else None,
-                     bias_to=gbq, dx16=dy.data_ptr(), lddx=Cc)
-    if padded:
-        if attn.qkv.bias is not None:
-            self._op(ops, "fvit_unpad_heads_f32", gbq, 1, self.G(attn.qkv.bias), 1, 3 * Cp, 1, hd, hdp, 1, 0, None)
-            self._bwd_side.add(len(ops) - 1)   # fresh scratch in, parameter gradient out: leaf launch
-    # hat_norm1: rows r of the raster buffer = level rows ctr0 + r; gradient at (ct + hat_pe) first
-    # accumulated in place (identity map), summed over images for hat_pos_embed, then moved to the
-    # xs carrier rows it was gathered from
-    ln = blk.hat_norm1
-    self._op(ops, "fvit_ln_bwd", dy.data_ptr(), Cc, None, c["xh1"].data_ptr(), Cc, c["rs1"].data_ptr(),
-             ln.weight.data_ptr(), rows_c, Cc, gc_ptr, Cc, None, 1, 0, ("scal", 1), self.G(ln.weight), self.G(ln.bias))
-    if sv["hat_pe"] is not None:
-        self._op(ops, "fvit_group_sum", gc_ptr, Cc, B, n_ct, 0, Cc, ("scal", 1), sv["hat_pe"]["dout"])
-        _posemb_bwd(self, sv["hat_pe"])
-    self._op(ops, "fvit_scatter_add_rows", gc_ptr, Cc, g_ptr, Cc, tl["ct_gather"].data_ptr(), rows_c, Cc)
-
-
 class TokenLevelEmitters:
     """TrainPlan mixin: launch-list emitters of the transformer levels, the head and the build drivers (the functions
     above take the plan as `self`; `_attn_bwd_entry` is a plain helper)."""
@@ -920,7 +748,6 @@ class TokenLevelEmitters:
     _posemb_train = _posemb_train
     _bias_train = _bias_train
     _attn_fwd_train = _attn_fwd_train
-    _gemm_train_branch = _gemm_train_branch
     _emit_token_level_train = _emit_token_level_train
     _mlp_fwd_train = _mlp_fwd_train
     _emit_head_train = _emit_head_train
@@ -936,4 +763,3 @@ class TokenLevelEmitters:
     _attn_bwd = _attn_bwd
     _unpad_row_map = _unpad_row_map
     _emit_token_level_bwd = _emit_token_level_bwd
-    _attn_bwd_carrier = _attn_bwd_carrier
