@@ -701,7 +701,9 @@ cpb_mlp_wide_kernel(const float* __restrict__ coords, int P, const float* __rest
 }
 
 // bias[h][r][c] = (r >= ng && c >= ng) ? 16*sigmoid(table[index[(r-ng)*L + (c-ng)]][h]) : 0
-// with L = ws*ws local tokens and ng = S - L carrier tokens on the top/left (fv.py:276-299).
+// with L = ws*ws local tokens and ng = S - L carrier tokens on the top/left (fv.py:276-299). A negative ng (S < L:
+// the detection backbone's carrier attention on a grid smaller than the built one) crops the table's top-left instead,
+// as F.pad with negative padding does; r, c >= ng then always holds and r - ng < L.
 __global__ void attn_bias_kernel(const float* __restrict__ table, const long long* __restrict__ index,
                                  int heads, int S, int L, float* __restrict__ bias) {
   const int ng = S - L;
@@ -722,6 +724,10 @@ __global__ void attn_bias_kernel(const float* __restrict__ table, const long lon
 // TokenInitializer (fv.py:733-738): ct = AvgPool_{kh x kw, stride sh x sw}(dwconv3x3(x) + b), written
 // to the carrier rows of the window-major token buffer. x is read through `pix_map` (pixel (b,h,w) of
 // the (padded) Hp x Wp map -> row of xs, or -1 for padding pixels which read as zero).
+// kNchwTokens (detection backbone, dino/models/dino/fastervit.py:591): the pooled NCHW map of image b is read back as
+// [oh*ow, C] tokens without a permute, so value (c, p) lands in token t, channel k with c*oh*ow + p = t*C + k, stored
+// to row ct_row_map[b*oh*ow + t]; otherwise value (c, p) is channel c of row ct_row_map[b*oh*ow + p].
+template <bool kNchwTokens>
 __global__ void token_init_kernel(const float* __restrict__ xs, long long ldx,
                                   const int* __restrict__ pix_map, int B, int Hp, int Wp, int C,
                                   const float* __restrict__ w, const float* __restrict__ bias, int kh,
@@ -753,7 +759,13 @@ __global__ void token_init_kernel(const float* __restrict__ xs, long long ldx,
           }
       }
     const float v = acc / (float)(kh * kw) + bias[c];
-    out[(long long)ct_row_map[pos] * ldo + c] = v;
+    if (kNchwTokens) {
+      const long long hw = (long long)oh * ow;
+      const long long f = (long long)c * hw + (pos - (long long)b * hw);
+      out[(long long)ct_row_map[(long long)b * hw + f / C] * ldo + f % C] = v;
+    } else {
+      out[(long long)ct_row_map[pos] * ldo + c] = v;
+    }
   }
 }
 
@@ -1068,7 +1080,7 @@ int fvit_cpb_mlp_fwd(const float* coords, int32_t P, const float* w0, const floa
 
 int fvit_attn_bias_fwd(const float* table, const int64_t* index, int32_t heads, int32_t S, int32_t L,
                        float* bias, void* stream) {
-  FVIT_CHECK(table && index && bias && heads > 0 && S >= L && L > 0, "fvit_attn_bias_fwd: bad arguments");
+  FVIT_CHECK(table && index && bias && heads > 0 && S > 0 && L > 0, "fvit_attn_bias_fwd: bad arguments");
   const long long total = (long long)heads * S * S;
   attn_bias_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
       table, (const long long*)index, heads, S, L, bias);
@@ -1082,9 +1094,22 @@ int fvit_token_init_fwd(const float* xs, int64_t ldx, const int32_t* pix_map, in
   FVIT_CHECK(xs && pix_map && w && bias && ct_row_map && out, "fvit_token_init_fwd: null argument");
   FVIT_CHECK((oh - 1) * sh + kh <= Hp && (ow - 1) * sw + kw <= Wp, "fvit_token_init_fwd: pool window out of range");
   const long long total = (long long)B * oh * ow * C;
-  token_init_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
+  token_init_kernel<false><<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
       xs, ldx, pix_map, B, Hp, Wp, C, w, bias, kh, kw, sh, sw, oh, ow, ct_row_map, out, ldo);
   return post_launch("token_init_kernel");
+}
+
+int fvit_token_init_nchw_fwd(const float* xs, int64_t ldx, const int32_t* pix_map, int32_t B, int32_t Hp,
+                             int32_t Wp, int32_t C, const float* w, const float* bias, int32_t kh, int32_t kw,
+                             int32_t sh, int32_t sw, int32_t oh, int32_t ow, const int32_t* ct_row_map,
+                             float* out, int64_t ldo, void* stream) {
+  FVIT_CHECK(xs && pix_map && w && bias && ct_row_map && out && B > 0 && C > 0 && oh > 0 && ow > 0,
+             "fvit_token_init_nchw_fwd: bad arguments");
+  FVIT_CHECK((oh - 1) * sh + kh <= Hp && (ow - 1) * sw + kw <= Wp, "fvit_token_init_nchw_fwd: pool window out of range");
+  const long long total = (long long)B * oh * ow * C;
+  token_init_kernel<true><<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
+      xs, ldx, pix_map, B, Hp, Wp, C, w, bias, kh, kw, sh, sw, oh, ow, ct_row_map, out, ldo);
+  return post_launch("token_init_nchw_kernel");
 }
 
 int fvit_propagate_fwd(float* xs, int64_t ldx, const int32_t* src_map, int32_t rows, int32_t C,

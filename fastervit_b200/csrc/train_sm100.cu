@@ -740,7 +740,7 @@ __global__ void unpad_heads_kernel(const float* __restrict__ src, long long lds,
 }
 
 // d table[idx][h] += *scalar * dbias[h][r][c] * b (1 - b/16) with b = bias[h][r][c] = 16 sigmoid(table[idx][h])
-// for r, c >= ng (backward of fvit_attn_bias_fwd; fv.py:276-299)
+// for r, c >= ng (backward of fvit_attn_bias_fwd; fv.py:276-299); a negative ng (S < L) skips the cropped entries
 __global__ void attn_bias_bwd_kernel(const float* __restrict__ dbias, const float* __restrict__ bias,
                                      const long long* __restrict__ index, int heads, int S, int L,
                                      const float* __restrict__ scalar, float* __restrict__ dtable) {
@@ -750,6 +750,7 @@ __global__ void attn_bias_bwd_kernel(const float* __restrict__ dbias, const floa
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
     const int c = (int)(i % L), r = (int)((i / L) % L), h = (int)(i / ((long long)L * L));
+    if (r + ng < 0 || c + ng < 0) continue;   // S < L: the forward cropped this part of the table away
     const long long off = ((long long)h * S + r + ng) * S + c + ng;
     const float b = bias[off];
     const float dz = dbias[off] * b * (1.f - b * (1.f / 16.f)) * sc;
@@ -1330,9 +1331,23 @@ __global__ void unpack_conv_grad_kernel(const float* __restrict__ src, int ld, f
   }
 }
 
+// Element of the carrier gradient that belongs to pooled value (b, c, o = y0*ow + x0): channel c of row
+// ct_row_map[b*nout + o], or -- kNchwTokens, the detection backbone's NCHW read-back (fvit_token_init_nchw_fwd) --
+// channel f % C of row ct_row_map[b*nout + f / C] with f = c*nout + o.
+template <bool kNchwTokens>
+__device__ __forceinline__ long long ct_grad_at(const int* __restrict__ ct_row_map, int b, int o, int nout, int c, int C,
+                                                long long ldg) {
+  if (kNchwTokens) {
+    const long long f = (long long)c * nout + o;
+    return (long long)ct_row_map[(long long)b * nout + f / C] * ldg + f % C;
+  }
+  return (long long)ct_row_map[(long long)b * nout + o] * ldg + c;
+}
+
 // TokenInitializer backward: for ct[b, (y0,x0), c] = bias + mean_{pool window} dwconv3x3(x):
 //   dx[pixel] += sum over pooled outputs / taps ; dw[c][tap] += ... ; dbias[c] += sum gct. One thread per
 //   (b, pixel, channel) gathers from the (at most few) pooled outputs that cover the pixel's 3x3 halo.
+template <bool kNchwTokens>
 __global__ void token_init_bwd_kernel(const float* __restrict__ g, long long ldg, const int* __restrict__ pix_map,
                                       const int* __restrict__ ct_row_map, int B, int Hp, int Wp, int C,
                                       const float* __restrict__ w, int kh, int kw, int sh, int sw, int oh, int ow,
@@ -1359,8 +1374,7 @@ __global__ void token_init_bwd_kernel(const float* __restrict__ g, long long ldg
         const int x0lo = cx - kw + sw >= 0 ? (cx - kw + sw) / sw : 0, x0hi = min(ow - 1, cx / sw);
         for (int y0 = y0lo; y0 <= y0hi; ++y0)
           for (int x0 = x0lo; x0 <= x0hi; ++x0) {
-            const int crow = ct_row_map[((long long)b * oh + y0) * ow + x0];
-            acc = fmaf(wt, g[(long long)crow * ldg + c], acc);
+            acc = fmaf(wt, g[ct_grad_at<kNchwTokens>(ct_row_map, b, y0 * ow + x0, oh * ow, c, C, ldg)], acc);
           }
       }
     gx[(long long)row * ldgx + c] += acc;
@@ -1370,6 +1384,7 @@ __global__ void token_init_bwd_kernel(const float* __restrict__ g, long long ldg
 // per (image, 32 channels) stages the carrier gradients, forms the average-pool backward d conv[pixel] once
 // (instead of once per tap: 36 gathers per element in the kernel above) and applies the 9-tap transpose of the
 // depthwise convolution out of shared memory. Thread = (channel lane, pixel lane): 128-byte row accesses.
+template <bool kNchwTokens>
 __global__ void __launch_bounds__(256)
 token_init_bwd_tile_kernel(const float* __restrict__ g, long long ldg, const int* __restrict__ pix_map,
                            const int* __restrict__ ct_row_map, int Hp, int Wp, int C, const float* __restrict__ w,
@@ -1382,7 +1397,7 @@ token_init_bwd_tile_kernel(const float* __restrict__ g, long long ldg, const int
   const bool cok = c < C;
   const int nout = oh * ow, npix = Hp * Wp;
   for (int o = pl; o < nout; o += 8)
-    sg[o * 32 + cl] = cok ? g[(long long)ct_row_map[b * nout + o] * ldg + c] : 0.f;
+    sg[o * 32 + cl] = cok ? g[ct_grad_at<kNchwTokens>(ct_row_map, b, o, nout, c, C, ldg)] : 0.f;
   __syncthreads();
   const float inv = 1.f / (float)(kh * kw);
   for (int p = pl; p < npix; p += 8) {
@@ -1420,6 +1435,7 @@ token_init_bwd_tile_kernel(const float* __restrict__ g, long long ldg, const int
   }
 }
 // dw[c][tap] += sc * sum_{b,y0,x0} gct * mean_pool x[.. + tap - 1] ; dbias[c] += sc * sum gct
+template <bool kNchwTokens>
 __global__ void token_init_wgrad_kernel(const float* __restrict__ g, long long ldg, const __half* __restrict__ xs,
                                         long long ldx, const int* __restrict__ pix_map,
                                         const int* __restrict__ ct_row_map, int B, int Hp, int Wp, int C, int kh,
@@ -1434,7 +1450,7 @@ __global__ void token_init_wgrad_kernel(const float* __restrict__ g, long long l
   if (c < C) {
     for (long long pos = blockIdx.y * 4 + lane_p; pos < (long long)B * oh * ow; pos += gridDim.y * 4) {
       const int x0 = (int)(pos % ow), y0 = (int)((pos / ow) % oh), b = (int)(pos / ((long long)ow * oh));
-      const float gv = g[(long long)ct_row_map[pos] * ldg + c];
+      const float gv = g[ct_grad_at<kNchwTokens>(ct_row_map, b, y0 * ow + x0, oh * ow, c, C, ldg)];
       ab += gv;
       // dw[tap] += gv/(kh kw) * sum over the pool window of x[conv pixel + tap - 1]: walk the (kh+2) x (kw+2) input
       // patch once and add each pixel to the (up to 9) taps that see it
@@ -1785,7 +1801,7 @@ int fvit_unpad_heads_f32(const float* src, int64_t lds, float* dst, int64_t ldd,
 
 int fvit_attn_bias_bwd(const float* dbias, const float* bias, const int64_t* index, int32_t heads, int32_t S,
                        int32_t L, const float* scalar, float* dtable, void* stream) {
-  FVIT_CHECK(dbias && bias && index && dtable && heads > 0 && S >= L && L > 0, "fvit_attn_bias_bwd: bad arguments");
+  FVIT_CHECK(dbias && bias && index && dtable && heads > 0 && S > 0 && L > 0, "fvit_attn_bias_bwd: bad arguments");
   const long long total = (long long)heads * L * L;
   attn_bias_bwd_kernel<<<grid_cap(total, 256, 8), 256, 0, (cudaStream_t)stream>>>(
       dbias, bias, (const long long*)index, heads, S, L, scalar, dtable);
@@ -1936,44 +1952,77 @@ int fvit_unpack_conv_grad(const float* src, int32_t ld_ci, float* dst, int32_t c
   return post_launch("unpack_conv_grad_kernel");
 }
 
+}  // extern "C" (the launch templates below have C++ linkage)
+
 // the input-gradient kernels of the TokenInitializer backward (fvit_token_init_bwd, fvit_token_init_dgrad)
+template <bool kNchwTokens>
 static int token_init_dx_launch(const float* g, int64_t ldg, const int32_t* pix_map, const int32_t* ct_row_map, int32_t B,
                                 int32_t Hp, int32_t Wp, int32_t C, const float* w, int32_t kh, int32_t kw, int32_t sh,
                                 int32_t sw, int32_t oh, int32_t ow, float* gx, int64_t ldgx, void* stream) {
   const size_t tile_smem = ((size_t)oh * ow + (size_t)Hp * Wp) * 32 * sizeof(float);
   if (tile_smem <= 48 * 1024 && B <= 65535) {  // the whole map of one image fits: pool backward formed once per pixel
     dim3 gt((unsigned)((C + 31) / 32), (unsigned)B);
-    token_init_bwd_tile_kernel<<<gt, 256, tile_smem, (cudaStream_t)stream>>>(g, ldg, pix_map, ct_row_map, Hp, Wp, C, w, kh,
+    token_init_bwd_tile_kernel<kNchwTokens><<<gt, 256, tile_smem, (cudaStream_t)stream>>>(g, ldg, pix_map, ct_row_map, Hp, Wp, C, w, kh,
                                                                              kw, sh, sw, oh, ow, gx, ldgx);
     return post_launch("token_init_bwd_tile_kernel");
   }
   const int cb = C >= 256 ? 256 : (C >= 128 ? 128 : 64);
   const long long npos = (long long)B * Hp * Wp;
   dim3 gd((unsigned)((C + cb - 1) / cb), (unsigned)(npos < 65535 ? npos : 65535));
-  token_init_bwd_kernel<<<gd, cb, 0, (cudaStream_t)stream>>>(g, ldg, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw,
+  token_init_bwd_kernel<kNchwTokens><<<gd, cb, 0, (cudaStream_t)stream>>>(g, ldg, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw,
                                                              oh, ow, gx, ldgx);
   return post_launch("token_init_bwd_kernel");
 }
+
+template <bool kNchwTokens>
+static int token_init_bwd_launch(const float* g, int64_t ldg, const void* x16, int64_t ldx, const int32_t* pix_map,
+                                 const int32_t* ct_row_map, int32_t B, int32_t Hp, int32_t Wp, int32_t C, const float* w,
+                                 int32_t kh, int32_t kw, int32_t sh, int32_t sw, int32_t oh, int32_t ow, const float* scalar,
+                                 float* gx, int64_t ldgx, float* dw, float* dbias, void* stream) {
+  FVIT_CHECK(g && x16 && pix_map && ct_row_map && w && gx && dw && dbias, "fvit_token_init_bwd: null argument");
+  const int npos4 = (B * oh * ow + 3) / 4;
+  dim3 gw((unsigned)((C + 127) / 128), (unsigned)(npos4 < 512 ? npos4 : 512));
+  token_init_wgrad_kernel<kNchwTokens><<<gw, 512, 0, (cudaStream_t)stream>>>(g, ldg, (const __half*)x16, ldx, pix_map,
+                                                                             ct_row_map, B, Hp, Wp, C, kh, kw, sh, sw, oh,
+                                                                             ow, scalar, dw, dbias);
+  int rc = post_launch("token_init_wgrad_kernel");
+  if (rc) return rc;
+  return token_init_dx_launch<kNchwTokens>(g, ldg, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw, oh, ow, gx, ldgx,
+                                           stream);
+}
+
+extern "C" {
 
 int fvit_token_init_bwd(const float* g, int64_t ldg, const void* x16, int64_t ldx, const int32_t* pix_map,
                         const int32_t* ct_row_map, int32_t B, int32_t Hp, int32_t Wp, int32_t C, const float* w,
                         int32_t kh, int32_t kw, int32_t sh, int32_t sw, int32_t oh, int32_t ow, const float* scalar,
                         float* gx, int64_t ldgx, float* dw, float* dbias, void* stream) {
-  FVIT_CHECK(g && x16 && pix_map && ct_row_map && w && gx && dw && dbias, "fvit_token_init_bwd: null argument");
-  const int npos4 = (B * oh * ow + 3) / 4;
-  dim3 gw((unsigned)((C + 127) / 128), (unsigned)(npos4 < 512 ? npos4 : 512));
-  token_init_wgrad_kernel<<<gw, 512, 0, (cudaStream_t)stream>>>(g, ldg, (const __half*)x16, ldx, pix_map, ct_row_map, B, Hp, Wp, C, kh, kw,
-                                                                sh, sw, oh, ow, scalar, dw, dbias);
-  int rc = post_launch("token_init_wgrad_kernel");
-  if (rc) return rc;
-  return token_init_dx_launch(g, ldg, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw, oh, ow, gx, ldgx, stream);
+  return token_init_bwd_launch<false>(g, ldg, x16, ldx, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw, oh, ow,
+                                      scalar, gx, ldgx, dw, dbias, stream);
+}
+
+int fvit_token_init_nchw_bwd(const float* g, int64_t ldg, const void* x16, int64_t ldx, const int32_t* pix_map,
+                             const int32_t* ct_row_map, int32_t B, int32_t Hp, int32_t Wp, int32_t C, const float* w,
+                             int32_t kh, int32_t kw, int32_t sh, int32_t sw, int32_t oh, int32_t ow, const float* scalar,
+                             float* gx, int64_t ldgx, float* dw, float* dbias, void* stream) {
+  return token_init_bwd_launch<true>(g, ldg, x16, ldx, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw, oh, ow,
+                                     scalar, gx, ldgx, dw, dbias, stream);
 }
 
 int fvit_token_init_dgrad(const float* g, int64_t ldg, const int32_t* pix_map, const int32_t* ct_row_map, int32_t B,
                           int32_t Hp, int32_t Wp, int32_t C, const float* w, int32_t kh, int32_t kw, int32_t sh,
                           int32_t sw, int32_t oh, int32_t ow, float* gx, int64_t ldgx, void* stream) {
   FVIT_CHECK(g && pix_map && ct_row_map && w && gx && B > 0 && C > 0, "fvit_token_init_dgrad: bad arguments");
-  return token_init_dx_launch(g, ldg, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw, oh, ow, gx, ldgx, stream);
+  return token_init_dx_launch<false>(g, ldg, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw, oh, ow, gx, ldgx,
+                                     stream);
+}
+
+int fvit_token_init_nchw_dgrad(const float* g, int64_t ldg, const int32_t* pix_map, const int32_t* ct_row_map, int32_t B,
+                               int32_t Hp, int32_t Wp, int32_t C, const float* w, int32_t kh, int32_t kw, int32_t sh,
+                               int32_t sw, int32_t oh, int32_t ow, float* gx, int64_t ldgx, void* stream) {
+  FVIT_CHECK(g && pix_map && ct_row_map && w && gx && B > 0 && C > 0, "fvit_token_init_nchw_dgrad: bad arguments");
+  return token_init_dx_launch<true>(g, ldg, pix_map, ct_row_map, B, Hp, Wp, C, w, kh, kw, sh, sw, oh, ow, gx, ldgx,
+                                    stream);
 }
 
 int fvit_propagate_bwd(float* g, int64_t ldg, const float* xs, int64_t ldx, const int32_t* src_map, int32_t rows, int32_t C,

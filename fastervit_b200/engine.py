@@ -53,6 +53,71 @@ def _ct_window_perm(cs: int, sr: list[int]) -> torch.Tensor:
     return idx.permute(0, 1, 3, 2, 4, 5).reshape(Wd * Hd)
 
 
+def grid_coords(h: int, w: int, norm: int) -> torch.Tensor:
+    """[h*w, 2] inputs of a rank-2 positional MLP (PosEmbMLPSwinv1D, fv.py:355-365): the 'ij' grid arange(h) x arange(w),
+    shifted and divided by `norm`"""
+    r, c = torch.arange(h, dtype=torch.float32), torch.arange(w, dtype=torch.float32)
+    grid = torch.stack(torch.meshgrid(r, c, indexing="ij"))
+    return ((grid - norm) / norm).flatten(1).t().contiguous()
+
+
+def conv_level_pad(model, i: int, Hc: int, Wc: int) -> tuple[int, int]:
+    """(Hb, Wb): the map a convolutional level runs on. The detection backbone pads every level, the convolutional ones
+    included, to a multiple of its window and crops after (dino/models/dino/fastervit.py:686-707); classification
+    models run conv levels on the map as it is."""
+    if not getattr(model, "carriers_from_input", False):
+        return Hc, Wc
+    ws = model.levels[i].window_size
+    return _ru(Hc, ws), _ru(Wc, ws)
+
+
+def token_geometry(model, i: int, Hc: int, Wc: int) -> dict:
+    """Window and carrier geometry of transformer level i for an Hc x Wc input map: the one function that decides it for
+    the inference and the training plans.
+      Hp, Wp, nwh, nww   the map padded to the window, and its window grid
+      has_ct, sr         carrier tokens present; the carrier window grid the ct_dewindow / ct_window maps follow
+      pool               ((kh, sh, oh), (kw, sw, ow)) of the tokenizer's average pool
+      tokens             "map": tokenizer output (b, y, x) is carrier (y, x) of the grid (fv.py:733-738);
+                         "nchw": the pooled NCHW map is read back as [oh*ow, C] tokens (fvit_token_init_nchw_fwd)
+      pe_coords, hat_pe_coords   inputs of the window-token / carrier positional MLPs (None: no such MLP)
+      own_tables         positional tables / biases are plan buffers, not the modules' `relative_bias`
+    Classification models: the carrier grid is the sr_ratio fixed at construction (another window grid raises), the pool
+    is TokenInitializer.pool and the positional grids are scaled by side // 2 (fv.py:355-360). The detection backbone
+    (model.carriers_from_input, fastervit_b200.detection): everything follows the input -- carrier grid cs*nwh x cs*nww,
+    pool from the padded map (dino/models/dino/fastervit.py:569-592), grids scaled by (h*w) // 2 (fastervit.py:192-196)."""
+    level = model.levels[i]
+    ws, cs = level.window_size, model.cfg["ct_size"]
+    det = bool(getattr(model, "carriers_from_input", False))
+    Hp, Wp = _ru(Hc, ws), _ru(Wc, ws)
+    if not (model.any_res or det) and (Hp != Hc or Wp != Wc):
+        raise L.FvitError(f"level {i}: {Hc}x{Wc} map is not a multiple of window {ws} "
+                          "(use a *_any_res model for such resolutions)")
+    nwh, nww = Hp // ws, Wp // ws
+    has_ct = len(level.blocks) > 0 and level.blocks[0].has_carriers
+    g = dict(Hp=Hp, Wp=Wp, nwh=nwh, nww=nww, has_ct=has_ct, sr=None, pool=None, tokens="map", hat_pe_coords=None,
+             pe_coords=grid_coords(ws, ws, (ws * ws) // 2 if det else ws // 2), own_tables=det)
+    if not has_ct:
+        return g
+    if det:
+        pool = []
+        for r in (Hp, Wp):
+            out = int(cs * r / ws)
+            stride = int(r / out)
+            pool.append((r - (out - 1) * stride, stride, out))
+        hg, wg = pool[0][2], pool[1][2]
+        if (hg, wg) != (cs * nwh, cs * nww):
+            raise L.FvitError(f"level {i}: carrier grid {hg}x{wg} does not tile the {nwh}x{nww} windows")
+        g.update(sr=[nwh, nww], pool=pool, tokens="nchw", hat_pe_coords=grid_coords(hg, wg, (hg * wg) // 2))
+        return g
+    sr = list(level.sr_ratio)
+    if sr != [nwh, nww]:
+        raise L.FvitError(f"level {i}: input gives {nwh}x{nww} windows but the model was built for {sr}")
+    n = int((cs * cs * sr[0] * sr[1]) ** 0.5)
+    g.update(sr=sr, pool=level.global_tokenizer.pool if level.do_gt else None,
+             hat_pe_coords=grid_coords(n, n, n // 2) if hasattr(level.blocks[0], "hat_pos_embed") else None)
+    return g
+
+
 class _Bufs:
     """Device buffer factory: zero-initialised persistent tensors, named for debugging."""
 
@@ -143,7 +208,7 @@ class Plan:
         B = self.B
         if where["kind"] == "conv":      # zero-bordered NHWC fp32 map
             lv = where["lv"]
-            t = lv["x32"].view(B, lv["H"] + 2, lv["W"] + 2, lv["C"])[:, 1:-1, 1:-1]
+            t = lv["x32"].view(B, lv["Hb"] + 2, lv["Wb"] + 2, lv["C"])[:, 1:lv["H"] + 1, 1:lv["W"] + 1]
             return t.permute(0, 3, 1, 2).clone()
         tl = where["tl"]
         if where["kind"] == "tok_map":   # window-major token buffer read through the (cropped) pixel map
@@ -280,12 +345,13 @@ class Plan:
                    flops=2.0 * B * H1 * W1 * in_dim * k1)
 
         lvl = self._conv_level_buffers(0, dim, H0, W0)
+        self._zero_window_padding(lvl)
         w16, ldw = self._pack_conv("stem.conv2", pe[3])
         s2, t2 = self._fold("stem.bn2", dim, pe[4])
         self._gemm(a=stem_planes.data_ptr(), a_rows=pl_rows, lda=ld_in, a_planes=4,
                    a_plane_stride=pl_rows * ld_in, b=w16.data_ptr(), ldb=ldw, m=pl_rows, n=dim, kc=in_dim,
                    taps=self._s2_taps(W0), col_scale=s2.data_ptr(), col_shift=t2.data_ptr(), act=L.ACT_RELU,
-                   m_alg=lvl["npix"], row_map=self._plane_to_padded_map("stem.to_l0", B, H0, W0).data_ptr(),
+                   m_alg=lvl["npix"], row_map=self._plane_to_padded_map("stem.to_l0", B, H0, W0, lvl["Hb"], lvl["Wb"]).data_ptr(),
                    out_f32=lvl["x32"].data_ptr(), ld_o32=lvl["C"], out_f16=lvl["x16"].data_ptr(),
                    ld_o16=lvl["ld"])
 
@@ -296,6 +362,7 @@ class Plan:
             if level.conv:
                 if i > 0:
                     lvl = self._conv_level_buffers(i, Cc, Hc, Wc)
+                    self._zero_window_padding(lvl)
                     self._emit_downsample_conv(i - 1, prev, lvl, to_conv=True)
                     self._mark(f"levels.{i - 1}", kind="conv", lv=lvl)
                 self._emit_conv_blocks(i, level, lvl)
@@ -317,8 +384,11 @@ class Plan:
                     self._mark(f"levels.{i}", kind="tok_map", tl=tl)
             if level.downsample is not None:
                 Hc, Wc, Cc = (Hc + 1) // 2, (Wc + 1) // 2, Cc * 2
-        # ---------------- head: BN folded into the average pool, then the classifier GEMM
         self.feat = prev
+        if getattr(m, "norm", None) is None:   # the detection backbone: level maps only, no classifier tail
+            self.pooled = self.logits = None
+            return
+        # ---------------- head: BN folded into the average pool, then the classifier GEMM
         nf = m.num_features
         sN, tN = self._fold("norm", nf, m.norm)
         T = prev["H"] * prev["W"]
@@ -366,10 +436,13 @@ class Plan:
         return self.bufs.i32(name, (((yi & 1) * 2 + (xi & 1)) * pl_rows + bi * (Ho + 1) * (Wo + 1)
                                     + ((yi >> 1) + 1) * (Wo + 1) + (xi >> 1) + 1).reshape(-1))
 
-    def _plane_to_padded_map(self, name: str, B: int, Ho: int, Wo: int) -> torch.Tensor:
-        """plane-space output row (b, a+1, c+1) -> zero-bordered level row; border rows -> -1."""
+    def _plane_to_padded_map(self, name: str, B: int, Ho: int, Wo: int, Hb: int | None = None,
+                             Wb: int | None = None) -> torch.Tensor:
+        """plane-space output row (b, a+1, c+1) -> zero-bordered level row of an (Hb, Wb) map (default (Ho, Wo); larger
+        when the level runs on a window-padded map, conv_level_pad); border rows -> -1."""
+        Hb, Wb = Hb or Ho, Wb or Wo
         bi, ai, ci = torch.meshgrid(torch.arange(B), torch.arange(Ho + 1), torch.arange(Wo + 1), indexing="ij")
-        dst = bi * (Ho + 2) * (Wo + 2) + ai * (Wo + 2) + ci  # (a-1)+1 = a
+        dst = bi * (Hb + 2) * (Wb + 2) + ai * (Wb + 2) + ci  # (a-1)+1 = a
         dst = torch.where((ai >= 1) & (ci >= 1), dst, torch.full_like(dst, -1))
         return self.bufs.i32(name, dst.reshape(-1))
 
@@ -377,31 +450,43 @@ class Plan:
         """plane-space output row (b, a+1, c+1) of Downsample i -> the row of pixel (a, c) in the next level: its
         zero-bordered conv map, or its window-major token buffer (dst["pix_map_host"]); border rows -> -1."""
         if "pix_map_host" not in dst:
-            return self._plane_to_padded_map(f"ds{i}.rmap", self.B, Ho, Wo)
+            return self._plane_to_padded_map(f"ds{i}.rmap", self.B, Ho, Wo, dst["Hb"], dst["Wb"])
         full = torch.full((self.B, Ho + 1, Wo + 1), -1, dtype=torch.int64)
         full[:, 1:, 1:] = dst["pix_map_host"][:, :Ho, :Wo]
         return self.bufs.i32(f"ds{i}.rmap", full.reshape(-1))
 
     def _conv_level_buffers(self, i: int, Cc: int, Hc: int, Wc: int, f16=("x16", "h16")) -> dict:
         """geometry, row maps and buffers of a conv level's zero-bordered map: the fp32 residual stream x32 and one
-        [rows, ld] fp16 matrix per name in f16"""
+        [rows, ld] fp16 matrix per name in f16. The map is Hb x Wb (conv_level_pad): the blocks compute every pixel of
+        it, the Hc x Wc top-left part (pix) is the level's input and output."""
         B, nb = self.B, self.bufs
-        rows = B * (Hc + 2) * (Wc + 2)
+        Hb, Wb = conv_level_pad(self.model, i, Hc, Wc)
+        rows = B * (Hb + 2) * (Wb + 2)
         ld = _ru(Cc, 8)
-        bi, yi, xi = torch.meshgrid(torch.arange(B), torch.arange(Hc + 2), torch.arange(Wc + 2), indexing="ij")
-        inside = (yi >= 1) & (yi <= Hc) & (xi >= 1) & (xi <= Wc)
-        ident = torch.arange(rows).view(B, Hc + 2, Wc + 2)
+        bi, yi, xi = torch.meshgrid(torch.arange(B), torch.arange(Hb + 2), torch.arange(Wb + 2), indexing="ij")
+        inside = (yi >= 1) & (yi <= Hb) & (xi >= 1) & (xi <= Wb)
+        ident = torch.arange(rows).view(B, Hb + 2, Wb + 2)
         interior = nb.i32(f"l{i}.interior", torch.where(inside, ident, torch.full_like(ident, -1)).reshape(-1))
-        pix = nb.i32(f"l{i}.pix", ident[:, 1:-1, 1:-1].reshape(-1))  # pixel (b,y,x) -> padded row
-        d = dict(C=Cc, H=Hc, W=Wc, ld=ld, rows=rows, npix=B * Hc * Wc, interior=interior, pix=pix,
+        pix = nb.i32(f"l{i}.pix", ident[:, 1:Hc + 1, 1:Wc + 1].reshape(-1))  # pixel (b,y,x) -> padded row
+        # the pixels the blocks compute (their BatchNorms' statistics included): the whole Hb x Wb map
+        cpix = pix if (Hb, Wb) == (Hc, Wc) else nb.i32(f"l{i}.cpix", ident[:, 1:-1, 1:-1].reshape(-1))
+        d = dict(C=Cc, H=Hc, W=Wc, Hb=Hb, Wb=Wb, ld=ld, rows=rows, npix=B * Hc * Wc, interior=interior, pix=pix,
+                 cpix=cpix, cnpix=B * Hb * Wb,
                  x32=nb.new(f"l{i}.x32", (rows, Cc), torch.float32))
         for k in f16:
             d[k] = nb.new(f"l{i}.{k}", (rows, ld), torch.float16)
         return d
 
+    def _zero_window_padding(self, lv: dict) -> None:
+        """A conv level on a window-padded map (conv_level_pad) enters with zeros there (F.pad, dino/models/dino/
+        fastervit.py:690-691), which the blocks then overwrite: re-zeroed every forward before the map is written."""
+        if (lv["Hb"], lv["Wb"]) != (lv["H"], lv["W"]):
+            for t in (lv["x32"], lv["x16s"][0] if "x16s" in lv else lv["x16"]):   # (train plans: the first block's operand)
+                self.ops.append(("zero", t, "memset"))
+
     # ---- conv levels ------------------------------------------------------------------------------
     def _emit_conv_blocks(self, i: int, level, lv: dict) -> None:
-        Cc, Wp = lv["C"], lv["W"] + 2
+        Cc, Wp = lv["C"], lv["Wb"] + 2
         taps = [((dy - 1) * Wp + (dx - 1), 0) for dy in range(3) for dx in range(3)]
         for j, blk in enumerate(level.blocks):
             nm = f"l{i}.b{j}"
@@ -451,15 +536,8 @@ class Plan:
     def _token_level_buffers(self, i: int, level, Cc: int, Hc: int, Wc: int) -> dict:
         B, nb = self.B, self.bufs
         ws, cs = level.window_size, self.model.cfg["ct_size"]
-        Hp, Wp = _ru(Hc, ws), _ru(Wc, ws)
-        if not self.model.any_res and (Hp != Hc or Wp != Wc):
-            raise L.FvitError(f"level {i}: {Hc}x{Wc} map is not a multiple of window {ws} "
-                              "(use a *_any_res model for such resolutions)")
-        nwh, nww = Hp // ws, Wp // ws
-        has_ct = len(level.blocks) > 0 and level.blocks[0].has_carriers
-        sr = level.sr_ratio
-        if has_ct and (sr[0] != nwh or sr[1] != nww):
-            raise L.FvitError(f"level {i}: input gives {nwh}x{nww} windows but the model was built for {sr}")
+        geo = token_geometry(self.model, i, Hc, Wc)
+        Hp, Wp, nwh, nww, has_ct, sr = geo["Hp"], geo["Wp"], geo["nwh"], geo["nww"], geo["has_ct"], geo["sr"]
         ncw = cs * cs if has_ct else 0
         S = ncw + ws * ws
         nwin = nwh * nww
@@ -473,7 +551,8 @@ class Plan:
         win = (bi * nwh + yi // ws) * nww + xi // ws
         pix_map = win * S + ncw + (yi % ws) * ws + (xi % ws)          # [B, Hp, Wp] -> xs row
         d = dict(C=Cc, H=Hc, W=Wc, Hp=Hp, Wp=Wp, ws=ws, cs=cs, S=S, ncw=ncw, nwin=nwin, nW=nW, n_ct=n_ct,
-                 xs=xs, pix_map_host=pix_map, padded=(Hp != Hc or Wp != Wc),
+                 xs=xs, pix_map_host=pix_map, padded=(Hp != Hc or Wp != Wc), pool=geo["pool"], tokens=geo["tokens"],
+                 pe_coords=geo["pe_coords"], hat_pe_coords=geo["hat_pe_coords"], own_tables=geo["own_tables"],
                  pix_map=nb.i32(f"l{i}.pix_map", pix_map.reshape(-1)),
                  crop_map=nb.i32(f"l{i}.crop_map", pix_map[:, :Hc, :Wc].reshape(-1)),
                  xn16=nb.new(f"l{i}.xn16", (nW * S, Cc), torch.float16),
@@ -497,11 +576,16 @@ class Plan:
             d["ctqkv16"] = nb.new(f"l{i}.ctqkv16", (B * n_ct, 3 * Cp), torch.float16)
             d["ctao16"] = nb.new(f"l{i}.ctao16", (B * n_ct, Cp), torch.float16)
             d["cth16"] = nb.new(f"l{i}.cth16", (B * n_ct, int(Cc * self.model.cfg["mlp_ratio"])), torch.float16)
-            # tokenizer output (b, y0, x0) over the (cs*nwh) x (cs*nww) carrier grid -> xs row
-            oh, ow = cs * nwh, cs * nww
-            bt, y0, x0 = torch.meshgrid(torch.arange(B), torch.arange(oh), torch.arange(ow), indexing="ij")
-            wloc = (y0 // cs) * nww + x0 // cs
-            d["ct_rows"] = nb.i32(f"l{i}.ct_rows", ((bt * nwin + wloc) * S + (y0 % cs) * cs + x0 % cs).reshape(-1))
+            if geo["tokens"] == "nchw":
+                # tokenizer token t of image b is window-major carrier t (the first block's ct_dewindow input)
+                bt, t = torch.meshgrid(torch.arange(B), torch.arange(n_ct), indexing="ij")
+                d["ct_rows"] = nb.i32(f"l{i}.ct_rows", ((bt * nwin + t // ncw) * S + t % ncw).reshape(-1))
+            else:
+                # tokenizer output (b, y0, x0) over the (cs*nwh) x (cs*nww) carrier grid -> xs row
+                oh, ow = cs * nwh, cs * nww
+                bt, y0, x0 = torch.meshgrid(torch.arange(B), torch.arange(oh), torch.arange(ow), indexing="ij")
+                wloc = (y0 // cs) * nww + x0 // cs
+                d["ct_rows"] = nb.i32(f"l{i}.ct_rows", ((bt * nwin + wloc) * S + (y0 % cs) * cs + x0 % cs).reshape(-1))
             # propagation source (nearest-neighbour upsample cs -> ws, fv.py:656, 699-700)
             r = torch.arange(nW * S)
             t = r % S - ncw
@@ -598,44 +682,50 @@ class Plan:
                  hdp, 0, 1)
         return wq, ldq, qb_ptr, wp, Cp
 
-    def _emit_bias(self, nm: str, rpb, S: int, hidden=None) -> dict:
+    def _emit_bias(self, nm: str, rpb, S: int, hidden=None, own: bool = False) -> dict:
         """PosEmbMLPSwinv2D (fv.py:276-307): table MLP + gather + 16*sigmoid, written straight into the
         module's `relative_bias` buffer (which the reference also overwrites every forward). With a `hidden` buffer
-        (training) the MLP also saves its hidden activations for the backward, and so runs in deploy mode too."""
+        (training) the MLP also saves its hidden activations for the backward, and so runs in deploy mode too.
+        own: into a plan buffer instead (token_geometry's own_tables: S changes with the input, and a module buffer
+        reallocated for one shape would leave every other cached plan pointing at freed memory)."""
         npts = rpb.relative_coords_table.shape[1] * rpb.relative_coords_table.shape[2]
         table = self.bufs.new(nm + ".table", (npts, rpb.num_heads), torch.float32)
-        if tuple(rpb.relative_bias.shape) != (1, rpb.num_heads, S, S):
-            rpb.relative_bias = torch.zeros(1, rpb.num_heads, S, S, device=self.device)
+        if own:
+            out = self.bufs.new(nm + ".out", (1, rpb.num_heads, S, S), torch.float32)
+        else:
+            if tuple(rpb.relative_bias.shape) != (1, rpb.num_heads, S, S):
+                rpb.relative_bias = torch.zeros(1, rpb.num_heads, S, S, device=self.device)
+            out = rpb.relative_bias
         tgt = self.prep_ops  # batch independent: recomputed only when the weights change
         n0 = len(tgt)
         self._op(tgt, "fvit_cpb_mlp_fwd", rpb.relative_coords_table.data_ptr(), npts, rpb.cpb_mlp[0].weight.data_ptr(),
                  rpb.cpb_mlp[0].bias.data_ptr(), rpb.cpb_mlp[2].weight.data_ptr(), rpb.num_heads,
                  table.data_ptr(), P(hidden))
         self._op(tgt, "fvit_attn_bias_fwd", table.data_ptr(), rpb.relative_position_index.data_ptr(),
-                 rpb.num_heads, S, rpb.window ** 2, rpb.relative_bias.data_ptr())
-        if hidden is None:
+                 rpb.num_heads, S, rpb.window ** 2, out.data_ptr())
+        if hidden is None and not own:
             self._deploy_guard(tgt, n0, rpb)
-        return dict(mod=rpb, out=rpb.relative_bias, hidden=hidden, npts=npts, S=S)
+        return dict(mod=rpb, out=out, hidden=hidden, npts=npts, S=S)
 
-    def _emit_pos_embed(self, nm: str, tpe, n_side: int, Cc: int, hidden=None) -> dict:
-        """PosEmbMLPSwinv1D rank 2 (fv.py:355-365): MLP over the centred n x n grid, written into the
-        module's `relative_bias` buffer; the add itself is fused into the following LayerNorm. `hidden`: as
-        _emit_bias."""
-        r = torch.arange(n_side, dtype=torch.float32)
-        grid = torch.stack(torch.meshgrid(r, r, indexing="ij"))          # 2, n, n
-        grid = (grid - n_side // 2) / (n_side // 2)
-        npts = n_side * n_side
+    def _emit_pos_embed(self, nm: str, tpe, coords_host: torch.Tensor, Cc: int, hidden=None, own: bool = False) -> dict:
+        """PosEmbMLPSwinv1D rank 2 (fv.py:355-365): MLP over the grid coordinates `coords_host` ([npts, 2],
+        token_geometry), written into the module's `relative_bias` buffer; the add itself is fused into the following
+        LayerNorm. `hidden`, `own`: as _emit_bias."""
+        npts = coords_host.shape[0]
         coords = self.bufs.new(nm + ".coords", (npts, 2), torch.float32)
-        coords.copy_(grid.flatten(1).t())
-        if tuple(tpe.relative_bias.shape) != (1, npts, Cc):
-            tpe.relative_bias = torch.zeros(1, npts, Cc, device=self.device)
+        coords.copy_(coords_host)
+        if own:
+            out = self.bufs.new(nm + ".out", (1, npts, Cc), torch.float32)
+        else:
+            if tuple(tpe.relative_bias.shape) != (1, npts, Cc):
+                tpe.relative_bias = torch.zeros(1, npts, Cc, device=self.device)
+            out = tpe.relative_bias
         n0 = len(self.prep_ops)
         self._op(self.prep_ops, "fvit_cpb_mlp_fwd", coords.data_ptr(), npts, tpe.cpb_mlp[0].weight.data_ptr(),
-                 tpe.cpb_mlp[0].bias.data_ptr(), tpe.cpb_mlp[2].weight.data_ptr(), Cc, tpe.relative_bias.data_ptr(),
-                 P(hidden))
-        if hidden is None:
+                 tpe.cpb_mlp[0].bias.data_ptr(), tpe.cpb_mlp[2].weight.data_ptr(), Cc, out.data_ptr(), P(hidden))
+        if hidden is None and not own:
             self._deploy_guard(self.prep_ops, n0, tpe)
-        return dict(mod=tpe, out=tpe.relative_bias, hidden=hidden, coords=coords, npts=npts, D=Cc)
+        return dict(mod=tpe, out=out, hidden=hidden, coords=coords, npts=npts, D=Cc)
 
     def _emit_branch_out(self, nm: str, lin: nn.Linear, gamma, a, lda, rows, stream_buf, act=L.ACT_NONE,
                          out16=None, ld16=0) -> None:
@@ -665,25 +755,28 @@ class Plan:
         # (the downsample GEMM that fills the window tokens was emitted before this call)
         if level.do_gt and has_ct:
             tk = level.global_tokenizer
-            (kh, sh_, oh), (kw, sw_, ow) = tk.pool
-            self._op(self.ops, "fvit_token_init_fwd", xs_ptr, Cc, tl["pix_map"].data_ptr(), B, tl["Hp"], tl["Wp"],
+            (kh, sh_, oh), (kw, sw_, ow) = tl["pool"]
+            entry = "fvit_token_init_nchw_fwd" if tl["tokens"] == "nchw" else "fvit_token_init_fwd"
+            self._op(self.ops, entry, xs_ptr, Cc, tl["pix_map"].data_ptr(), B, tl["Hp"], tl["Wp"],
                      Cc, tk.pos_embed.weight.data_ptr(), tk.pos_embed.bias.data_ptr(), kh, kw, sh_, sw_, oh, ow,
                      tl["ct_rows"].data_ptr(), xs_ptr, Cc)
+        own = tl["own_tables"]
         for j, blk in enumerate(level.blocks):
             nm = f"l{i}.b{j}"
-            pe = self._emit_pos_embed(nm + ".pe", blk.pos_embed, ws, Cc)["out"]
+            pe = self._emit_pos_embed(nm + ".pe", blk.pos_embed, tl["pe_coords"], Cc, own=own)["out"]
             if has_ct:
                 ctr_ptr = xs_ptr + tl["ctr0"] * Cc * 4
                 rows_c = B * n_ct
                 hat_pe = None
-                if hasattr(blk, "hat_pos_embed"):
-                    hat_pe = self._emit_pos_embed(nm + ".hat_pe", blk.hat_pos_embed, int(n_ct ** 0.5), Cc)["out"]
+                if tl["hat_pe_coords"] is not None:
+                    hat_pe = self._emit_pos_embed(nm + ".hat_pe", blk.hat_pos_embed, tl["hat_pe_coords"], Cc,
+                                                  own=own)["out"]
                 # ct = dewindow(ct) + hat_pos_embed ; LN -> fp16                 (fv.py:673-679)
                 self._op(self.ops, "fvit_ln_fwd", xs_ptr, Cc, tl["ct_gather"].data_ptr(), rows_c, Cc,
                          hat_pe.data_ptr() if hat_pe is not None else None, n_ct, 0, ctr_ptr, Cc,
                          blk.hat_norm1.weight.data_ptr(), blk.hat_norm1.bias.data_ptr(), float(blk.hat_norm1.eps),
                          tl["ctn16"].data_ptr(), Cc, None, None, None, None, 0)
-                hb = self._emit_bias(nm + ".hat_bias", blk.hat_attn.pos_emb_funct, n_ct)["out"]
+                hb = self._emit_bias(nm + ".hat_bias", blk.hat_attn.pos_emb_funct, n_ct, own=own)["out"]
                 self._emit_attention(nm + ".hat_attn", blk.hat_attn, blk.gamma1, rows_c, B, n_ct, tl["ctn16"], Cc,
                                      tl["ctqkv16"], tl["ctao16"], hb, ctr_ptr)
                 self._op(self.ops, "fvit_ln_fwd", ctr_ptr, Cc, None, rows_c, Cc, None, 1, 0, None, 0,
@@ -697,7 +790,7 @@ class Plan:
             self._op(self.ops, "fvit_ln_fwd", xs_ptr, Cc, tl["norm1_gather"].data_ptr() if has_ct else None, rows,
                      Cc, pe.data_ptr(), S, ncw, xs_ptr, Cc, blk.norm1.weight.data_ptr(), blk.norm1.bias.data_ptr(),
                      float(blk.norm1.eps), tl["xn16"].data_ptr(), Cc, None, None, None, None, 0)
-            ab = self._emit_bias(nm + ".bias", blk.attn.pos_emb_funct, S)["out"]
+            ab = self._emit_bias(nm + ".bias", blk.attn.pos_emb_funct, S, own=own)["out"]
             self._emit_attention(nm + ".attn", blk.attn, blk.gamma3, rows, nW, S, tl["xn16"], Cc, tl["qkv16"],
                                  tl["ao16"], ab, xs_ptr)
             self._op(self.ops, "fvit_ln_fwd", xs_ptr, Cc, None, rows, Cc, None, 1, 0, None, 0,
@@ -899,9 +992,19 @@ class Engine:
 
     def __init__(self, model):
         self.model = model
-        self.plans: dict = {}
+        self.plans: dict = {}     # in least-recently-used-first order
         self._prepped: dict = {}
         self._ptr_sig: tuple | None = None
+
+    def trim_plans(self) -> None:
+        """Keep at most model.plan_cache_size plans (None or absent: no bound), dropping the least recently used. A
+        dropped plan's device memory goes once nothing holds it: an autograd node of a forward that has not run its
+        backward yet keeps its plan until then. Its `_prepped` entry goes with it (keyed by id(), which a new plan may
+        reuse: a stale entry would skip that plan's weight packing)."""
+        cap = getattr(self.model, "plan_cache_size", None)
+        while cap is not None and len(self.plans) > cap:
+            plan = self.plans.pop(next(iter(self.plans)))
+            self._prepped.pop(id(plan), None)
 
     def _check_weights(self) -> tuple:
         """The kernels read parameters / buffers through raw pointers as dense row-major fp32 (int64 for the
@@ -950,19 +1053,25 @@ class Engine:
             # the level norms are not the model's own tensors (the backbone's norm{i}): the plan reads them through raw
             # pointers too, so a reallocation of one of them (`bn.weight.data = ...`) rebuilds it
             norm_sig = self._norm_sig(spec)
-        plan = self.plans.get(key)
+        plan = self.plans.pop(key, None)
         if plan is not None and getattr(plan, "_norm_sig", ()) != norm_sig:
-            del self.plans[key]
+            self._prepped.pop(id(plan), None)
             plan = None
-        if plan is None:
-            with torch.cuda.device(x.device):
-                if training or (spec is not None and spec.get("eval")):
-                    from .engine_train import TrainPlan
-                    plan = TrainPlan(self.model, x.shape[0], x.shape[2], x.shape[3], x.device, spec=spec)
-                else:
-                    plan = Plan(self.model, x.shape[0], x.shape[2], x.shape[3], training, x.device)
-            plan._norm_sig = norm_sig
-            self.plans[key] = plan
+        if plan is not None:
+            self.plans[key] = plan     # most recently used last
+            return plan
+        if getattr(self.model, "carriers_from_input", False) and spec is not None and spec.get("eval"):
+            raise L.FvitError("the detection backbone has no eval-mode gradients: train it under .train(), or run eval "
+                              "under torch.no_grad()")
+        with torch.cuda.device(x.device):
+            if training or (spec is not None and spec.get("eval")):
+                from .engine_train import TrainPlan
+                plan = TrainPlan(self.model, x.shape[0], x.shape[2], x.shape[3], x.device, spec=spec)
+            else:
+                plan = Plan(self.model, x.shape[0], x.shape[2], x.shape[3], training, x.device)
+        plan._norm_sig = norm_sig
+        self.plans[key] = plan
+        self.trim_plans()
         return plan
 
     @staticmethod

@@ -98,10 +98,11 @@ def _emit_conv_part_train(self) -> dict:
              bn1["sh"].data_ptr(), L.ACT_RELU, None, 0, None, 0, planes.data_ptr(), ld_in, None)
     # conv2 (stride 2) -> raw2 in the level-0 layout
     lvl = self._conv_level_train_buffers(0, dim, H0, W0, len(m.levels[0].blocks))
+    self._zero_window_padding(lvl)
     w2, ldw2 = self._pack_conv("stem.conv2", pe[3])
     raw2 = nb.new("stem.raw2", (lvl["rows"], lvl["ld"]), torch.float16)
     bn2 = _bn_train(self, "stem.bn2", pe[4], B * H0 * W0)
-    to_l0 = self._plane_to_padded_map("stem.to_l0", B, H0, W0)
+    to_l0 = self._plane_to_padded_map("stem.to_l0", B, H0, W0, lvl["Hb"], lvl["Wb"])
     self._gemm(a=planes.data_ptr(), a_rows=pl_rows, lda=ld_in, a_planes=4, a_plane_stride=pl_rows * ld_in, b=w2.data_ptr(),
                ldb=ldw2, m=pl_rows, n=dim, kc=in_dim, taps=self._s2_taps(W0), m_alg=B * H0 * W0,
                col_shift=_bn_col_shift(self, bn2, None), row_map=to_l0.data_ptr(),
@@ -122,6 +123,7 @@ def _emit_conv_part_train(self) -> dict:
         if i > 0:
             Hc, Wc, Cc = (Hc + 1) // 2, (Wc + 1) // 2, Cc * 2
             lvl = self._conv_level_train_buffers(i, Cc, Hc, Wc, len(level.blocks))
+            self._zero_window_padding(lvl)
             self._emit_downsample_train(i - 1, prev, lvl)
         self._emit_conv_blocks_train(i, level, lvl)
         lvl["kind"] = "conv"
@@ -148,7 +150,8 @@ def _conv_level_train_buffers(self, i: int, Cc: int, Hc: int, Wc: int, depth: in
 
 def _emit_conv_blocks_train(self, i: int, level, lv: dict) -> None:
     B, nb = self.B, self.bufs
-    Cc, Wp, rows, ld, npix = lv["C"], lv["W"] + 2, lv["rows"], lv["ld"], lv["npix"]
+    # the blocks compute the whole (window-padded, conv_level_pad) map: statistics and affine passes over cpix
+    Cc, Wp, rows, ld, npix, pix = lv["C"], lv["Wb"] + 2, lv["rows"], lv["ld"], lv["cnpix"], lv["cpix"]
     taps = [((dy - 1) * Wp + (dx - 1), 0) for dy in range(3) for dx in range(3)]
     lv["taps"] = taps
     lv["blocks_sv"] = []
@@ -158,7 +161,7 @@ def _emit_conv_blocks_train(self, i: int, level, lv: dict) -> None:
         nm = f"l{i}.b{j}"
         rate = self._drop_rate(i)
         self._block_counter += 1
-        rs = self._drop_buf(f"levels.{i}.blocks.{j}", rate, B, (lv["H"] + 2) * (lv["W"] + 2))
+        rs = self._drop_buf(f"levels.{i}.blocks.{j}", rate, B, (lv["Hb"] + 2) * (lv["Wb"] + 2))
         w1, ld1 = self._pack_conv(nm + ".conv1", blk.conv1)
         w2, ld2 = self._pack_conv(nm + ".conv2", blk.conv2)
         rawA = nb.new(nm + ".rawA", (rows, ld), torch.float16)
@@ -171,13 +174,13 @@ def _emit_conv_blocks_train(self, i: int, level, lv: dict) -> None:
                    m_alg=npix, col_shift=_bn_col_shift(self, bnA, blk.conv1.bias), row_map=lv["interior"].data_ptr(),
                    out_f16=rawA.data_ptr(), ld_o16=ld, col_sum=bnA["col_sum"], col_sumsq=bnA["col_sumsq"])
         _bn_finalize(self, bnA)
-        self._op(self.ops, "fvit_affine_rows", rawA.data_ptr(), ld, lv["pix"].data_ptr(), npix, Cc, bnA["sc"].data_ptr(),
+        self._op(self.ops, "fvit_affine_rows", rawA.data_ptr(), ld, pix.data_ptr(), npix, Cc, bnA["sc"].data_ptr(),
                  bnA["sh"].data_ptr(), L.ACT_GELU, None, 0, None, 0, h16.data_ptr(), ld, None)
         self._gemm(a=h16.data_ptr(), a_rows=rows, lda=ld, b=w2.data_ptr(), ldb=ld2, m=rows, n=Cc, kc=Cc, taps=taps,
                    m_alg=npix, col_shift=_bn_col_shift(self, bnB, blk.conv2.bias), row_map=lv["interior"].data_ptr(),
                    out_f16=rawB.data_ptr(), ld_o16=ld, col_sum=bnB["col_sum"], col_sumsq=bnB["col_sumsq"])
         _bn_finalize(self, bnB)
-        self._op(self.ops, "fvit_affine_rows", rawB.data_ptr(), ld, lv["pix"].data_ptr(), npix, Cc, bnB["sc"].data_ptr(),
+        self._op(self.ops, "fvit_affine_rows", rawB.data_ptr(), ld, pix.data_ptr(), npix, Cc, bnB["sc"].data_ptr(),
                  bnB["sh"].data_ptr(), L.ACT_NONE, lv["x32"].data_ptr(), Cc, lv["x32"].data_ptr(), Cc, xout.data_ptr(), ld, rs)
         # data-gradient operands: flipped / transposed packed weights
         wT1 = nb.new(nm + ".conv1.wT16", (Cc, 9 * _ru(Cc, 64)), torch.float16)
@@ -319,10 +322,10 @@ def _emit_conv_blocks_bwd(self, lv: dict, input_grad: bool = True) -> None:
     """input_grad=False: nothing below reads the gradient of the level's input (the frozen prefix ends here), so the
     first block's conv1 data-gradient GEMM is not emitted. A data-only level: the two BatchNorm passes without their
     reductions and the two data-gradient GEMMs per block."""
-    Cc, rows, ld, npix = lv["C"], lv["rows"], lv["ld"], lv["npix"]
+    Cc, rows, ld, npix = lv["C"], lv["rows"], lv["ld"], lv["cnpix"]
     data_only = self.data_only[1 + lv["level_index"]]
     g = lv["g"].data_ptr()
-    pix, interior = lv["pix"].data_ptr(), lv["interior"].data_ptr()
+    pix, interior = lv["cpix"].data_ptr(), lv["interior"].data_ptr()   # (the whole computed map, _emit_conv_blocks_train)
     shifts = [s for (s, _) in lv["taps"]]
     for sv in reversed(lv["blocks_sv"]):
         blk, bnA, bnB = sv["blk"], sv["bnA"], sv["bnB"]

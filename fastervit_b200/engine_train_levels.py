@@ -177,20 +177,20 @@ def _inject(self, level: int, g=True) -> None:
                  self.G(bn.weight) if bn is not None else None, self.G(bn.bias) if bn is not None else None)
 
 
-def _posemb_train(self, nm: str, tpe, n_side: int, Cc: int) -> dict:
+def _posemb_train(self, nm: str, tpe, coords: torch.Tensor, Cc: int, own: bool = False) -> dict:
     """Plan._emit_pos_embed saving the MLP's hidden activations, plus the scratch slice of its output gradient"""
-    hidden = self.bufs.new(nm + ".hidden", (n_side ** 2, 512), torch.float32)
-    pe = self._emit_pos_embed(nm, tpe, n_side, Cc, hidden=hidden)
+    hidden = self.bufs.new(nm + ".hidden", (coords.shape[0], 512), torch.float32)
+    pe = self._emit_pos_embed(nm, tpe, coords, Cc, hidden=hidden, own=own)
     pe["dout"] = ("scr", self._scratch(nm + ".dpe", pe["npts"] * Cc))
     return pe
 
 
-def _bias_train(self, nm: str, rpb, S: int) -> dict:
+def _bias_train(self, nm: str, rpb, S: int, own: bool = False) -> dict:
     """Plan._emit_bias saving the table MLP's hidden activations, plus the scratch slices of the bias and table
     gradients"""
     npts = rpb.relative_coords_table.shape[1] * rpb.relative_coords_table.shape[2]
     hidden = self.bufs.new(nm + ".hidden", (npts, 512), torch.float32)
-    bs = self._emit_bias(nm, rpb, S, hidden=hidden)
+    bs = self._emit_bias(nm, rpb, S, hidden=hidden, own=own)
     bs["dbias"] = ("scr", self._scratch(nm + ".dbias", rpb.num_heads * S * S))
     bs["dtable"] = ("scr", self._scratch(nm + ".dtable", npts * rpb.num_heads))
     return bs
@@ -253,8 +253,9 @@ def _emit_token_level_train(self, i: int, level, tl: dict) -> None:
     tl["blocks_sv"] = []
     if level.do_gt and has_ct:
         tk = level.global_tokenizer
-        (kh, sh_, oh), (kw, sw_, ow) = tk.pool
-        self._op(self.ops, "fvit_token_init_fwd", xs_ptr, Cc, tl["pix_map"].data_ptr(), B, tl["Hp"], tl["Wp"], Cc,
+        (kh, sh_, oh), (kw, sw_, ow) = tl["pool"]
+        entry = "fvit_token_init_nchw_fwd" if tl["tokens"] == "nchw" else "fvit_token_init_fwd"
+        self._op(self.ops, entry, xs_ptr, Cc, tl["pix_map"].data_ptr(), B, tl["Hp"], tl["Wp"], Cc,
                  tk.pos_embed.weight.data_ptr(), tk.pos_embed.bias.data_ptr(), kh, kw, sh_, sw_, oh, ow,
                  tl["ct_rows"].data_ptr(), xs_ptr, Cc)
 
@@ -275,13 +276,14 @@ def _emit_token_level_train(self, i: int, level, tl: dict) -> None:
         if has_ct:
             sv["rs_hat_attn"] = self._drop_buf(key + ".hat_attn", rate, B, n_ct)
             sv["rs_hat_mlp"] = self._drop_buf(key + ".hat_mlp", rate, B, n_ct)
-        sv["pe"] = self._posemb_train(nm + ".pe", blk.pos_embed, ws, Cc)
+        sv["pe"] = self._posemb_train(nm + ".pe", blk.pos_embed, tl["pe_coords"], Cc, own=tl["own_tables"])
         if has_ct:
             ctr_ptr = xs_ptr + tl["ctr0"] * Cc * 4
             rows_c = B * n_ct
             sv["hat_pe"] = None
-            if hasattr(blk, "hat_pos_embed"):
-                sv["hat_pe"] = self._posemb_train(nm + ".hat_pe", blk.hat_pos_embed, int(n_ct ** 0.5), Cc)
+            if tl["hat_pe_coords"] is not None:
+                sv["hat_pe"] = self._posemb_train(nm + ".hat_pe", blk.hat_pos_embed, tl["hat_pe_coords"], Cc,
+                                                  own=tl["own_tables"])
             c = dict(y1=new16(nm + ".c.y1", rows_c, Cc), xh1=new16(nm + ".c.xh1", rows_c, Cc), rs1=new32(nm + ".c.rs1", rows_c),
                      mu1=new32(nm + ".c.mu1", rows_c), y2=new16(nm + ".c.y2", rows_c, Cc), xh2=new16(nm + ".c.xh2", rows_c, Cc),
                      rs2=new32(nm + ".c.rs2", rows_c), mu2=new32(nm + ".c.mu2", rows_c),
@@ -293,7 +295,7 @@ def _emit_token_level_train(self, i: int, level, tl: dict) -> None:
                      sv["hat_pe"]["out"].data_ptr() if sv["hat_pe"] else None, n_ct, 0, ctr_ptr, Cc,
                      blk.hat_norm1.weight.data_ptr(), blk.hat_norm1.bias.data_ptr(), float(blk.hat_norm1.eps),
                      c["y1"].data_ptr(), Cc, None, c["mu1"].data_ptr(), c["rs1"].data_ptr(), c["xh1"].data_ptr(), Cc)
-            sv["c_bias"] = self._bias_train(nm + ".hat_bias", blk.hat_attn.pos_emb_funct, n_ct)
+            sv["c_bias"] = self._bias_train(nm + ".hat_bias", blk.hat_attn.pos_emb_funct, n_ct, own=tl["own_tables"])
             sv["c_attn"] = self._attn_fwd_train(nm + ".hat_attn", blk.hat_attn, blk.gamma1, rows_c, B, n_ct, c["y1"],
                                                 c["qkv"], c["ao"], sv["c_bias"], ctr_ptr, c["u1"], sv["rs_hat_attn"])
             self._op(self.ops, "fvit_ln_fwd", ctr_ptr, Cc, None, rows_c, Cc, None, 1, 0, None, 0,
@@ -311,7 +313,7 @@ def _emit_token_level_train(self, i: int, level, tl: dict) -> None:
                  sv["pe"]["out"].data_ptr(), S, ncw, xs_ptr, Cc, blk.norm1.weight.data_ptr(), blk.norm1.bias.data_ptr(),
                  float(blk.norm1.eps), w["y1"].data_ptr(), Cc, None, w["mu1"].data_ptr(), w["rs1"].data_ptr(),
                  w["xh1"].data_ptr(), Cc)
-        sv["w_bias"] = self._bias_train(nm + ".bias", blk.attn.pos_emb_funct, S)
+        sv["w_bias"] = self._bias_train(nm + ".bias", blk.attn.pos_emb_funct, S, own=tl["own_tables"])
         sv["w_attn"] = self._attn_fwd_train(nm + ".attn", blk.attn, blk.gamma3, rows, nW, S, w["y1"], w["qkv"], w["ao"],
                                             sv["w_bias"], xs_ptr, w["u1"], sv["rs_attn"])
         self._op(self.ops, "fvit_ln_fwd", xs_ptr, Cc, None, rows, Cc, None, 1, 0, None, 0, blk.norm2.weight.data_ptr(),
@@ -423,6 +425,11 @@ def _build_backward(self) -> None:
             self.grad_buckets.append((lo, hi))
             self.bwd_ops.append(("bucket", (lo, hi), "grad_bucket"))
 
+    for lv in self.conv_lv:
+        if lv["cpix"] is not lv["pix"]:
+            # a window-padded conv level (conv_level_pad): its blocks' backward writes the padding rows of g, which
+            # nothing above it does; they start every backward at zero
+            self.bwd_ops.append(("zero", lv["g"], "memset"))
     if self.kind is None:
         self._emit_head_bwd(self.feat)
     elif self.kind == "pooled":
@@ -729,12 +736,13 @@ def _emit_token_level_bwd(self, tl: dict, after_block=None) -> None:
     level = self.model.levels[tl["level_index"]]
     if level.do_gt and has_ct:
         tk = level.global_tokenizer
-        (kh, sh_, oh), (kw, sw_, ow) = tk.pool
+        (kh, sh_, oh), (kw, sw_, ow) = tl["pool"]
+        nchw = "_nchw" if tl["tokens"] == "nchw" else ""
         if do:
-            self._op(ops, "fvit_token_init_dgrad", g_ptr, Cc, tl["pix_map"].data_ptr(), tl["ct_rows"].data_ptr(), B, tl["Hp"],
+            self._op(ops, f"fvit_token_init{nchw}_dgrad", g_ptr, Cc, tl["pix_map"].data_ptr(), tl["ct_rows"].data_ptr(), B, tl["Hp"],
                      tl["Wp"], Cc, tk.pos_embed.weight.data_ptr(), kh, kw, sh_, sw_, oh, ow, g_ptr, Cc)
             return
-        self._op(ops, "fvit_token_init_bwd", g_ptr, Cc, tl["x0_16"].data_ptr(), Cc, tl["pix_map"].data_ptr(),
+        self._op(ops, f"fvit_token_init{nchw}_bwd", g_ptr, Cc, tl["x0_16"].data_ptr(), Cc, tl["pix_map"].data_ptr(),
                  tl["ct_rows"].data_ptr(), B, tl["Hp"], tl["Wp"], Cc, tk.pos_embed.weight.data_ptr(), kh, kw, sh_, sw_, oh, ow,
                  ("scal", 1), g_ptr, Cc, self.G(tk.pos_embed.weight), self.G(tk.pos_embed.bias))
 

@@ -132,6 +132,9 @@ _OP_SIGS: dict[str, list] = {
     "fvit_cpb_mlp_fwd": [_P, _I, _P, _P, _P, _I, _P, _P, _P],
     "fvit_attn_bias_fwd": [_P, _P, _I, _I, _I, _P, _P],
     "fvit_token_init_fwd": [_P, _L, _P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _L, _P],
+    "fvit_token_init_nchw_bwd": [_P, _L, _P, _L, _P, _P, _I, _I, _I, _I, _P, _I, _I, _I, _I, _I, _I, _P, _P, _L, _P, _P, _P],
+    "fvit_token_init_nchw_dgrad": [_P, _L, _P, _P, _I, _I, _I, _I, _P, _I, _I, _I, _I, _I, _I, _P, _L, _P],
+    "fvit_token_init_nchw_fwd": [_P, _L, _P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _L, _P],
     "fvit_propagate_fwd": [_P, _L, _P, _I, _I, _P, _P],
     "fvit_pool_affine_fwd": [_P, _L, _P, _I, _I, _I, _P, _P, _P, _L, _P],
     "fvit_feature_map_fwd": [_P, _L, _P, _I, _I, _I, _P, _P, _P, _P],

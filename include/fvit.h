@@ -266,7 +266,7 @@ int fvit_bn_finalize_pivot(const float* sum, const float* sumsq, const float* pi
 int fvit_cpb_mlp_fwd(const float* coords, int32_t P, const float* w0, const float* b0, const float* w1,
                      int32_t D, float* out, float* hidden_out, void* stream);
 /* bias[h][r][c] = 16*sigmoid(table[index[(r-ng)*L + (c-ng)]][h]) for r,c >= ng = S-L, else 0
- * (PosEmbMLPSwinv2D.forward fv.py:276-299). */
+ * (PosEmbMLPSwinv2D.forward fv.py:276-299). S < L (ng < 0) crops the top-left of the L x L table. */
 int fvit_attn_bias_fwd(const float* table, const int64_t* index, int32_t heads, int32_t S, int32_t L,
                        float* bias, void* stream);
 
@@ -277,6 +277,13 @@ int fvit_token_init_fwd(const float* xs, int64_t ldx, const int32_t* pix_map, in
                         int32_t Wp, int32_t C, const float* w, const float* bias, int32_t kh, int32_t kw,
                         int32_t sh, int32_t sw, int32_t oh, int32_t ow, const int32_t* ct_row_map,
                         float* out, int64_t ldo, void* stream);
+/* The same pooled values stored as the detection backbone reads them (dino/models/dino/fastervit.py:591): image b's
+ * NCHW map reinterpreted as [oh*ow, C] tokens, value (c, p) -> token t, channel k with c*oh*ow + p = t*C + k, written to
+ * row ct_row_map[b*oh*ow + t] of `out`. */
+int fvit_token_init_nchw_fwd(const float* xs, int64_t ldx, const int32_t* pix_map, int32_t B, int32_t Hp,
+                             int32_t Wp, int32_t C, const float* w, const float* bias, int32_t kh, int32_t kw,
+                             int32_t sh, int32_t sw, int32_t oh, int32_t ow, const int32_t* ct_row_map,
+                             float* out, int64_t ldo, void* stream);
 
 /* ---- carrier -> window propagation (fv.py:697-700): xs[r] += gamma * xs[src_map[r]] (src_map < 0:
  * row untouched; gamma NULL = 1). */
@@ -406,7 +413,8 @@ int fvit_attn_loop_bwd_long(const void* qkv, int64_t ldq, const void* dout, int6
 int fvit_unpad_heads_f32(const float* src, int64_t lds, float* dst, int64_t ldd, int32_t rows_src, int32_t cols_src,
                          int32_t hd, int32_t hdp, int32_t pad_rows, int32_t pad_cols, const float* scalar,
                          void* stream);
-/* Backward of fvit_attn_bias_fwd: dtable[index][h] += *scalar * dbias * b*(1 - b/16), b = 16 sigmoid(table). */
+/* Backward of fvit_attn_bias_fwd: dtable[index][h] += *scalar * dbias * b*(1 - b/16), b = 16 sigmoid(table); with
+ * S < L only the entries the forward kept. */
 int fvit_attn_bias_bwd(const float* dbias, const float* bias, const int64_t* index, int32_t heads, int32_t S,
                        int32_t L, const float* scalar, float* dtable, void* stream);
 /* Backward of fvit_cpb_mlp_fwd (needs the saved hidden activations): accumulates dw0 [512,2], db0 [512],
@@ -502,6 +510,15 @@ int fvit_ln_dgrad(const void* dy16, int64_t lddy, const int32_t* dy_map, const v
 int fvit_token_init_dgrad(const float* g, int64_t ldg, const int32_t* pix_map, const int32_t* ct_row_map, int32_t B,
                           int32_t Hp, int32_t Wp, int32_t C, const float* w, int32_t kh, int32_t kw, int32_t sh,
                           int32_t sw, int32_t oh, int32_t ow, float* gx, int64_t ldgx, void* stream);
+/* fvit_token_init_bwd / fvit_token_init_dgrad for the carrier tokens of fvit_token_init_nchw_fwd: the gradient of pooled
+ * value (c, p) of image b is channel (c*oh*ow + p) % C of row ct_row_map[b*oh*ow + (c*oh*ow + p) / C]. */
+int fvit_token_init_nchw_bwd(const float* g, int64_t ldg, const void* x16, int64_t ldx, const int32_t* pix_map,
+                             const int32_t* ct_row_map, int32_t B, int32_t Hp, int32_t Wp, int32_t C, const float* w,
+                             int32_t kh, int32_t kw, int32_t sh, int32_t sw, int32_t oh, int32_t ow, const float* scalar,
+                             float* gx, int64_t ldgx, float* dw, float* dbias, void* stream);
+int fvit_token_init_nchw_dgrad(const float* g, int64_t ldg, const int32_t* pix_map, const int32_t* ct_row_map, int32_t B,
+                               int32_t Hp, int32_t Wp, int32_t C, const float* w, int32_t kh, int32_t kw, int32_t sh,
+                               int32_t sw, int32_t oh, int32_t ow, float* gx, int64_t ldgx, void* stream);
 
 /* ---- optimizer step on the flat gradient buffer (SURVEY §8 f.1; train.py:879-899) -----------------------
  * Replaces, for the training loop either side of loss.backward(): GradScaler.unscale_ + the non-finite check,
