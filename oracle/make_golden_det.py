@@ -8,9 +8,10 @@ timm stand-in and a util.misc.NestedTensor stand-in (oracle/ref_shim). Each case
 state_dict with the oracle's deterministic synthetic weights (synth_fill_), runs its eval forward in fp64 at every shape
 of SHAPES (batch 2) and stores samples of the normed level maps together with the carrier geometry the reference used
 (pool kernel / stride, tokenizer output grid, carrier sequence length), and the train steps of TRAIN (maps, running
-statistics after the step, parameter-gradient samples). It also stores the missing / unexpected keys of
-load_state_dict(classification state_dict, strict=False), and `det_schema.pt` holds the state_dict schema (keys,
-shapes, dtypes) of the eight full-size build_fastervit names. The tests never need the reference.
+statistics after the step, parameter-gradient samples); those of TRAIN_DETR go to <case>_detr.pt. It also stores the
+missing / unexpected keys of load_state_dict(classification state_dict, strict=False), and `det_schema.pt` holds the
+state_dict schema (keys, shapes, dtypes) of the eight full-size build_fastervit names. The tests never need the
+reference.
 """
 from __future__ import annotations
 
@@ -58,6 +59,10 @@ CASES = {
 # The reference's _freeze_stages raises for frozen_stages >= 2 (it names a missing `self.network`): the generator
 # freezes what it means to -- patch_embed and levels[:frozen_stages - 1] in eval mode without gradients -- itself.
 TRAIN = [((96, 160), -1), ((320, 480), -1), ((96, 160), 2)]
+# DETR training sizes with more than 64 carriers: 480 x 544 and 544 x 800 (100 and 160 carriers: the key-loop attention
+# with one and two key tiles; tokenizer pools of kernel 8 x 8 and 8 x 11, stride 3). Their input seeds continue TRAIN's;
+# they are stored in a file of their own, <case>_detr.pt, so that each golden file stays small.
+TRAIN_DETR = [((480, 544), -1), ((544, 800), -1)]
 SEED_G = 11
 
 
@@ -122,13 +127,16 @@ def run_case(det, case: str) -> None:
                                  "masks": {i: o.mask.clone() for i, o in outs.items()}}
         print(f"  {case} {H}x{W}: {geo}", flush=True)
     out["train"] = {}
+    detr = {k: out[k] for k in ("case", "name", "kwargs", "seeds")} | {"train": {}}
     if case != "det_tiny_hd64":
-        for ti, ((H, W), fs) in enumerate(TRAIN):
-            out["train"][(H, W, fs)] = run_train(det, name, kw, H, W, fs, SEED_X + 50 + ti)
+        for ti, ((H, W), fs) in enumerate(TRAIN + TRAIN_DETR):
+            dst = out if ti < len(TRAIN) else detr
+            dst["train"][(H, W, fs)] = run_train(det, name, kw, H, W, fs, SEED_X + 50 + ti)
     GOLDEN.mkdir(parents=True, exist_ok=True)
-    path = GOLDEN / f"{case}.pt"
-    torch.save(out, path, _use_new_zipfile_serialization=False)
-    print(f"{case}: {path.name} {path.stat().st_size / 1024:.0f} KiB, {time.time() - t0:.1f}s", flush=True)
+    for res, path in ((out, GOLDEN / f"{case}.pt"), (detr, GOLDEN / f"{case}_detr.pt")):
+        if res["train"] or res is out:
+            torch.save(res, path, _use_new_zipfile_serialization=False)
+            print(f"{case}: {path.name} {path.stat().st_size / 1024:.0f} KiB, {time.time() - t0:.1f}s", flush=True)
 
 
 def run_train(det, name: str, kw: dict, H: int, W: int, fs: int, x_seed: int) -> dict:

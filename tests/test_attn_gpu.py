@@ -21,7 +21,9 @@ def _ref(qkv, groups, S, heads, hd, hdp, bias, scale):
 
 @pytest.mark.parametrize("S,heads,hd,groups", [(53, 8, 32, 37), (49, 16, 32, 20), (16, 8, 32, 11), (53, 16, 49, 9),
                                                (60, 8, 32, 5), (36, 16, 32, 31), (128, 2, 64, 3), (64, 4, 24, 6),
-                                               (53, 8, 32, 1024)])
+                                               (53, 8, 32, 1024),
+                                               # detection carrier attention: one sequence per image
+                                               (4, 8, 32, 2), (8, 4, 16, 2), (100, 16, 49, 2), (120, 8, 32, 2)])
 @pytest.mark.parametrize("with_bias", [True, False])
 def test_attn_tc_matches_torch(S, heads, hd, groups, with_bias):
     from fastervit_b200 import lib
@@ -44,7 +46,10 @@ def test_attn_tc_matches_torch(S, heads, hd, groups, with_bias):
 
 @pytest.mark.parametrize("S,heads,hd,groups", [(148, 8, 32, 30), (148, 8, 32, 480), (196, 16, 49, 8), (144, 4, 24, 5),
                                                (256, 2, 64, 3), (576, 4, 49, 2), (1024, 2, 49, 1), (2304, 1, 49, 1),
-                                               (132, 3, 32, 7), (68, 4, 16, 12), (104, 8, 32, 300), (128, 2, 64, 5)])
+                                               (132, 3, 32, 7), (68, 4, 16, 12), (104, 8, 32, 300), (128, 2, 64, 5),
+                                               # detection carrier attention (one sequence per image): last key tile
+                                               # of 120, 12, 124 and 128 rows
+                                               (120, 8, 32, 2), (140, 4, 16, 2), (252, 16, 49, 2), (384, 8, 32, 2)])
 @pytest.mark.parametrize("with_bias", [True, False])
 def test_attn_loop_matches_torch(S, heads, hd, groups, with_bias):
     """Key-loop tensor-core attention: the any-res level-2 geometry (S = 148, BASELINE config 4), the 21k windows and
@@ -94,7 +99,8 @@ def test_attn_simt_matches_torch(S, heads, hd, groups):
 
 
 @pytest.mark.parametrize("S,heads,hd,groups", [(53, 8, 32, 37), (49, 16, 32, 20), (16, 8, 32, 11), (53, 16, 49, 9),
-                                               (60, 8, 32, 5), (36, 4, 24, 13), (53, 8, 32, 1024)])
+                                               (60, 8, 32, 5), (36, 4, 24, 13), (53, 8, 32, 1024),
+                                               (4, 8, 32, 2), (8, 16, 49, 2)])   # detection carriers, per image
 @pytest.mark.parametrize("tc", [True, False])
 def test_attn_backward_matches_autograd(S, heads, hd, groups, tc):
     """dq, dk, dv and dbias of both backward kernels (wgmma / SIMT) vs torch autograd in fp32."""
@@ -137,7 +143,9 @@ def test_attn_backward_matches_autograd(S, heads, hd, groups, tc):
                                                (148, 8, 32, 9), (576, 16, 49, 150), (2304, 1, 32, 1),
                                                (68, 4, 16, 12), (104, 8, 32, 7), (128, 2, 64, 5), (100, 3, 49, 200),
                                                (196, 16, 49, 4), (144, 4, 24, 5), (256, 2, 64, 3), (132, 3, 32, 7),
-                                               (148, 8, 32, 200)])
+                                               (148, 8, 32, 200),
+                                               # detection carrier attention (one sequence per image)
+                                               (120, 8, 32, 2), (140, 4, 16, 2), (252, 16, 49, 2), (384, 8, 32, 2)])
 def test_attn_loop_long_backward_matches_autograd(S, heads, hd, groups):
     """fvit_attn_loop_bwd_long (any number of 128-row tiles: the any-res S = 148 windows, the 21k models' 576 / 1024 /
     2304-token windows): dq, dk,

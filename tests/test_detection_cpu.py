@@ -1,10 +1,15 @@
 """Host-side checks of the DINO detection backbone (fastervit_b200.detection): state_dict schema and checkpoint loading
-against the reference module, the per-input carrier geometry against what the reference used at every golden shape (the
-plans are built on the CPU, nothing is launched), and the plan cache bound."""
+against the reference module, the per-input carrier geometry against what the reference used at every golden shape, the
+kernels the plans pick at DETR training sizes (the plans are built on the CPU, nothing is launched), and the plan cache
+bound."""
+import sys
 from pathlib import Path
 
 import pytest
 import torch
+
+sys.path.insert(0, str(Path(__file__).resolve().parent))   # tests/_token_init.py
+from _token_init import detr_shapes, level_sizes  # noqa: E402
 
 GOLDEN = Path(__file__).parent / "golden"
 CASES = ["det_tiny_fv0", "det_tiny_fv4", "det_tiny_21k"]
@@ -42,14 +47,6 @@ def test_tiny_schema_and_classification_checkpoint_keys(case):
     assert sorted(res.unexpected_keys) == g["load_cls"]["unexpected"]
 
 
-def _level_sizes(H, W):
-    h, w = (H + 1) // 2, (W + 1) // 2
-    sizes = [((h + 1) // 2, (w + 1) // 2)]
-    for _ in range(3):
-        sizes.append(((sizes[-1][0] + 1) // 2, (sizes[-1][1] + 1) // 2))
-    return sizes
-
-
 @pytest.mark.parametrize("case", ["det_tiny_fv0", "det_tiny_fv4"])
 def test_carrier_geometry_matches_the_reference(case):
     from fastervit_b200.detection import build_fastervit
@@ -59,7 +56,7 @@ def test_carrier_geometry_matches_the_reference(case):
     shapes0 = {k: tuple(v.shape) for k, v in det.state_dict().items()}
     for (H, W), ref in g["shapes"].items():
         geo_ref = ref["geometry"]
-        Hc, Wc = _level_sizes(H, W)[2]
+        Hc, Wc = level_sizes(H, W)[2]
         geo = token_geometry(det, 2, Hc, Wc)
         (kh, sh, oh), (kw, sw, ow) = geo["pool"]
         assert ((kh, kw), (sh, sw)) == geo_ref["pool"], (H, W)
@@ -82,6 +79,88 @@ def test_carrier_geometry_matches_the_reference(case):
         assert torch.equal(grid_coords(2, 4, 4)[-1], torch.tensor([(1 - 4) / 4, (3 - 4) / 4]))
     # the modules' buffers keep their construction shapes (the plans own the per-shape tables)
     assert {k: tuple(v.shape) for k, v in det.state_dict().items()} == shapes0
+
+
+def _launches(plan):
+    """every launch of a plan's lists as (name, args), deploy-guarded ones unwrapped"""
+    for ops in (v for v in vars(plan).values() if isinstance(v, list)):
+        for op in ops:
+            if isinstance(op, tuple) and len(op) == 3 and isinstance(op[2], str):
+                yield op[2], (op[1][2] if op[0] == "unless_deploy" else op[1])
+
+
+# where each entry point keeps (Hp, Wp) and (kh, kw, sh, sw, oh, ow) in its argument list (include/fvit.h)
+_TOKEN_INIT_ARGS = {"fvit_token_init_nchw_fwd": (4, 9), "fvit_token_init_nchw_bwd": (7, 11),
+                    "fvit_token_init_nchw_dgrad": (5, 9)}
+# where each attention entry point keeps S
+_ATTN_S = {"fvit_attn_tc_fwd": 3, "fvit_hat_attn_fwd": 7, "fvit_attn_loop_fwd": 3, "fvit_attn_core_fwd": 3,
+           "fvit_attn_tc_bwd": 5, "fvit_attn_core_bwd": 5, "fvit_attn_loop_bwd_long": 8}
+
+
+@pytest.mark.parametrize("hw", [(64, 64), (96, 96)] + detr_shapes(40))
+def test_detr_size_plans_launch_what_the_kernel_tests_cover(hw):
+    """The eval plan and the levels-mode train plan (batch 2, the spec forward_levels passes) of the fv0-like detection
+    backbone at DETR training sizes: the tokenizer launches carry token_geometry's pool, whose windows tile the padded
+    map exactly; carrier attention takes the tile kernels only where they fit (forward S <= 128, tensor-core backward S
+    <= 64) and the key-loop kernels only for S % 4 == 0 (TMA-staged bias rows); every bias-table backward matches its
+    forward's (S, L); every scatter_add_rows map is injective (a plain read-modify-write, include/fvit.h)."""
+    from fastervit_b200.detection import build_fastervit
+    from fastervit_b200.engine import Plan, token_geometry
+    from fastervit_b200.engine_train import TrainPlan
+    H, W = hw
+    det = build_fastervit("faster_vit_0_224", out_indices=(0, 1, 2, 3), drop_path_rate=0.0, dim=16, in_dim=16,
+                          depths=[1, 1, 2, 1], num_heads=[1, 2, 4, 8])
+    geos = {}
+    for i, (Hc, Wc) in enumerate(level_sizes(H, W)):
+        if det.levels[i].conv:
+            continue
+        geo = token_geometry(det, i, Hc, Wc)
+        if geo["has_ct"]:
+            (kh, sh, oh), (kw, sw, ow) = geo["pool"]
+            assert (oh - 1) * sh + kh == geo["Hp"] and (ow - 1) * sw + kw == geo["Wp"], (hw, i, geo["pool"])
+            geos[i] = ((geo["Hp"], geo["Wp"]), (kh, kw, sh, sw, oh, ow))
+    assert geos, "level 2 has carriers at every size"
+    n_ct = {g[1][4] * g[1][5] for g in geos.values()}
+    spec = dict(kind="levels", outs=tuple((i, getattr(det, f"norm{i}")) for i in range(4)), frozen=-1)
+    cpu = torch.device("cpu")
+    plans = [Plan(det.eval(), 2, H, W, False, cpu), TrainPlan(det.train(), 2, H, W, cpu, spec)]
+    for plan in plans:
+        launches = list(_launches(plan))
+        names = [n for n, _ in launches]
+        tok = [(n, a) for n, a in launches if n in _TOKEN_INIT_ARGS]
+        assert names.count("fvit_token_init_nchw_fwd") == len(geos), hw
+        assert "fvit_token_init_fwd" not in names and "fvit_token_init_bwd" not in names
+        for n, a in tok:
+            hp, kp = _TOKEN_INIT_ARGS[n]
+            assert (tuple(a[hp:hp + 2]), tuple(a[kp:kp + 6])) in geos.values(), (hw, n, a[hp:hp + 2], a[kp:kp + 6])
+        carrier_s = set()
+        for n, a in launches:
+            if n not in _ATTN_S:
+                continue
+            S = a[_ATTN_S[n]]
+            if S in n_ct:
+                carrier_s.add(S)
+            if n in ("fvit_attn_tc_fwd", "fvit_hat_attn_fwd"):
+                assert S <= 128, (hw, n, S)
+            if n == "fvit_attn_tc_bwd":
+                assert S <= 64, (hw, n, S)
+            if n in ("fvit_attn_loop_fwd", "fvit_attn_loop_bwd_long"):
+                assert S % 4 == 0, (hw, n, S)
+        assert carrier_s == n_ct, (hw, carrier_s, n_ct)
+        bias_fwd = {a[5]: (a[3], a[4]) for n, a in launches if n == "fvit_attn_bias_fwd"}
+        assert {(S, L) for S, L in bias_fwd.values() if S in n_ct} == {(s, 16) for s in n_ct}   # the 4 x 4 table
+        for n, a in launches:
+            if n == "fvit_attn_bias_bwd":
+                assert bias_fwd.get(a[1]) == (a[4], a[5]), (hw, bias_fwd.get(a[1]), a[4:6])
+    train = plans[1]
+    assert any(n == "fvit_token_init_nchw_bwd" for n, _ in _launches(train))
+    by_ptr = {t.data_ptr(): t for t in train.bufs.named.values()}
+    scatters = [a for n, a in _launches(train) if n == "fvit_scatter_add_rows"]
+    assert scatters, "the carriers' backward scatters them back"
+    for a in scatters:
+        mp = by_ptr[a[4]].flatten()[:a[5]]
+        valid = mp[mp >= 0]
+        assert valid.numel() == torch.unique(valid).numel(), (hw, "map repeats a destination row")
 
 
 def test_classification_geometry_is_unchanged():

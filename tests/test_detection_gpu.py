@@ -2,10 +2,14 @@
 goldens of the unmodified reference module at every golden shape (224^2, a carrier grid smaller than the bias table,
 non-square and odd sizes, 160 carriers on the key-loop attention), and a shape sweep under the plan-cache bound."""
 import gc
+import sys
 from pathlib import Path
 
 import pytest
 import torch
+
+sys.path.insert(0, str(Path(__file__).resolve().parent))   # tests/_token_init.py
+from _token_init import detr_shapes  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 GOLDEN = Path(__file__).parent / "golden"
@@ -50,21 +54,6 @@ def test_level_maps_match_the_reference_at_every_shape(case):
             assert torch.equal(o.mask.cpu(), ref["masks"][k]), (H, W, k)
 
 
-def _detr_shapes(n, seed=0):
-    """(H, W) of n distinct batches of DETR's multi-scale training augmentation: short side from 480..800 in steps of
-    32, long side capped at 1333, a random aspect ratio per batch (rounded to multiples of 4 to keep the sweep short)"""
-    g = torch.Generator().manual_seed(seed)
-    shapes = []
-    while len(shapes) < n:
-        s = 480 + 32 * int(torch.randint(0, 11, (1,), generator=g))
-        r = 1.0 + float(torch.rand(1, generator=g)) * 0.8
-        long = min(int(s * r), 1333)
-        hw = (s // 4 * 4, long // 4 * 4) if torch.rand(1, generator=g) < 0.5 else (long // 4 * 4, s // 4 * 4)
-        if hw not in shapes:
-            shapes.append(hw)
-    return shapes
-
-
 def test_shape_sweep_under_the_plan_cache_bound():
     from fastervit_b200.detection import build_fastervit
     from oracle import fastervit_oracle as O
@@ -72,7 +61,7 @@ def test_shape_sweep_under_the_plan_cache_bound():
                           num_heads=[1, 2, 4, 8])
     O.synth_fill_(det.state_dict(), 3)
     det = det.cuda().eval()
-    shapes = _detr_shapes(10)
+    shapes = detr_shapes(10)
     xs = {hw: O.synth_input(1, list(hw), 7, torch.float32).cuda() for hw in shapes}
     gc.collect()     # (earlier tests' models: a model and its engine reference each other)
     torch.cuda.synchronize()
@@ -118,12 +107,16 @@ def _rel_l2(a, b, floor):
 @pytest.mark.parametrize("case", ["det_tiny_fv0", "det_tiny_fv4", "det_tiny_21k"])
 def test_train_mode_matches_the_reference(case):
     """train mode at 96 x 160 (window-padded conv levels, 8 carriers: the cropped bias table) and 320 x 480 (non-square
-    carrier grid), frozen_stages -1 and 2: the normed maps, every BatchNorm's running statistics after the step, and the
-    parameter gradients of loss = sum_k <map_k, G_k> against the reference's fp64 train step"""
+    carrier grid), frozen_stages -1 and 2, and at the DETR training sizes of <case>_detr.pt, 480 x 544 and 544 x 800 (100
+    and 160 carriers: the key-loop attention, one and two key tiles; pools of kernel 8 x 8 and 8 x 11 on the fallback
+    tokenizer backward): the normed maps, every BatchNorm's running statistics after the step, and the parameter
+    gradients of loss = sum_k <map_k, G_k> against the reference's fp64 train step"""
     from fastervit_b200.detection import build_fastervit
     from oracle import fastervit_oracle as O
     g = torch.load(GOLDEN / f"{case}.pt", weights_only=False)
-    for (H, W, fs), ref in g["train"].items():
+    train = g["train"] | torch.load(GOLDEN / f"{case}_detr.pt", weights_only=False)["train"]
+    assert len(train) == 5
+    for (H, W, fs), ref in train.items():
         det = build_fastervit(g["name"], out_indices=(0, 1, 2, 3), drop_path_rate=0.0, frozen_stages=fs, **g["kwargs"])
         O.synth_fill_(det.state_dict(), g["seeds"]["w"])
         det = det.cuda().train()

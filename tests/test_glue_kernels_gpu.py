@@ -5,9 +5,14 @@ counts that are not multiples of the block or vector width, maps containing -1, 
 the fp32 / fp16 values the launch lists pass, so the tolerances cover fp32 arithmetic only (`_close` as in
 test_train_ops_gpu.py)."""
 import math
+import sys
+from pathlib import Path
 
 import pytest
 import torch
+
+sys.path.insert(0, str(Path(__file__).resolve().parent))   # tests/_token_init.py
+from _token_init import token_init_problem  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -462,10 +467,13 @@ def test_headpad_vec_and_unpad_heads_round_trip():
 
 
 # ------------------------------------------------------------------------------------------ attention bias
-@pytest.mark.parametrize("S,L_", [(49, 49), (53, 49), (148, 144)])
+@pytest.mark.parametrize("S,L_", [(49, 49), (53, 49), (148, 144), (4, 16), (8, 16), (36, 64)])
 def test_attn_bias_fwd_bwd(S, L_):
     """bias[h][r][c] = 16 sigmoid(table[index[(r-ng)*L + (c-ng)]][h]) for r, c >= ng = S - L, else 0; the backward
-    accumulates repeated index entries with the device scalar, carrier rows / columns contribute nothing."""
+    accumulates repeated index entries with the device scalar, carrier rows / columns contribute nothing. S < L (the
+    detection backbone's carrier grid smaller than the table it was built with) is F.pad with negative amounts
+    (dino/models/dino/fastervit.py:132): the bottom-right S x S block of the table, the cropped entries get no
+    gradient."""
     L = _L()
     g = _g(S + L_)
     heads, ntab = 4, 2 * L_
@@ -476,11 +484,13 @@ def test_attn_bias_fwd_bwd(S, L_):
     torch.cuda.synchronize()
     ng = S - L_
     td = table.double().requires_grad_(True)
-    full = torch.zeros(heads, S, S, dtype=torch.float64, device="cuda")
     inner = 16 * torch.sigmoid(td[index].view(L_, L_, heads).permute(2, 0, 1))
-    full[:, ng:, ng:] = inner
+    full = torch.nn.functional.pad(inner, (ng, 0, ng, 0))
     _close(bias, full.detach(), 1e-6, "bias fwd")
-    assert (bias[:, :ng] == 0).all() and (bias[:, :, :ng] == 0).all()
+    if ng > 0:
+        assert (bias[:, :ng] == 0).all() and (bias[:, :, :ng] == 0).all()
+    else:
+        assert torch.equal(full.detach(), inner.detach()[:, -ng:, -ng:])
     dbias = torch.randn(heads, S, S, device="cuda", generator=g)
     full.backward(dbias.double())
     dt = torch.randn(ntab, heads, device="cuda", generator=g)
@@ -547,27 +557,9 @@ def test_ln_fwd_maps_posadd_writeback(C, eps):
 
 # ------------------------------------------------------------------------------------------ carrier tokens
 # (Hp, Wp, kh, kw, sh, sw): the fv 14 x 14 / ct 2 windowing (k5 s3 -> 4 x 4), a non-square any-res map with
-# non-overlapping windows, and a map larger than the backward's shared-memory tile (its fallback kernel)
-TOKEN_INIT_CASES = [(14, 14, 5, 5, 3, 3), (10, 21, 5, 7, 5, 7), (24, 30, 6, 6, 6, 6)]
-
-
-def _token_init_problem(g, B, Hp, Wp, C, kh, kw, sh, sw):
-    oh, ow = (Hp - kh) // sh + 1, (Wp - kw) // sw + 1
-    npix = B * Hp * Wp
-    total = npix + 17
-    pix_map = torch.randperm(total, device="cuda", generator=g)[:npix].int()
-    pad = torch.rand(npix, device="cuda", generator=g) < 0.15        # padding pixels of an any-res map read as zero
-    pix_map[pad] = -1
-    xs = torch.randn(total, C + 4, device="cuda", generator=g)
-    xmap = torch.zeros(npix, C, dtype=torch.float64, device="cuda")
-    xmap[~pad] = xs[pix_map[~pad].long(), :C].double()
-    xmap = xmap.view(B, Hp, Wp, C).permute(0, 3, 1, 2)
-    w = torch.randn(C, 1, 3, 3, device="cuda", generator=g) * 0.3
-    bias = torch.randn(C, device="cuda", generator=g) * 0.1
-    nct = B * oh * ow
-    ct_rows = (torch.randperm(nct + 9, device="cuda", generator=g)[:nct]).int()
-    return dict(oh=oh, ow=ow, npix=npix, total=total, pix_map=pix_map, pad=pad, xs=xs, xmap=xmap, w=w, bias=bias,
-                nct=nct, ct_rows=ct_rows)
+# non-overlapping windows, a map larger than the backward's shared-memory tile (its fallback kernel), and a DETR-size
+# level-2 map on the fallback kernel whose pools overlap (one conv pixel feeds up to 3 x 4 pooled outputs)
+TOKEN_INIT_CASES = [(14, 14, 5, 5, 3, 3), (10, 21, 5, 7, 5, 7), (24, 30, 6, 6, 6, 6), (35, 56, 8, 11, 3, 3)]
 
 
 @pytest.mark.parametrize("Hp,Wp,kh,kw,sh,sw", TOKEN_INIT_CASES)
@@ -576,7 +568,7 @@ def test_token_init_fwd(Hp, Wp, kh, kw, sh, sw):
     zero pixel); carrier rows outside ct_row_map keep their sentinels."""
     L = _L()
     B, C = 2, 40
-    P = _token_init_problem(_g(Hp * Wp + kh), B, Hp, Wp, C, kh, kw, sh, sw)
+    P = token_init_problem(_g(Hp * Wp + kh), B, Hp, Wp, C, kh, kw, sh, sw)
     ldo = C + 8
     out = torch.full((P["nct"] + 9, ldo), 7.0, device="cuda")
     L.call("fvit_token_init_fwd", P["xs"].data_ptr(), C + 4, P["pix_map"].data_ptr(), B, Hp, Wp, C, P["w"].data_ptr(),
@@ -600,7 +592,7 @@ def test_token_init_bwd_non_square_and_padding_pixels(Hp, Wp, kh, kw, sh, sw):
     write nothing), dw, dbias against autograd of the forward above."""
     L = _L()
     B, C = 2, 40
-    P = _token_init_problem(_g(7 * Hp * Wp + kw), B, Hp, Wp, C, kh, kw, sh, sw)
+    P = token_init_problem(_g(7 * Hp * Wp + kw), B, Hp, Wp, C, kh, kw, sh, sw)
     x16 = P["xs"].half()
     xmap = torch.zeros(P["npix"], C, dtype=torch.float64, device="cuda")
     keep = ~P["pad"]
