@@ -159,6 +159,179 @@ feature_map_eval_bwd_apply_kernel(const float* __restrict__ dy, const int* __res
     if (row[k] >= 0) g[row[k] * ldg + c] = gv[k] + k1 * tile[threadIdx.x][threadIdx.y + 8 * k];
 }
 
+// ---- channel LayerNorm outputs (timm LayerNorm2d: per pixel over C, no statistics across pixels)
+// A block = (32, 8) threads takes 32 pixels t0 .. t0+31 of one image. Thread (x, y) owns pixels y + 8k (k < 4) and sweeps
+// the channels in 32-wide slabs with the channel along the lane: the token rows are read coalesced, and the per-pixel
+// sums over C are lane reductions of the warp that owns the pixel, so mean / rstd end up in that warp's registers.
+// The NCHW side goes through a 32 x 32 shared tile, coalesced along t (as feature_map_bwd_apply_kernel).
+// Statistics are moments about a per-pixel pivot (the pixel's channel 0): the level rows carry large per-channel
+// offsets, and E[x^2] - E[x]^2 about 0 would cancel.
+__device__ __forceinline__ long long ln_row(const int* __restrict__ row_map, int b, int T, int t) {
+  return row_map ? (long long)row_map[(long long)b * T + t] : (long long)b * T + t;
+}
+
+__global__ void __launch_bounds__(256)
+feature_map_ln_fwd_kernel(const float* __restrict__ xs, long long ldx, const int* __restrict__ row_map, int T, int C,
+                          const float* __restrict__ w, const float* __restrict__ bias, float eps,
+                          float* __restrict__ out, float* __restrict__ mean_out, float* __restrict__ rstd_out) {
+  __shared__ float tile[32][33];
+  const int b = blockIdx.y, t0 = blockIdx.x * 32, lane = threadIdx.x;
+  long long row[4];
+  float piv[4], s1[4], s2[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int t = t0 + threadIdx.y + 8 * k;
+    row[k] = t < T ? ln_row(row_map, b, T, t) : -1;
+    piv[k] = row[k] >= 0 ? __ldg(xs + row[k] * ldx) : 0.f;
+    s1[k] = s2[k] = 0.f;
+  }
+  for (int c0 = 0; c0 < C; c0 += 32) {
+    const int c = c0 + lane;
+    if (c >= C) break;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (row[k] < 0) continue;
+      const float d = xs[row[k] * ldx + c] - piv[k];
+      s1[k] += d;
+      s2[k] = fmaf(d, d, s2[k]);
+    }
+  }
+  float m1[4], rs[4];   // (x - mean = (x - pivot) - m1: both differences stay small next to the offsets)
+  const float inv_c = 1.f / (float)C;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      s1[k] += __shfl_xor_sync(0xffffffffu, s1[k], o);
+      s2[k] += __shfl_xor_sync(0xffffffffu, s2[k], o);
+    }
+    m1[k] = s1[k] * inv_c;
+    rs[k] = rsqrtf(fmaxf(s2[k] * inv_c - m1[k] * m1[k], 0.f) + eps);
+    if (lane == 0 && row[k] >= 0) {
+      const long long p = (long long)b * T + t0 + threadIdx.y + 8 * k;
+      if (mean_out) mean_out[p] = piv[k] + m1[k];
+      if (rstd_out) rstd_out[p] = rs[k];
+    }
+  }
+  for (int c0 = 0; c0 < C; c0 += 32) {
+    const int c = c0 + lane;
+    if (c < C) {
+      const float wc = __ldg(w + c), bc = __ldg(bias + c);
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        tile[lane][threadIdx.y + 8 * k] =
+            row[k] >= 0 ? fmaf((xs[row[k] * ldx + c] - piv[k] - m1[k]) * rs[k], wc, bc) : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int cc = c0 + threadIdx.y + 8 * k, t = t0 + lane;
+      if (cc < C && t < T) out[((long long)b * C + cc) * T + t] = tile[threadIdx.y + 8 * k][lane];
+    }
+    __syncthreads();
+  }
+}
+
+// Backward, grid-strided over (image, 32-pixel tile) items by one wave of blocks. Per item: pass 1 stages each dy slab
+// [c][t] (coalesced NCHW reads), reads the x slab along c and gathers the per-pixel sums of w*dy and w*dy*xhat (lane
+// reductions) and, with dw, the per-channel sums of dy*xhat and dy (shared-memory accumulators over every item of
+// the block, one global atomic per channel at the end). Pass 2 re-reads the slabs (L2-resident: the block just read
+// them) and adds S * rstd * (w*dy - mean_c(w*dy) - xhat * mean_c(w*dy*xhat)) into g.
+__global__ void __launch_bounds__(256)
+feature_map_ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ xs, long long ldx,
+                          const int* __restrict__ row_map, int B, int T, int C, const float* __restrict__ mean,
+                          const float* __restrict__ rstd, const float* __restrict__ w, const float* __restrict__ gs,
+                          const float* __restrict__ scalar, float* __restrict__ g, long long ldg,
+                          float* __restrict__ dw, float* __restrict__ dbeta) {
+  extern __shared__ float acc[];   // [2][C] when dw: sum dy * xhat, sum dy
+  __shared__ float tile[32][33];
+  const int lane = threadIdx.x, ntt = (T + 31) / 32;
+  if (dw)
+    for (int i = threadIdx.y * 32 + lane; i < 2 * C; i += 256) acc[i] = 0.f;
+  __syncthreads();
+  const float S = g ? __ldg(gs) : 0.f;
+  const float inv_c = 1.f / (float)C;
+  for (long long item = blockIdx.x; item < (long long)B * ntt; item += gridDim.x) {
+    const int b = (int)(item / ntt), t0 = (int)(item % ntt) * 32;
+    long long row[4];
+    float mu[4], rs[4], a1[4], a2[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int t = t0 + threadIdx.y + 8 * k;
+      row[k] = t < T ? ln_row(row_map, b, T, t) : -1;
+      mu[k] = row[k] >= 0 ? __ldg(mean + (long long)b * T + t) : 0.f;
+      rs[k] = row[k] >= 0 ? __ldg(rstd + (long long)b * T + t) : 0.f;
+      a1[k] = a2[k] = 0.f;
+    }
+    for (int c0 = 0; c0 < C; c0 += 32) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const int cc = c0 + threadIdx.y + 8 * k, t = t0 + lane;
+        tile[threadIdx.y + 8 * k][lane] = (cc < C && t < T) ? dy[((long long)b * C + cc) * T + t] : 0.f;
+      }
+      __syncthreads();
+      const int c = c0 + lane;
+      if (c < C) {
+        const float wc = __ldg(w + c);
+        float cw = 0.f, cb = 0.f;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          if (row[k] < 0) continue;
+          const float d = tile[lane][threadIdx.y + 8 * k];
+          const float xh = (xs[row[k] * ldx + c] - mu[k]) * rs[k];
+          a1[k] = fmaf(wc, d, a1[k]);
+          a2[k] = fmaf(wc * d, xh, a2[k]);
+          cw = fmaf(d, xh, cw);
+          cb += d;
+        }
+        if (dw) {
+          atomicAdd(acc + c, cw);
+          atomicAdd(acc + C + c, cb);
+        }
+      }
+      __syncthreads();
+    }
+    if (!g) continue;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        a1[k] += __shfl_xor_sync(0xffffffffu, a1[k], o);
+        a2[k] += __shfl_xor_sync(0xffffffffu, a2[k], o);
+      }
+      a1[k] *= inv_c;
+      a2[k] *= inv_c;
+    }
+    for (int c0 = 0; c0 < C; c0 += 32) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const int cc = c0 + threadIdx.y + 8 * k, t = t0 + lane;
+        tile[threadIdx.y + 8 * k][lane] = (cc < C && t < T) ? dy[((long long)b * C + cc) * T + t] : 0.f;
+      }
+      __syncthreads();
+      const int c = c0 + lane;
+      if (c < C) {
+        const float wc = __ldg(w + c);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          if (row[k] < 0) continue;
+          const float xh = (xs[row[k] * ldx + c] - mu[k]) * rs[k];
+          const float dx = wc * tile[lane][threadIdx.y + 8 * k] - a1[k] - xh * a2[k];
+          g[row[k] * ldg + c] += S * rs[k] * dx;
+        }
+      }
+      __syncthreads();
+    }
+  }
+  if (!dw) return;
+  __syncthreads();
+  const float sc = scalar ? __ldg(scalar) : 1.f;
+  for (int i = threadIdx.y * 32 + lane; i < C; i += 256) {
+    atomicAdd(dw + i, acc[i] * sc);
+    atomicAdd(dbeta + i, acc[C + i] * sc);
+  }
+}
+
 // dw[c] += s2[c] * scalar, dbeta[c] += s1[c] * scalar
 __global__ void bn_affine_grad_kernel(const float* __restrict__ s1, const float* __restrict__ s2,
                                       const float* __restrict__ scalar, int C, float* __restrict__ dw,
@@ -310,6 +483,39 @@ int fvit_feature_map_eval_bwd(const float* dy, const int32_t* row_map, int32_t B
     return post_launch("bn_affine_grad_kernel");
   }
   return 0;
+}
+
+int fvit_feature_map_ln_fwd(const float* xs, int64_t ldx, const int32_t* row_map, int32_t B, int32_t T, int32_t C,
+                            const float* w, const float* b, float eps, float* out_nchw, float* mean, float* rstd,
+                            void* stream) {
+  FVIT_CHECK(xs && w && b && out_nchw && B > 0 && T > 0 && C > 0 && B <= 65535 && ldx >= C && eps >= 0.f,
+             "fvit_feature_map_ln_fwd: bad arguments");
+  FVIT_CHECK((mean == nullptr) == (rstd == nullptr), "fvit_feature_map_ln_fwd: mean and rstd come in pairs");
+  feature_map_ln_fwd_kernel<<<dim3((T + 31) / 32, B), dim3(32, 8), 0, (cudaStream_t)stream>>>(
+      xs, ldx, row_map, T, C, w, b, eps, out_nchw, mean, rstd);
+  return post_launch("feature_map_ln_fwd_kernel");
+}
+
+int fvit_feature_map_ln_bwd(const float* dy, const float* xs, int64_t ldx, const int32_t* row_map, int32_t B,
+                            int32_t T, int32_t C, const float* mean, const float* rstd, const float* w, const float* gs,
+                            const float* scalar, float* g, int64_t ldg, float* dw, float* dbeta, void* stream) {
+  FVIT_CHECK(dy && xs && mean && rstd && w && B > 0 && T > 0 && C > 0 && ldx >= C,
+             "fvit_feature_map_ln_bwd: bad arguments");
+  FVIT_CHECK(!g || (gs && ldg >= C), "fvit_feature_map_ln_bwd: the input gradient needs gs and ldg >= C");
+  FVIT_CHECK((dw == nullptr) == (dbeta == nullptr), "fvit_feature_map_ln_bwd: dw / dbeta come in pairs");
+  FVIT_CHECK(2LL * C * 4 <= 48 * 1024, "fvit_feature_map_ln_bwd: C above 6144");
+  if (!g && !dw) return 0;
+  const size_t smem = dw ? 2 * (size_t)C * sizeof(float) : 0;
+  // one wave of resident blocks, grid-strided over the (image, 32-pixel tile) items (feature_map_bwd_stats_kernel)
+  int per_sm = 0;
+  FVIT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, feature_map_ln_bwd_kernel, 256, smem));
+  if (per_sm < 1) per_sm = 1;
+  const long long items = (long long)B * ((T + 31) / 32);
+  long long gx = (long long)num_sms() * per_sm;
+  if (gx > items) gx = items;
+  feature_map_ln_bwd_kernel<<<(unsigned)gx, dim3(32, 8), smem, (cudaStream_t)stream>>>(
+      dy, xs, ldx, row_map, B, T, C, mean, rstd, w, gs, scalar, g, ldg, dw, dbeta);
+  return post_launch("feature_map_ln_bwd_kernel");
 }
 
 int fvit_head_eval_bwd(const float* dlogits, int64_t ldl, int32_t B, int32_t ncls, const float* feats, int32_t C,

@@ -131,8 +131,11 @@ class FasterViTDet(FasterViT):
                               "under torch.no_grad() (or with every parameter frozen)")
         if any(getattr(m, "deploy", False) for m in self.modules()):
             raise L.FvitError("deploy mode is not supported by the detection backbone")
-        norms = [getattr(self, f"norm{i}") for i in self.out_indices]
+        norms = [self._level_norm(i) for i in self.out_indices]
         return self._get_engine().forward_levels(x, self.out_indices, norms=norms, frozen_stages=self.frozen_stages)
+
+    def _level_norm(self, i: int) -> nn.Module:
+        return getattr(self, f"norm{i}")
 
     def forward(self, tensor_list):
         """{k: type(tensor_list)(map_k, mask resized to map_k)} for the k-th out index

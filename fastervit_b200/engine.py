@@ -36,6 +36,36 @@ def P(t):
     return None if t is None else t.data_ptr()
 
 
+def norm_kind(m) -> str:
+    """What a 2-D norm module computes, judged by what it is (callers bring their own classes):
+    "bn"     nn.BatchNorm2d: batch statistics in train mode, running statistics in eval mode;
+    "frozen" a fixed affine from running statistics: buffers weight / bias / running_mean / running_var, an eps and no
+             parameters (torchvision.ops.FrozenBatchNorm2d, DETR-family copies of it);
+    "ln"     a per-pixel LayerNorm over the channels (timm LayerNorm2d): an nn.LayerNorm subclass over one dimension
+             with an elementwise affine and a bias.
+    Anything else raises FvitError."""
+    if isinstance(m, nn.BatchNorm2d):
+        return "bn"
+    bufs = dict(m.named_buffers(recurse=False))
+    if (not any(True for _ in m.parameters()) and isinstance(getattr(m, "eps", None), float)
+            and all(isinstance(bufs.get(n), torch.Tensor) and bufs[n].dim() == 1
+                    for n in ("weight", "bias", "running_mean", "running_var"))):
+        return "frozen"
+    if (isinstance(m, nn.LayerNorm) and type(m) is not nn.LayerNorm and len(m.normalized_shape) == 1
+            and m.elementwise_affine and m.weight is not None and m.bias is not None):
+        return "ln"
+    raise L.FvitError(f"unsupported norm {type(m).__name__}: accepted are nn.BatchNorm2d, a frozen BatchNorm (buffers "
+                      "weight / bias / running_mean / running_var, an eps, no parameters) and a channel LayerNorm "
+                      "(an nn.LayerNorm subclass such as timm's LayerNorm2d, one normalized dimension, affine, with a "
+                      "bias)")
+
+
+def norm_params(m) -> tuple:
+    """the trainable tensors of a level norm (None: a raw output): weight and bias of a BatchNorm2d or a channel
+    LayerNorm, none for a frozen BatchNorm"""
+    return () if m is None or norm_kind(m) == "frozen" else (m.weight, m.bias)
+
+
 # ---------------------------------------------------------------------------------- index maps
 def _ct_dewindow_perm(cs: int, sr: list[int]) -> torch.Tensor:
     """raster position r -> window-major carrier index it is read from; the literal index algebra of
@@ -385,7 +415,7 @@ class Plan:
             if level.downsample is not None:
                 Hc, Wc, Cc = (Hc + 1) // 2, (Wc + 1) // 2, Cc * 2
         self.feat = prev
-        if getattr(m, "norm", None) is None:   # the detection backbone: level maps only, no classifier tail
+        if getattr(m, "head", None) is None:   # the downstream backbones: level maps only, no classifier tail
             self.pooled = self.logits = None
             return
         # ---------------- head: BN folded into the average pool, then the classifier GEMM
@@ -1082,7 +1112,7 @@ class Engine:
             if bn is None:
                 continue
             for name in ("weight", "bias", "running_mean", "running_var"):
-                t = getattr(bn, name)
+                t = getattr(bn, name, None)   # (a channel LayerNorm has no running statistics)
                 if t is None:
                     continue
                 if t.dtype != torch.float32 or not t.is_contiguous():
@@ -1220,7 +1250,7 @@ class Engine:
         params = list(self._params)
         known = {id(p) for p in params}
         for _, bn in outs:
-            for p in (() if bn is None else (bn.weight, bn.bias)):
+            for p in norm_params(bn):
                 if id(p) not in known:
                     known.add(id(p))
                     params.append(p)
@@ -1242,8 +1272,16 @@ class Engine:
             if bn is None:
                 res.append(f)
                 continue
-            # the level norm folded into the layout-conversion kernel, running statistics (fastervit.py:816-827)
             B, C, H, W = f.shape
+            if norm_kind(bn) == "ln":   # a channel LayerNorm: the same kernel as in train mode, no statistics saved
+                rows = f.permute(0, 2, 3, 1).reshape(B * H * W, C).contiguous()
+                out = torch.empty(B, C, H, W, dtype=torch.float32, device=f.device)
+                with torch.cuda.device(f.device):
+                    L.call("fvit_feature_map_ln_fwd", rows.data_ptr(), C, None, B, H * W, C, bn.weight.data_ptr(),
+                           bn.bias.data_ptr(), float(bn.eps), out.data_ptr(), None, None)
+                res.append(out)
+                continue
+            # the level norm folded into the layout-conversion kernel, running statistics (fastervit.py:816-827)
             scale = (bn.weight * torch.rsqrt(bn.running_var + bn.eps)).float().contiguous()
             shift = (bn.bias - bn.running_mean * scale).float().contiguous()
             rows = f.permute(0, 2, 3, 1).reshape(B * H * W, C).contiguous()     # token-major view of the level output

@@ -19,14 +19,14 @@ import os
 import torch
 
 from . import lib as L
-from .engine import Plan, _ru
+from .engine import Plan, _ru, norm_kind, norm_params
 from .engine_train_conv import ConvPartEmitters
 from .engine_train_levels import _ONE, TokenLevelEmitters
 
 
 def levels_path(model, outs) -> set[int]:
-    """ids of the parameters the level outputs `outs` ((level, BatchNorm2d or None), ...) depend on: the stem, the levels
-    up to the highest requested one without its Downsample, and the level norms"""
+    """ids of the parameters the level outputs `outs` ((level, norm or None), ...) depend on: the stem, the levels up to
+    the highest requested one without its Downsample, and the level norms' weights and biases (engine.norm_params)"""
     stop = max(i for i, _ in outs)
     on = set()
     for name, p in model.named_parameters():
@@ -37,8 +37,7 @@ def levels_path(model, outs) -> set[int]:
         elif name.startswith("patch_embed."):
             on.add(id(p))
     for _, bn in outs:
-        if bn is not None:
-            on.update((id(bn.weight), id(bn.bias)))
+        on.update(map(id, norm_params(bn)))
     return on
 
 
@@ -84,8 +83,8 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         for i, bn in outs:
             if not 0 <= i < nlev:
                 raise L.FvitError(f"out index {i} is not a level of this model (0 .. {nlev - 1})")
-            if bn is not None and (not isinstance(bn, torch.nn.BatchNorm2d) or bn.weight is None
-                                   or bn.running_mean is None or bn.momentum is None):
+            if bn is not None and norm_kind(bn) == "bn" and (bn.weight is None or bn.running_mean is None
+                                                              or bn.momentum is None):
                 raise L.FvitError("level norms must be affine BatchNorm2d modules with running statistics and a momentum")
         self.stop_level = max(i for i, _ in outs) if self.kind == "levels" else nlev - 1
         fs = int(spec.get("frozen", -1)) if spec is not None else -1
@@ -94,6 +93,13 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         frozen_mods = ([model.patch_embed] if self.stem_frozen else []) + [model.levels[i] for i in range(self.n_frozen_lv)]
         self._frozen_bn = {id(b) for fm in ([model] if self.eval_grad else frozen_mods) for b in fm.modules()
                            if isinstance(b, torch.nn.BatchNorm2d)}
+        # frozen BatchNorms of the stem (the tracking backbone's FrozenBatchNorm2d): a fixed affine from running
+        # statistics in every mode, crossed by the data gradient alone, while the convolutions around them still train
+        stem_norms = (model.patch_embed.conv_down[1], model.patch_embed.conv_down[4])
+        if any(norm_kind(b) not in ("bn", "frozen") for b in stem_norms):
+            raise L.FvitError("the stem norms are BatchNorm2d or frozen BatchNorms")
+        self._fixed_bn = {id(b) for b in stem_norms if norm_kind(b) == "frozen"}
+        self._frozen_bn |= self._fixed_bn
         self._frozen_params = {id(p) for fm in frozen_mods for p in fm.parameters()}
         stages = [model.patch_embed, *model.levels]
         mask = spec.get("data_only") if spec is not None else None
@@ -119,7 +125,7 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
         # so that the data-parallel buckets reduce them too
         known = {id(p) for p in self.params}
         for _, bn in (self.spec or {}).get("outs", ()):
-            for p in (() if bn is None else (bn.weight, bn.bias)):
+            for p in norm_params(bn):
                 if id(p) not in known:
                     known.add(id(p))
                     self.params.append(p)
@@ -678,7 +684,8 @@ def _check_eval_backward(m, weights_changed: bool, recomputes: bool = True) -> N
 def _norm_versions(outs) -> tuple:
     """autograd versions of the level norms' tensors (the backbone's norm{i} are not part of the model's weights key)"""
     return tuple(t._version for _, bn in outs if bn is not None
-                 for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
+                 for t in (getattr(bn, n, None) for n in ("weight", "bias", "running_mean", "running_var"))
+                 if t is not None)
 
 
 class _EvalDenseGradFunction(torch.autograd.Function):

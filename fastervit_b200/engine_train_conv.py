@@ -19,8 +19,9 @@ from .engine import P, _ru
 
 def _bn_train(self, name: str, bn: nn.BatchNorm2d, count: int, ls=None) -> dict:
     """statistics accumulators + finalize launch; returns the saved vectors. A BatchNorm on running statistics (the
-    frozen prefix, an eval-mode plan) has no accumulators: its GEMM gets col_sum = col_sumsq = None."""
-    C = bn.num_features
+    frozen prefix, an eval-mode plan, a frozen BatchNorm of the stem) has no accumulators: its GEMM gets col_sum =
+    col_sumsq = None."""
+    C = bn.running_mean.numel()   # (a frozen BatchNorm need not have num_features)
     nb = self.bufs
     st = nb.new(name + ".stats", (2, C), torch.float32)
     frozen = id(bn) in self._frozen_bn
@@ -56,7 +57,7 @@ def _bn_finalize(self, d: dict, ls=None) -> None:
     bn = d["bn"]
     if id(bn) in self._frozen_bn:
         # frozen prefix (an eval()-ed module of the backbone, fastervit.py:801-812): running statistics, not updated
-        self._op(self.ops, "fvit_affine_fold", d["sc"].data_ptr(), d["sh"].data_ptr(), bn.num_features,
+        self._op(self.ops, "fvit_affine_fold", d["sc"].data_ptr(), d["sh"].data_ptr(), bn.running_mean.numel(),
                  bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
                  float(bn.eps), None, P(ls))
         return
@@ -251,10 +252,12 @@ def _bn_bwd(self, d: dict, gin, g_is_f16: int, ldg: int, g_rows, raw, ldr: int, 
             ldo: int, o_rows, row_scale=None, data_only=False) -> None:
     """BatchNorm2d backward of d (_bn_train) into fp16 rows `out`: batch statistics (fvit_bn_bwd), or the running
     statistics of an eval-mode plan (fvit_bn_eval_bwd: no mean(dy) terms, one pass). data_only (running statistics,
-    no stochastic depth: a frozen or eval stage): the streaming fvit_bn_eval_dgrad, dy times the forward's folded scale"""
+    no stochastic depth: a frozen or eval stage), or a frozen BatchNorm of the stem (no parameters; the convolutions
+    around it keep their weight gradients): the streaming fvit_bn_eval_dgrad, dy times the forward's folded scale"""
     bn = d["bn"]
-    if data_only:
-        self._op(self.bwd_ops, "fvit_bn_eval_dgrad", gin, g_is_f16, ldg, g_rows, raw, ldr, r_rows, nrows, bn.num_features,
+    if data_only or id(bn) in self._fixed_bn:
+        self._op(self.bwd_ops, "fvit_bn_eval_dgrad", gin, g_is_f16, ldg, g_rows, raw, ldr, r_rows, nrows,
+                 bn.running_mean.numel(),
                  d["sc"].data_ptr(), d["sh"].data_ptr(), act, None, None, out, ldo, o_rows)
         return
     if self.eval_grad:

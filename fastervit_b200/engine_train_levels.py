@@ -9,7 +9,7 @@ import torch
 import torch.nn as nn
 
 from . import lib as L
-from .engine import P, _ru
+from .engine import P, _ru, norm_kind
 
 
 def _drop_buf(self, name: str, rate: float, groups: int, group_size: int):
@@ -96,10 +96,13 @@ def _emit_dense_outputs(self) -> None:
     """Levels mode forward tail: every requested level output (x before its Downsample, live in the level's buffer
     until the plan's next forward: the backward never writes it) as an NCHW fp32 map in a static buffer, through its
     BatchNorm2d with batch statistics (fvit_colstats_pivot_f32 -> fvit_bn_finalize_pivot, which also updates the running
-    statistics -> fvit_feature_map_fwd), or raw.
+    statistics -> fvit_feature_map_fwd), through a frozen BatchNorm (fvit_affine_fold of its running statistics ->
+    fvit_feature_map_fwd), through a channel LayerNorm (fvit_feature_map_ln_fwd, which saves the per-pixel mean / rstd),
+    or raw.
     Eval plan (engine_train._EvalDenseGradFunction): the outputs come from the inference launch list, so this forward
-    writes no output map; it only keeps each norm's running mean / rstd for the backward's xhat (one fvit_affine_fold
-    with unit weight and zero bias: rstd = rsqrt(running_var + eps), nothing updated)."""
+    writes no BatchNorm output map; it only keeps each norm's running mean / rstd for the backward's xhat (one
+    fvit_affine_fold with unit weight and zero bias: rstd = rsqrt(running_var + eps), nothing updated). Frozen
+    BatchNorms and LayerNorms run as in train mode (their math does not depend on it)."""
     B, nb = self.B, self.bufs
     self.dense, self.outputs = [], []
     tot = 1
@@ -109,11 +112,36 @@ def _emit_dense_outputs(self) -> None:
         C, H, W = lv["C"], lv["H"], lv["W"]
         T = H * W
         out = None if self.eval_grad else nb.new(f"dense.out{k}", (B, C, H, W), torch.float32)
-        d = dict(level=i, lv=lv, x=x, rows=rows, C=C, T=T, bn=bn, out=out,
+        kind = None if bn is None else norm_kind(bn)
+        d = dict(level=i, lv=lv, x=x, rows=rows, C=C, T=T, bn=bn if kind == "bn" else None, norm=bn, kind=kind, out=out,
                  dy=nb.new(f"dense.dy{k}", (B, C, H, W), torch.float32), acc=tot)
         tot += 2 * _ru(C, 4)
-        if bn is not None and bn.num_features != C:
-            raise L.FvitError(f"the norm of level {i} has {bn.num_features} features, the level has {C} channels")
+        if bn is not None and bn.weight.numel() != C:
+            raise L.FvitError(f"the norm of level {i} has {bn.weight.numel()} features, the level has {C} channels")
+        if kind in ("frozen", "ln"):
+            if out is None:
+                out = nb.new(f"dense.out{k}", (B, C, H, W), torch.float32)
+            if kind == "frozen":   # running statistics, never written
+                sc = nb.new(f"dense.norm{k}.scale", (C,), torch.float32)
+                sh = nb.new(f"dense.norm{k}.shift", (C,), torch.float32)
+                self._op(self.ops, "fvit_affine_fold", sc.data_ptr(), sh.data_ptr(), C, bn.weight.data_ptr(),
+                         bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(), float(bn.eps), None,
+                         None)
+                self._op(self.ops, "fvit_feature_map_fwd", x.data_ptr(), C, rows.data_ptr(), B, T, C, sc.data_ptr(),
+                         sh.data_ptr(), out.data_ptr())
+                d.update(sc=sc, mu=None, rs=None)
+            else:
+                mu = nb.new(f"dense.norm{k}.pmean", (B * T,), torch.float32)
+                rs = nb.new(f"dense.norm{k}.prstd", (B * T,), torch.float32)
+                self._op(self.ops, "fvit_feature_map_ln_fwd", x.data_ptr(), C, rows.data_ptr(), B, T, C,
+                         bn.weight.data_ptr(), bn.bias.data_ptr(), float(bn.eps), out.data_ptr(), mu.data_ptr(),
+                         rs.data_ptr())
+                d.update(mu=None, rs=None, pmean=mu, prstd=rs)
+            d["out"] = out
+            self.dense.append(d)
+            if not self.eval_grad:
+                self.outputs.append(out)
+            continue
         if self.eval_grad:
             if bn is not None:
                 rs = nb.new(f"dense.norm{k}.rstd", (C,), torch.float32)
@@ -161,6 +189,19 @@ def _inject(self, level: int, g=True) -> None:
         if d["level"] != level:
             continue
         bn, lv = d["bn"], d["lv"]
+        if d["kind"] == "ln":   # per-pixel statistics: the same backward in train and eval mode
+            ln = d["norm"]
+            self._op(self.bwd_ops, "fvit_feature_map_ln_bwd", d["dy"].data_ptr(), d["x"].data_ptr(), d["C"],
+                     d["rows"].data_ptr(), self.B, d["T"], d["C"], d["pmean"].data_ptr(), d["prstd"].data_ptr(),
+                     ln.weight.data_ptr(), ("scal", 0), None, lv["g"].data_ptr() if g else None, d["C"],
+                     self.G(ln.weight), self.G(ln.bias))
+            continue
+        if d["kind"] == "frozen":   # a fixed per-channel scale of dy, no parameters
+            if g:
+                self._op(self.bwd_ops, "fvit_feature_map_eval_bwd", d["dy"].data_ptr(), d["rows"].data_ptr(), self.B,
+                         d["T"], d["C"], d["sc"].data_ptr(), _const_vec(self, 1.0, d["C"]).data_ptr(), None, None,
+                         ("scal", 0), None, lv["g"].data_ptr(), d["C"], None, None)
+            continue
         if bn is None and not g:
             continue
         if self.eval_grad:   # running statistics: a per-channel scale of dy, and dw / dbeta straight from the stats pass

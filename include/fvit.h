@@ -330,6 +330,21 @@ int fvit_grad_scale_finalize(const float* amax, float target, float* gs, void* s
 int fvit_feature_map_eval_bwd(const float* dy, const int32_t* row_map, int32_t B, int32_t T, int32_t C,
                               const float* rstd, const float* w, const float* s1, const float* s2, const float* gs,
                               const float* scalar, float* g, int64_t ldg, float* dw, float* dbeta, void* stream);
+/* Level outputs through a channel LayerNorm (timm LayerNorm2d, the MOTRv2 tracking backbone's output norms), in train
+ * and eval mode alike. Pixel p = b*T + t reads the fp32 row xs[row_map[p]] (row_map NULL: row p; row stride ldx >= C).
+ * fvit_feature_map_ln_fwd: out[b][c][t] = (x[c] - mean_p) * rstd_p * w[c] + b[c] with mean_p / rstd_p =
+ *   rsqrt(var_p + eps) over the C channels of the pixel (biased variance, fp32, moments about the pixel's channel 0);
+ *   mean[p], rstd[p] are written when given (both or neither: NULL in inference).
+ * fvit_feature_map_ln_bwd: from the NCHW map gradient dy and the forward's mean / rstd, with xhat = (x - mean_p) * rstd_p:
+ *   g[row_map[p]][c] += S * rstd_p * (w[c]*dy - mean_c(w*dy) - xhat * mean_c(w*dy*xhat)) (S = gs[0]; g NULL: none);
+ *   dw[c] += (*scalar) * sum_p dy * xhat, dbeta[c] += (*scalar) * sum_p dy (both or neither; scalar NULL = 1), summed
+ *   with float atomics. C <= 6144. */
+int fvit_feature_map_ln_fwd(const float* xs, int64_t ldx, const int32_t* row_map, int32_t B, int32_t T, int32_t C,
+                            const float* w, const float* b, float eps, float* out_nchw, float* mean, float* rstd,
+                            void* stream);
+int fvit_feature_map_ln_bwd(const float* dy, const float* xs, int64_t ldx, const int32_t* row_map, int32_t B,
+                            int32_t T, int32_t C, const float* mean, const float* rstd, const float* w, const float* gs,
+                            const float* scalar, float* g, int64_t ldg, float* dw, float* dbeta, void* stream);
 /* Backward of forward_head (faster_vit.py:955-958: AdaptiveAvgPool2d(1) + flatten + Linear), fp32 throughout, from
  * dlogits [B, ncls] (row stride ldl). feats: the fp32 input, NCHW [B, C, T] (T = H*W) or pooled [B, C] (T = 1).
  * dfeats[b][c][t] = (sum_k dlogits[b][k] * W[k][c]) / T (written); dW[k][c] += sum_b dlogits[b][k] * pooled[b][c] with
