@@ -186,22 +186,23 @@ __device__ __forceinline__ int colsum16_owner_col(int lane) {
 // Epilogue specialisation: GENERIC = every option decided at run time (backward modes, statistics,
 // split-K atomics); otherwise ACT / RESID / O32 / O16 are compile-time and the unused paths vanish
 // (the epilogue is instruction-issue bound, so this is worth ~2.5x on short-K tiles).
-// FEAT: compile-time feature mask (see EF_* below); EF_GENERIC keeps every switch at run time.
+// FEAT: compile-time feature mask (the FVIT_GEMM_F_* bits of include/fvit.h); EF_GENERIC keeps every switch at run
+// time.
 enum : uint32_t {
-  EF_GENERIC = 1u << 0,
-  EF_ACT_SHIFT = 1,          // 3 bits: FVIT_ACT_* code
-  EF_RESID = 1u << 4,
-  EF_O32 = 1u << 5,
-  EF_O16 = 1u << 6,
-  EF_STATS = 1u << 7,
-  EF_PRE = 1u << 8,
-  EF_ATOMIC = 1u << 9,
-  EF_ALPHAPTR = 1u << 10,
-  EF_CS2 = 1u << 11,
-  EF_RS = 1u << 12,
-  EF_OSUM = 1u << 13,        // per-column sum of the rounded 16-bit output (bias gradient of the next layer)
-  EF_PREGRAD = 1u << 14,     // out_pre16 receives gelu'(v) (consumed by FVIT_ACT_MUL_AUX in the backward pass)
-  EF_DIRECT = 1u << 15,      // 16-bit outputs only: row-per-thread epilogue, 32-byte stores
+  EF_GENERIC = FVIT_GEMM_F_GENERIC,
+  EF_ACT_SHIFT = FVIT_GEMM_F_ACT_SHIFT,
+  EF_RESID = FVIT_GEMM_F_RESID,
+  EF_O32 = FVIT_GEMM_F_O32,
+  EF_O16 = FVIT_GEMM_F_O16,
+  EF_STATS = FVIT_GEMM_F_STATS,
+  EF_PRE = FVIT_GEMM_F_PRE,
+  EF_ATOMIC = FVIT_GEMM_F_ATOMIC,
+  EF_ALPHAPTR = FVIT_GEMM_F_ALPHAPTR,
+  EF_CS2 = FVIT_GEMM_F_CS2,
+  EF_RS = FVIT_GEMM_F_RS,
+  EF_OSUM = FVIT_GEMM_F_OSUM,        // per-column sum of the rounded 16-bit output (bias gradient of the next layer)
+  EF_PREGRAD = FVIT_GEMM_F_PREGRAD,  // out_pre16 receives gelu'(v) (consumed by FVIT_ACT_MUL_AUX in the backward pass)
+  EF_DIRECT = FVIT_GEMM_F_DIRECT,    // 16-bit outputs only: row-per-thread epilogue, 32-byte stores
 };
 // work unit -> (M tile, N tile, K split). Plain GEMMs keep the K splits of a tile adjacent; the tap-in-N mode
 // walks all tiles of one K range first so concurrently running CTAs share the A / B slices in L2.
@@ -951,10 +952,49 @@ static int get_tmap(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1
   return cached_tmap_16bit(out, base, rank, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
-}  // namespace fvit
+// The instantiated variants, one list for the launch table and for fvit_gemm_variants: the staging-tile epilogue
+// masks, then the masks that also have a row-per-thread (EF_DIRECT) form.
+#define FVIT_ACTF(x) ((uint32_t)(x) << EF_ACT_SHIFT)
+#define FVIT_GEMM_STAGED_VARIANTS(X)                                                                  \
+  /* inference / shared forward shapes */                                                            \
+  X(FVIT_ACTF(0) | EF_O16)                                  /* qkv */                                \
+  X(FVIT_ACTF(2) | EF_O16)                                  /* fc1, conv1 (eval) */                  \
+  X(FVIT_ACTF(1) | EF_O16)                                  /* stem conv1 (eval) */                  \
+  X(FVIT_ACTF(1) | EF_O32 | EF_O16)                         /* stem conv2 (eval) */                  \
+  X(FVIT_ACTF(0) | EF_RESID | EF_O32)                       /* proj, fc2, conv dgrad */              \
+  X(FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_O16)              /* conv2 (eval) */                       \
+  X(FVIT_ACTF(0) | EF_O32)                                  /* downsample, head */                   \
+  X(FVIT_ACTF(0) | EF_O32 | EF_O16)                         /* downsample -> next level */           \
+  /* training forward */                                                                             \
+  X(FVIT_ACTF(0) | EF_O16 | EF_STATS)                       /* raw conv + BN statistics */           \
+  X(FVIT_ACTF(2) | EF_O16 | EF_PRE)                         /* fc1 saving the pre-GELU value */      \
+  X(FVIT_ACTF(2) | EF_O16 | EF_PRE | EF_PREGRAD)            /* fc1 saving gelu' */                   \
+  X(FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_RS)               /* branch + stochastic depth */          \
+  X(FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_CS2 | EF_PRE)     /* branch with layer scale */            \
+  X(FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_CS2 | EF_PRE | EF_RS)  /* layer scale + stochastic depth */ \
+  /* backward */                                                                                     \
+  X(FVIT_ACTF(0) | EF_O32 | EF_ATOMIC | EF_ALPHAPTR)        /* wgrad split-K */                      \
+  X(FVIT_ACTF(0) | EF_O32 | EF_ALPHAPTR)                    /* wgrad single pass */                  \
+  X(FVIT_ACTF(0) | EF_O16 | EF_ALPHAPTR)                    /* dgrad */                              \
+  X(FVIT_ACTF(3) | EF_O16 | EF_ALPHAPTR)                    /* dgrad * gelu' */                      \
+  X(FVIT_ACTF(3) | EF_O16)                                  /* conv dgrad * gelu' */                 \
+  X(FVIT_ACTF(3) | EF_O16 | EF_ALPHAPTR | EF_OSUM)          /* fc2 dgrad * gelu' + fc1 bias grad */  \
+  X(FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR)                    /* fc2 dgrad * saved gelu' */            \
+  X(FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR | EF_OSUM)          /* ... + fc1 bias gradient */
+#define FVIT_GEMM_DIRECT_VARIANTS(X)                         \
+  X(FVIT_ACTF(0) | EF_O16)                                   \
+  X(FVIT_ACTF(1) | EF_O16)                                   \
+  X(FVIT_ACTF(2) | EF_O16)                                   \
+  X(FVIT_ACTF(2) | EF_O16 | EF_PRE | EF_PREGRAD)             \
+  X(FVIT_ACTF(0) | EF_O16 | EF_ALPHAPTR)                     \
+  X(FVIT_ACTF(3) | EF_O16)                                   \
+  X(FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR)                     \
+  X(FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR | EF_OSUM)
+#define FVIT_CASE(F) case (F):
 
-extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
-  using namespace fvit;
+// Argument validation and the kernel variant of one call: host only (no CUDA call, no device access), so the
+// variant of a launch can be queried on a machine without a GPU.
+static int select_variant(const fvit_gemm_args* a, uint32_t* variant) {
   FVIT_CHECK(a != nullptr, "fvit_gemm: null args");
   FVIT_CHECK(a->m > 0 && a->n > 0 && a->kc > 0, "fvit_gemm: bad dims m=%d n=%d kc=%d", a->m, a->n,
              a->kc);
@@ -983,6 +1023,90 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   FVIT_CHECK(a->tile_n == 0 || (a->tile_n >= 16 && a->tile_n <= 256 && a->tile_n % 16 == 0),
              "fvit_gemm: tile_n=%d invalid", a->tile_n);
   FVIT_CHECK(a->cta_group >= 0 && a->cta_group <= 2, "fvit_gemm: cta_group=%d invalid", a->cta_group);
+
+  // feature mask of this call: the matching specialisation if one was instantiated, else the generic kernel
+  const bool atomic_out = split_k > 1;
+  uint32_t feat = FVIT_ACTF(a->act);
+  if (a->resid && !atomic_out) feat |= EF_RESID;
+  if (a->out_f32) feat |= EF_O32;
+  if (a->out_f16) feat |= EF_O16;
+  if (a->col_sum) feat |= EF_STATS;
+  if (a->out_pre16) feat |= EF_PRE;
+  if (atomic_out) feat |= EF_ATOMIC;
+  if (a->alpha_ptr) feat |= EF_ALPHAPTR;
+  if (a->col_scale2) feat |= EF_CS2;
+  if (a->row_scale) feat |= EF_RS;
+  if (a->out_colsum) feat |= EF_OSUM;
+  if (a->pre_is_grad && a->out_pre16 && a->act == FVIT_ACT_GELU) feat |= EF_PREGRAD;
+  *variant = EF_GENERIC;
+  if (a->bf16) return 0;  // bf16 operands: only the generic kernel instantiates their MMAs
+  {
+    // row-per-thread epilogue (EF_DIRECT): 16-bit outputs only, everything a lane touches in 32-byte pieces
+    static int direct = -1;  // FVIT_GEMM_DIRECT=0: staging-tile epilogue everywhere (A/B)
+    if (direct < 0) {
+      const char* e = getenv("FVIT_GEMM_DIRECT");
+      direct = e ? atoi(e) : 1;
+    }
+    auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
+    const uint32_t allowed = EF_O16 | EF_PRE | EF_PREGRAD | EF_ALPHAPTR | EF_OSUM | (7u << EF_ACT_SHIFT);
+    const bool ok = direct && (feat & ~allowed) == 0 && (feat & EF_O16) && b_ntaps == 1 && a->n % 16 == 0 &&
+                    a->ld_out_f16 % 16 == 0 && al32(a->out_f16) &&
+                    (!a->out_pre16 || (a->ld_out_pre16 % 16 == 0 && al32(a->out_pre16))) &&
+                    (!a->aux || (a->ld_aux % 16 == 0 && al32(a->aux))) &&
+                    (!a->col_scale || (reinterpret_cast<uintptr_t>(a->col_scale) & 15) == 0) &&
+                    (!a->col_shift || (reinterpret_cast<uintptr_t>(a->col_shift) & 15) == 0) &&
+                    (!a->aux_scale || ((reinterpret_cast<uintptr_t>(a->aux_scale) & 15) == 0 &&
+                                       (reinterpret_cast<uintptr_t>(a->aux_shift) & 15) == 0));
+    if (ok) {
+      switch (feat) {  // the combinations with a direct specialisation
+        FVIT_GEMM_DIRECT_VARIANTS(FVIT_CASE)
+        feat |= EF_DIRECT;
+        break;
+        default:
+          break;
+      }
+    }
+  }
+#define FVIT_DIRECT_CASE(F) case EF_DIRECT | (F):
+  switch (feat) {
+    FVIT_GEMM_STAGED_VARIANTS(FVIT_CASE)
+    FVIT_GEMM_DIRECT_VARIANTS(FVIT_DIRECT_CASE)
+    *variant = feat;
+    break;
+    default:
+      break;
+  }
+#undef FVIT_DIRECT_CASE
+  return 0;
+}
+
+}  // namespace fvit
+
+extern "C" int fvit_gemm_variant(const fvit_gemm_args* a, uint32_t* variant) {
+  FVIT_CHECK(variant != nullptr, "fvit_gemm_variant: null variant");
+  return fvit::select_variant(a, variant);
+}
+
+extern "C" int fvit_gemm_variants(uint32_t* out, int cap) {
+  using namespace fvit;
+  int count = 0;
+#define FVIT_LIST(F) \
+  if (count < cap) out[count] = (F); \
+  ++count;
+#define FVIT_LIST_DIRECT(F) FVIT_LIST(EF_DIRECT | (F))
+  FVIT_GEMM_STAGED_VARIANTS(FVIT_LIST)
+  FVIT_GEMM_DIRECT_VARIANTS(FVIT_LIST_DIRECT)
+#undef FVIT_LIST_DIRECT
+#undef FVIT_LIST
+  return count;
+}
+
+extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
+  using namespace fvit;
+  uint32_t feat = 0;
+  if (const int rc = select_variant(a, &feat)) return rc;
+  const int b_ntaps = a->b_ntaps > 1 ? a->b_ntaps : 1;
+  const int split_k = a->split_k > 1 ? a->split_k : 1;
   const int sms = num_sms();
   // a requested width above the widest MMA is split into two equal tiles (multiples of 16)
   const int num_kb = ceil_div(a->kc, BK) * a->ntaps;
@@ -1108,54 +1232,6 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
       stages * stage_bytes + slab_bytes + SMEM_CTRL_BYTES + SMEM_ALIGN_SLACK + SMEM_ACC_BYTES + stats_bytes;
   const long long work = (long long)p.tiles_m * p.tiles_n * p.split_k;
   const int grid = (int)(work < sms ? work : sms);
-  // feature mask of this call; launch the matching specialisation if one was instantiated
-  uint32_t feat = ((uint32_t)a->act << EF_ACT_SHIFT);
-  if (a->resid && !p.atomic_out) feat |= EF_RESID;
-  if (a->out_f32) feat |= EF_O32;
-  if (a->out_f16) feat |= EF_O16;
-  if (a->col_sum) feat |= EF_STATS;
-  if (a->out_pre16) feat |= EF_PRE;
-  if (p.atomic_out) feat |= EF_ATOMIC;
-  if (a->alpha_ptr) feat |= EF_ALPHAPTR;
-  if (a->col_scale2) feat |= EF_CS2;
-  if (a->row_scale) feat |= EF_RS;
-  if (a->out_colsum) feat |= EF_OSUM;
-  if (p.pre_is_grad) feat |= EF_PREGRAD;
-  const bool needs_generic = a->bf16 != 0;  // bf16 operands: only the generic kernel instantiates their MMAs
-  {
-    // row-per-thread epilogue (EF_DIRECT): 16-bit outputs only, everything a lane touches in 32-byte pieces
-    static int direct = -1;  // FVIT_GEMM_DIRECT=0: staging-tile epilogue everywhere (A/B)
-    if (direct < 0) {
-      const char* e = getenv("FVIT_GEMM_DIRECT");
-      direct = e ? atoi(e) : 1;
-    }
-    auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
-    const uint32_t allowed = EF_O16 | EF_PRE | EF_PREGRAD | EF_ALPHAPTR | EF_OSUM | (7u << EF_ACT_SHIFT);
-    const bool ok = direct && (feat & ~allowed) == 0 && (feat & EF_O16) && b_ntaps == 1 && a->n % 16 == 0 &&
-                    a->ld_out_f16 % 16 == 0 && al32(a->out_f16) &&
-                    (!a->out_pre16 || (a->ld_out_pre16 % 16 == 0 && al32(a->out_pre16))) &&
-                    (!a->aux || (a->ld_aux % 16 == 0 && al32(a->aux))) &&
-                    (!a->col_scale || (reinterpret_cast<uintptr_t>(a->col_scale) & 15) == 0) &&
-                    (!a->col_shift || (reinterpret_cast<uintptr_t>(a->col_shift) & 15) == 0) &&
-                    (!a->aux_scale || ((reinterpret_cast<uintptr_t>(a->aux_scale) & 15) == 0 &&
-                                       (reinterpret_cast<uintptr_t>(a->aux_shift) & 15) == 0));
-    if (ok) {
-      switch (feat) {   // the combinations with a direct specialisation (launch table below)
-        case (0u << EF_ACT_SHIFT) | EF_O16:
-        case (1u << EF_ACT_SHIFT) | EF_O16:
-        case (2u << EF_ACT_SHIFT) | EF_O16:
-        case (2u << EF_ACT_SHIFT) | EF_O16 | EF_PRE | EF_PREGRAD:
-        case (0u << EF_ACT_SHIFT) | EF_O16 | EF_ALPHAPTR:
-        case (3u << EF_ACT_SHIFT) | EF_O16:
-        case (5u << EF_ACT_SHIFT) | EF_O16 | EF_ALPHAPTR:
-        case (5u << EF_ACT_SHIFT) | EF_O16 | EF_ALPHAPTR | EF_OSUM:
-          feat |= EF_DIRECT;
-          break;
-        default:
-          break;
-      }
-    }
-  }
 #define FVIT_GEMM_LAUNCH(F)                                                                          \
   do {                                                                                               \
     auto kfn = gemm_wgmma_kernel<(F)>;                                                               \
@@ -1167,54 +1243,18 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
     kfn<<<grid, GEMM_THREADS, smem_bytes, (cudaStream_t)stream>>>(tma, tmb, p);                      \
     return post_launch("gemm_wgmma_kernel");                                                         \
   } while (0)
-#define FVIT_ACTF(x) ((uint32_t)(x) << EF_ACT_SHIFT)
-  if (!needs_generic) {
-    switch (feat) {
-      // ---- inference / shared forward shapes
-      case FVIT_ACTF(0) | EF_O16: FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_O16);                               // qkv
-      case FVIT_ACTF(2) | EF_O16: FVIT_GEMM_LAUNCH(FVIT_ACTF(2) | EF_O16);                               // fc1, conv1 (eval)
-      case FVIT_ACTF(1) | EF_O16: FVIT_GEMM_LAUNCH(FVIT_ACTF(1) | EF_O16);                               // stem conv1 (eval)
-      case FVIT_ACTF(1) | EF_O32 | EF_O16: FVIT_GEMM_LAUNCH(FVIT_ACTF(1) | EF_O32 | EF_O16);             // stem conv2 (eval)
-      case FVIT_ACTF(0) | EF_RESID | EF_O32: FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_RESID | EF_O32);         // proj, fc2, conv dgrad
-      case FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_O16: FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_O16);  // conv2 (eval)
-      case FVIT_ACTF(0) | EF_O32: FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_O32);                               // downsample, head
-      case FVIT_ACTF(0) | EF_O32 | EF_O16: FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_O32 | EF_O16);             // downsample -> next level
-      // ---- training forward
-      case FVIT_ACTF(0) | EF_O16 | EF_STATS: FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_O16 | EF_STATS);         // raw conv + BN statistics
-      case FVIT_ACTF(2) | EF_O16 | EF_PRE: FVIT_GEMM_LAUNCH(FVIT_ACTF(2) | EF_O16 | EF_PRE);             // fc1 saving the pre-GELU value
-      case FVIT_ACTF(2) | EF_O16 | EF_PRE | EF_PREGRAD:
-        FVIT_GEMM_LAUNCH(FVIT_ACTF(2) | EF_O16 | EF_PRE | EF_PREGRAD);                                    // fc1 saving gelu'
-      case FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_RS: FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_RS);  // branch + stochastic depth
-      case FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_CS2 | EF_PRE:
-        FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_CS2 | EF_PRE);                             // branch with layer scale
-      case FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_CS2 | EF_PRE | EF_RS:
-        FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_RESID | EF_O32 | EF_CS2 | EF_PRE | EF_RS);                     // layer scale + stochastic depth
-      // ---- backward
-      case FVIT_ACTF(0) | EF_O32 | EF_ATOMIC | EF_ALPHAPTR: FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_O32 | EF_ATOMIC | EF_ALPHAPTR);  // wgrad split-K
-      case FVIT_ACTF(0) | EF_O32 | EF_ALPHAPTR: FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_O32 | EF_ALPHAPTR);   // wgrad single pass
-      case FVIT_ACTF(0) | EF_O16 | EF_ALPHAPTR: FVIT_GEMM_LAUNCH(FVIT_ACTF(0) | EF_O16 | EF_ALPHAPTR);   // dgrad
-      case FVIT_ACTF(3) | EF_O16 | EF_ALPHAPTR: FVIT_GEMM_LAUNCH(FVIT_ACTF(3) | EF_O16 | EF_ALPHAPTR);   // dgrad * gelu'
-      case FVIT_ACTF(3) | EF_O16: FVIT_GEMM_LAUNCH(FVIT_ACTF(3) | EF_O16);                               // conv dgrad * gelu'
-      case FVIT_ACTF(3) | EF_O16 | EF_ALPHAPTR | EF_OSUM:
-        FVIT_GEMM_LAUNCH(FVIT_ACTF(3) | EF_O16 | EF_ALPHAPTR | EF_OSUM);                                  // fc2 dgrad * gelu' + fc1 bias gradient
-      case FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR: FVIT_GEMM_LAUNCH(FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR);   // fc2 dgrad * saved gelu'
-      case FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR | EF_OSUM:
-        FVIT_GEMM_LAUNCH(FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR | EF_OSUM);                                  // ... + fc1 bias gradient
-      // ---- row-per-thread epilogue variants of the 16-bit-output launches
-      case EF_DIRECT | FVIT_ACTF(0) | EF_O16: FVIT_GEMM_LAUNCH(EF_DIRECT | FVIT_ACTF(0) | EF_O16);
-      case EF_DIRECT | FVIT_ACTF(1) | EF_O16: FVIT_GEMM_LAUNCH(EF_DIRECT | FVIT_ACTF(1) | EF_O16);
-      case EF_DIRECT | FVIT_ACTF(2) | EF_O16: FVIT_GEMM_LAUNCH(EF_DIRECT | FVIT_ACTF(2) | EF_O16);
-      case EF_DIRECT | FVIT_ACTF(2) | EF_O16 | EF_PRE | EF_PREGRAD:
-        FVIT_GEMM_LAUNCH(EF_DIRECT | FVIT_ACTF(2) | EF_O16 | EF_PRE | EF_PREGRAD);
-      case EF_DIRECT | FVIT_ACTF(0) | EF_O16 | EF_ALPHAPTR: FVIT_GEMM_LAUNCH(EF_DIRECT | FVIT_ACTF(0) | EF_O16 | EF_ALPHAPTR);
-      case EF_DIRECT | FVIT_ACTF(3) | EF_O16: FVIT_GEMM_LAUNCH(EF_DIRECT | FVIT_ACTF(3) | EF_O16);
-      case EF_DIRECT | FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR: FVIT_GEMM_LAUNCH(EF_DIRECT | FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR);
-      case EF_DIRECT | FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR | EF_OSUM:
-        FVIT_GEMM_LAUNCH(EF_DIRECT | FVIT_ACTF(5) | EF_O16 | EF_ALPHAPTR | EF_OSUM);
-      default: break;
-    }
+#define FVIT_LAUNCH_CASE(F) \
+  case (F):                 \
+    FVIT_GEMM_LAUNCH(F);
+#define FVIT_LAUNCH_DIRECT_CASE(F) FVIT_LAUNCH_CASE(EF_DIRECT | (F))
+  switch (feat) {
+    FVIT_GEMM_STAGED_VARIANTS(FVIT_LAUNCH_CASE)
+    FVIT_GEMM_DIRECT_VARIANTS(FVIT_LAUNCH_DIRECT_CASE)
+    default:
+      break;
   }
   FVIT_GEMM_LAUNCH(EF_GENERIC);
-#undef FVIT_ACTF
+#undef FVIT_LAUNCH_DIRECT_CASE
+#undef FVIT_LAUNCH_CASE
 #undef FVIT_GEMM_LAUNCH
 }

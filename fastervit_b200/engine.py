@@ -18,6 +18,7 @@ Tensor-core operands are fp16, accumulation fp32, residual stream / LayerNorm / 
 from __future__ import annotations
 
 import ctypes as C
+import gc
 
 import torch
 import torch.nn as nn
@@ -852,9 +853,19 @@ class Plan:
                 torch.cuda.synchronize()
                 g = torch.cuda.CUDAGraph()
                 n0 = L.launch_count()
-                # thread_local: other threads (NCCL's watchdog polling its events) must not invalidate the capture
-                with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                    fn()
+                # Dead reference cycles (e.g. the plans of a dropped model, with their CUDA graphs and memory pools)
+                # are collected now, not by an automatic collection in the middle of the capture: freeing device
+                # memory there invalidates the capture and leaves torch's RNG in capture state.
+                gc.collect()
+                gc_on = gc.isenabled()
+                gc.disable()
+                try:
+                    # thread_local: other threads (NCCL's watchdog polling its events) must not invalidate the capture
+                    with torch.cuda.graph(g, capture_error_mode="thread_local"):
+                        fn()
+                finally:
+                    if gc_on:
+                        gc.enable()
                 self._graphs[key] = (g, L.launch_count() - n0)
                 st = self._graphs[key]
             except Exception as exc:  # noqa: BLE001 - capture problems must not take the model down

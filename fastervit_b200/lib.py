@@ -16,6 +16,10 @@ import os as _os
 LIB_PATH = Path(_os.environ["FVIT_LIB"]) if _os.environ.get("FVIT_LIB") else _PKG / "libfvit_sm100.so"   # (A/B builds)
 
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_GELU_BWD, ACT_RELU_BWD, ACT_MUL_AUX = 0, 1, 2, 3, 4, 5
+# fvit_gemm kernel-variant bits (include/fvit.h FVIT_GEMM_F_*); the activation code sits in bits 1..3
+(GEMM_F_GENERIC, GEMM_F_RESID, GEMM_F_O32, GEMM_F_O16, GEMM_F_STATS, GEMM_F_PRE, GEMM_F_ATOMIC, GEMM_F_ALPHAPTR,
+ GEMM_F_CS2, GEMM_F_RS, GEMM_F_OSUM, GEMM_F_PREGRAD, GEMM_F_DIRECT) = (1 << b for b in (0, *range(4, 16)))
+GEMM_F_ACT_SHIFT = 1
 
 
 class FvitError(RuntimeError):
@@ -90,6 +94,9 @@ def _bind_ops(lib) -> None:
 
 _P, _I, _L, _F, _D = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_double
 _OP_SIGS: dict[str, list] = {
+    # kernel-variant queries of fvit_gemm (include/fvit.h "Kernel variants"; host only, no stream)
+    "fvit_gemm_variant": [_P, _P],
+    "fvit_gemm_variants": [_P, _I],
     "fvit_cast_pad_f16": [_P, _L, _P, _L, _I, _I, _I, _P],
     "fvit_pack_conv3x3_f16": [_P, _P, _I, _I, _I, _I, _P],
     "fvit_pack_conv3x3_taps_f16": [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P],
@@ -204,16 +211,7 @@ def reset_launch_count() -> None:
     load().fvit_reset_launch_count()
 
 
-def gemm(a: torch.Tensor, b: torch.Tensor, *, m: int | None = None, n: int | None = None,
-         kc: int | None = None, a_mn: bool = False, b_mn: bool = False,
-         taps: list[tuple[int, int]] | None = None, a_planes: int = 1, a_plane_stride: int = 0,
-         a_row_off: int = 0, b_row_off: int = 0, b_taps: list[int] | None = None, split_k: int = 1,
-         tile_n: int = 0,
-         alpha: float = 1.0, act: int = ACT_NONE,
-         col_scale=None, col_shift=None, col_scale2=None, aux=None, resid=None, row_map=None,
-         out_f32=None, out_f16=None, col_sum=None, col_sumsq=None, alpha_ptr=None, row_scale=None,
-         out_pre16=None, out_colsum=None, out_colsum_alpha=None, aux_scale=None,
-         aux_shift=None, pre_is_grad: bool = False, cta_group: int = 0) -> None:
+def gemm(a: torch.Tensor, b: torch.Tensor, **kw) -> None:
     """Thin functional wrapper over fvit_gemm for 2-D (strided) torch tensors.
 
     K-major operands are [rows, K] tensors, MN-major operands are [K, rows] tensors; only the row
@@ -222,6 +220,42 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, m: int | None = None, n: int | Non
     lib = load()
     if not a.is_cuda:
         raise FvitError("fvit_gemm needs CUDA tensors (no CPU fallback)")
+    check(lib.fvit_gemm(C.byref(_gemm_args(a, b, **kw)), stream_ptr()))
+
+
+def gemm_variant(a: torch.Tensor, b: torch.Tensor, **kw) -> int:
+    """The kernel variant (FVIT_GEMM_F_* mask) that gemm(a, b, **kw) launches; validates the same way, launches
+    nothing and touches no device memory (CPU tensors are fine: only their addresses and strides are read)."""
+    return gemm_args_variant(_gemm_args(a, b, **kw))
+
+
+def gemm_args_variant(g: GemmArgs) -> int:
+    """The kernel variant fvit_gemm launches for an already filled GemmArgs (e.g. one of a plan's launches)."""
+    out = C.c_uint32(0)
+    check(load().fvit_gemm_variant(C.addressof(g), C.addressof(out)))
+    return out.value
+
+
+def gemm_variants() -> list[int]:
+    """The instantiated kernel variants of fvit_gemm, in launch-table order."""
+    lib = load()
+    n = lib.fvit_gemm_variants(None, 0)
+    buf = (C.c_uint32 * n)()
+    lib.fvit_gemm_variants(C.addressof(buf), n)
+    return list(buf)
+
+
+def _gemm_args(a: torch.Tensor, b: torch.Tensor, *, m: int | None = None, n: int | None = None,
+               kc: int | None = None, a_mn: bool = False, b_mn: bool = False,
+               taps: list[tuple[int, int]] | None = None, a_planes: int = 1, a_plane_stride: int = 0,
+               a_row_off: int = 0, b_row_off: int = 0, b_taps: list[int] | None = None, split_k: int = 1,
+               tile_n: int = 0,
+               alpha: float = 1.0, act: int = ACT_NONE,
+               col_scale=None, col_shift=None, col_scale2=None, aux=None, resid=None, row_map=None,
+               out_f32=None, out_f16=None, col_sum=None, col_sumsq=None, alpha_ptr=None, row_scale=None,
+               out_pre16=None, out_colsum=None, out_colsum_alpha=None, aux_scale=None,
+               aux_shift=None, pre_is_grad: bool = False, cta_group: int = 0) -> GemmArgs:
+    """The GemmArgs of gemm(a, b, **kw)."""
     assert a.dtype in (torch.float16, torch.bfloat16) and b.dtype == a.dtype
     assert a.stride(-1) == 1 and b.stride(-1) == 1
     g = GemmArgs()
@@ -274,7 +308,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, m: int | None = None, n: int | Non
     g.aux_scale, g.aux_shift = ptr(aux_scale), ptr(aux_shift)
     g.pre_is_grad = 1 if pre_is_grad else 0
     g.cta_group = cta_group
-    check(lib.fvit_gemm(C.byref(g), stream_ptr()))
+    return g
 
 
 def call(name: str, *args) -> None:

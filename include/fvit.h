@@ -131,6 +131,33 @@ typedef struct fvit_gemm_args {
 
 int fvit_gemm(const fvit_gemm_args* args, void* stream);
 
+/* Kernel variants of fvit_gemm. Each call launches one compile-time instantiation whose feature mask equals the
+ * call's features (bits below), or the generic kernel, which decides every switch at run time. */
+enum {
+  FVIT_GEMM_F_GENERIC = 1 << 0,   /* every switch at run time (any other combination, bf16 operands) */
+  FVIT_GEMM_F_ACT_SHIFT = 1,      /* 3 bits from here: the FVIT_ACT_* code */
+  FVIT_GEMM_F_RESID = 1 << 4,     /* resid (not with split_k > 1) */
+  FVIT_GEMM_F_O32 = 1 << 5,       /* out_f32 */
+  FVIT_GEMM_F_O16 = 1 << 6,       /* out_f16 */
+  FVIT_GEMM_F_STATS = 1 << 7,     /* col_sum / col_sumsq */
+  FVIT_GEMM_F_PRE = 1 << 8,       /* out_pre16 */
+  FVIT_GEMM_F_ATOMIC = 1 << 9,    /* split_k > 1 */
+  FVIT_GEMM_F_ALPHAPTR = 1 << 10, /* alpha_ptr */
+  FVIT_GEMM_F_CS2 = 1 << 11,      /* col_scale2 */
+  FVIT_GEMM_F_RS = 1 << 12,       /* row_scale */
+  FVIT_GEMM_F_OSUM = 1 << 13,     /* out_colsum */
+  FVIT_GEMM_F_PREGRAD = 1 << 14,  /* pre_is_grad in effect (act == FVIT_ACT_GELU with out_pre16) */
+  FVIT_GEMM_F_DIRECT = 1 << 15    /* row-per-thread epilogue: 16-bit outputs only, n and every leading dimension a
+                                     multiple of 16 elements, outputs and aux 32-byte aligned, per-column vectors
+                                     16-byte aligned, b_ntaps <= 1 (FVIT_GEMM_DIRECT=0 turns it off) */
+};
+#define FVIT_GEMM_F_ACT(x) ((uint32_t)(x) << FVIT_GEMM_F_ACT_SHIFT)
+/* The kernel variant fvit_gemm would launch for *args (same validation, no launch, no device access):
+ * a FVIT_GEMM_F_* mask, FVIT_GEMM_F_GENERIC for the generic kernel. */
+int fvit_gemm_variant(const fvit_gemm_args* args, uint32_t* variant);
+/* The instantiated variants, in launch-table order; returns their count (writes at most cap). */
+int fvit_gemm_variants(uint32_t* out, int cap);
+
 /* ---- weight preparation (fp32 nn.Parameter -> packed fp16 tensor-core operands) ---------------- */
 /* dst[r][0:cols_pad] = (half)src[r][0:cols], zero padded; nn.Linear weights [out, in] (fv.py:393-395,
  * 545-547, 927) become K-major B operands with a 16-byte aligned row stride. */

@@ -452,7 +452,8 @@ def _wide(m, n, pad, gen=None, scale=1.0):
 @pytest.mark.parametrize("cg", [1, 2])
 @pytest.mark.parametrize("m,n,k,tile_n", [(512, 256, 128, 0), (1000, 3136, 200, 0), (333, 784, 72, 0), (700, 400, 136, 0),
                                           (300, 208, 64, 48), (2050, 1024, 784, 160)])
-@pytest.mark.parametrize("variant", ["plain", "bias_gelu", "gelu_pregrad", "dgrad_alpha", "mul_aux_osum", "gelu_bwd_aux"])
+@pytest.mark.parametrize("variant", ["plain", "bias_gelu", "bias_relu", "gelu_pregrad", "dgrad_alpha", "mul_aux_osum",
+                                     "gelu_bwd_aux"])
 def test_gemm_direct_epilogue_matches_staged(variant, m, n, k, tile_n, cg):
     lib = _lib()
     if cg == 2 and tile_n % 32:
@@ -471,6 +472,8 @@ def test_gemm_direct_epilogue_matches_staged(variant, m, n, k, tile_n, cg):
         extra = []
         if variant == "bias_gelu":
             kw.update(act=lib.ACT_GELU, col_shift=bias, col_scale=scale)
+        elif variant == "bias_relu":   # the eval stem's BatchNorm + ReLU
+            kw.update(act=lib.ACT_RELU, col_shift=bias, col_scale=scale)
         elif variant == "gelu_pregrad":
             p16 = _wide(m, n, pad)
             kw.update(act=lib.ACT_GELU, col_shift=bias, out_pre16=p16, pre_is_grad=True)
@@ -500,6 +503,8 @@ def test_gemm_direct_epilogue_matches_staged(variant, m, n, k, tile_n, cg):
         assert _rel(outs[0][0], 0.75 * ref) < 1e-3
     if variant == "bias_gelu":
         assert _rel(outs[0][0], torch.nn.functional.gelu(ref * scale.double() + bias.double())) < 1.5e-3
+    if variant == "bias_relu":
+        assert _rel(outs[0][0], torch.relu(ref * scale.double() + bias.double())) < 1.5e-3
 
 
 def test_gemm_direct_epilogue_row_map_scatter():
