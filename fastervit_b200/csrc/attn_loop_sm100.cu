@@ -9,7 +9,7 @@
 // so no accumulator is ever rescaled; the score recomputation is 2*S*S*hd FLOPs of a contraction that is < 3 % of
 // the model. Scores / probabilities never touch HBM.
 //
-//   warp 4     : TMA producer  — Q tile, K / V tiles through a 2-stage ring, relative-position-bias tiles
+//   warp 4     : TMA producer  — Q tile, K / V tiles through a 2-stage ring (1 at hdp 80), relative-position-bias tiles
 //                (fp32 [128 rows x 32 keys] units, one 128B-swizzled box each) through a 2-stage ring, all in the
 //                order the compute warpgroup consumes them
 //   warps 0..3 : one warpgroup — the score and P V MMAs (wgmma, two m64 halves), softmax with one thread per query
@@ -18,6 +18,7 @@
 #include <cuda_fp16.h>
 
 #include "../../include/fvit.h"
+#include "attn_head.cuh"
 #include "common.h"
 #include "ptx.cuh"
 
@@ -26,7 +27,6 @@ namespace fvit {
 constexpr int AL_THREADS = 160;
 constexpr int AL_ROWS = 128;
 constexpr int AL_PRODUCER = 4;  // the TMA warp; warps 0..3 are the compute warpgroup
-constexpr int AL_NKV = 2;       // K / V tile ring depth
 constexpr int AL_NB = 2;        // bias unit ring depth
 constexpr int AL_BUNIT = 32;    // key columns per bias unit
 constexpr int AL_ACC_LD = 132;  // floats per row of the fp32 score tile
@@ -42,24 +42,36 @@ struct AttnLoopParams {
 };
 
 template <int HDP>
+struct AttnLoopSmem {
+  static constexpr int TILE_BYTES = AL_ROWS * HDP * 2;
+  // K / V tile ring depth: at HDP 80 a second stage would push the layout past 227 KB
+  static constexpr int NKV = HDP == 80 ? 1 : 2;
+  static constexpr int BUNIT_BYTES = AL_ROWS * AL_BUNIT * 4;
+  static constexpr int O_LD = HDP + 4;
+  static constexpr int Q_OFF = 0;
+  static constexpr int KV_OFF = TILE_BYTES;
+  static constexpr int P_OFF = KV_OFF + NKV * TILE_BYTES;
+  static constexpr int BIAS_OFF = P_OFF + AL_ROWS * 128 * 2;
+  static constexpr int SACC_OFF = BIAS_OFF + AL_NB * BUNIT_BYTES;
+  static constexpr int OACC_OFF = SACC_OFF + AL_ROWS * AL_ACC_LD * 4;
+  static constexpr int CTRL_OFF = OACC_OFF + AL_ROWS * O_LD * 4;
+  static constexpr size_t BYTES = 1024 + CTRL_OFF + 256;
+  static_assert(BYTES <= 227 * 1024, "attn_loop_kernel: shared memory");
+};
+
+template <int HDP>
 __global__ void __launch_bounds__(AL_THREADS, 1)
-    attn_loop_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_bias,
-                     const __grid_constant__ AttnLoopParams p) {
-  constexpr uint32_t SWZ = HDP == 64 ? SWZ_128B : SWZ_64B;
-  constexpr uint32_t ROW_BYTES = HDP * 2;
-  constexpr uint32_t SBO_QKV = 8 * ROW_BYTES;
-  constexpr int TILE_BYTES = AL_ROWS * HDP * 2;
-  constexpr int NKV = AL_NKV, NB = AL_NB, BUNIT = AL_BUNIT;
-  constexpr int BUNIT_BYTES = AL_ROWS * BUNIT * 4;
+    attn_loop_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_qkv_b,
+                     const __grid_constant__ CUtensorMap tmap_bias, const __grid_constant__ AttnLoopParams p) {
+  using SM = AttnLoopSmem<HDP>;
+  using HT = HeadTile<HDP>;
+  constexpr int TILE_BYTES = SM::TILE_BYTES;
+  constexpr int NKV = SM::NKV, NB = AL_NB, BUNIT = AL_BUNIT;
+  constexpr int BUNIT_BYTES = SM::BUNIT_BYTES;
   constexpr int UNITS = 128 / BUNIT;              // bias units per key tile
-  constexpr int O_LD = HDP + 4;
-  constexpr int Q_OFF = 0;
-  constexpr int KV_OFF = TILE_BYTES;
-  constexpr int P_OFF = KV_OFF + NKV * TILE_BYTES;
-  constexpr int BIAS_OFF = P_OFF + AL_ROWS * 128 * 2;
-  constexpr int SACC_OFF = BIAS_OFF + NB * BUNIT_BYTES;
-  constexpr int OACC_OFF = SACC_OFF + AL_ROWS * AL_ACC_LD * 4;
-  constexpr int CTRL_OFF = OACC_OFF + AL_ROWS * O_LD * 4;
+  constexpr int O_LD = SM::O_LD;
+  constexpr int Q_OFF = SM::Q_OFF, KV_OFF = SM::KV_OFF, P_OFF = SM::P_OFF, BIAS_OFF = SM::BIAS_OFF;
+  constexpr int SACC_OFF = SM::SACC_OFF, OACC_OFF = SM::OACC_OFF, CTRL_OFF = SM::CTRL_OFF;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -75,6 +87,7 @@ __global__ void __launch_bounds__(AL_THREADS, 1)
 
   if (warp == AL_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmap_qkv);
+    if (HT::HB > 0) tma_prefetch_desc(&tmap_qkv_b);
     if (p.has_bias) tma_prefetch_desc(&tmap_bias);
     mbar_init(q_full, 1), mbar_init(q_empty, 1);
     for (int i = 0; i < NKV; ++i) mbar_init(&kv_full[i], 1), mbar_init(&kv_empty[i], 1);
@@ -100,7 +113,8 @@ __global__ void __launch_bounds__(AL_THREADS, 1)
         const int st = kv_cnt % NKV;
         mbar_wait(&kv_empty[st], ((kv_cnt / NKV) & 1) ^ 1);
         mbar_expect_tx(&kv_full[st], TILE_BYTES);
-        tma_load_2d(smem + KV_OFF + st * TILE_BYTES, &tmap_qkv, &kv_full[st], (which * p.heads + head) * HDP, row0 + j * 128);
+        HT::load(smem + KV_OFF + st * TILE_BYTES, AL_ROWS, 0, &tmap_qkv, &tmap_qkv_b, &kv_full[st],
+                 (which * p.heads + head) * HDP, row0 + j * 128);
         ++kv_cnt;
       };
       for (int w = blockIdx.x; w < items; w += gridDim.x, ++it) {
@@ -109,7 +123,7 @@ __global__ void __launch_bounds__(AL_THREADS, 1)
         const int row0 = grp * S;
         mbar_wait(q_empty, (it & 1) ^ 1);
         mbar_expect_tx(q_full, TILE_BYTES);
-        tma_load_2d(smem + Q_OFF, &tmap_qkv, q_full, head * HDP, row0 + qi * 128);
+        HT::load(smem + Q_OFF, AL_ROWS, 0, &tmap_qkv, &tmap_qkv_b, q_full, head * HDP, row0 + qi * 128);
         // consumption order: pass 1 K_0 b_0 K_1 b_1 ...; pass 2 K_0 b_0 V_0 K_1 b_1 V_1 ...
         for (int pass = 0; pass < 2; ++pass) {
           for (int j = 0; j < nkt; ++j) {
@@ -145,10 +159,9 @@ __global__ void __launch_bounds__(AL_THREADS, 1)
       mbar_wait(&kv_full[st], (kv_cnt / NKV) & 1);
       const uint32_t sK = smem_u32(smem + KV_OFF + st * TILE_BYTES);
       named_bar_sync(1, 128);  // every read of the previous score tile is done
-      wg_mma_128<128, 0, 0, HDP / 16>(
-          sacc, AL_ACC_LD,
-          [&](int h, int k) { return make_smem_desc(sQ + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
-          [&](int k) { return make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ); }, false);
+      wg_mma_128<128, 0, 0, HT::KSTEPS>(
+          sacc, AL_ACC_LD, [&](int h, int k) { return HT::kdesc(sQ, AL_ROWS, h * 64, k); },
+          [&](int k) { return HT::kdesc(sK, AL_ROWS, 0, k); }, false);
       named_bar_sync(1, 128);
       if (tid == 0) {
         mbar_arrive(&kv_empty[st]);
@@ -233,12 +246,12 @@ __global__ void __launch_bounds__(AL_THREADS, 1)
             const int st = kv_cnt % NKV;
             mbar_wait(&kv_full[st], (kv_cnt / NKV) & 1);
             const uint32_t sV = smem_u32(smem + KV_OFF + st * TILE_BYTES);
-            wg_mma_128<HDP, 0, 1, 8>(
-          oacc, O_LD,
+            wg_mma_128_head<HDP, 0, 8>(
+                oacc, O_LD,
                 [&](int h, int ks) {
                   return make_smem_desc(sPu + (ks >> 2) * (AL_ROWS * 128) + h * 64 * 128 + (ks & 3) * 32, 16, 1024, SWZ_128B);
                 },
-                [&](int ks) { return make_smem_desc(sV + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, j > 0);
+                sV, AL_ROWS, j > 0);
             named_bar_sync(1, 128);  // P V complete: V stage and P tile are free, O rows are readable
             if (tid == 0) mbar_arrive(&kv_empty[st]);
             ++kv_cnt;
@@ -249,36 +262,16 @@ __global__ void __launch_bounds__(AL_THREADS, 1)
       // O epilogue
       const float inv = row_ok ? 1.f / sum : 0.f;
       const long long grow = (long long)grp * S + qrow;
-      const float* orow_acc = oacc + r * O_LD;
-#pragma unroll
-      for (int c0 = 0; c0 < HDP; c0 += 32) {
-        uint32_t raw[32];
-        ld_row32(orow_acc + c0, raw);
-        if (row_ok) {
-          __half* orow = p.out + grow * p.ldo + head * HDP;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint32_t o4[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const __half2 hh = __floats2half2_rn(__uint_as_float(raw[q * 8 + 2 * u]) * inv,
-                                                   __uint_as_float(raw[q * 8 + 2 * u + 1]) * inv);
-              o4[u] = *reinterpret_cast<const uint32_t*>(&hh);
-            }
-            *reinterpret_cast<uint4*>(orow + c0 + q * 8) = make_uint4(o4[0], o4[1], o4[2], o4[3]);
-          }
-        }
-      }
+      if (row_ok) store_row_f16<HDP>(oacc + r * O_LD, inv, p.out + grow * p.ldo + head * HDP);
       if (p.lse && row_ok) p.lse[grow * p.heads + head] = mx + log2f(sum);
     }
   }
 }
 
 template <int HDP>
-static int launch_attn_loop(const CUtensorMap& tq, const CUtensorMap& tb, const AttnLoopParams& p, cudaStream_t st) {
-  constexpr size_t smem = 1024 + (size_t)(1 + AL_NKV) * AL_ROWS * HDP * 2 + AL_ROWS * 128 * 2 +
-                          AL_NB * AL_ROWS * AL_BUNIT * 4 + AL_ROWS * AL_ACC_LD * 4 + AL_ROWS * (HDP + 4) * 4 + 256;
-  static_assert(smem <= 227 * 1024, "attn_loop_kernel: shared memory");
+static int launch_attn_loop(const CUtensorMap& tq, const CUtensorMap& tqb, const CUtensorMap& tb, const AttnLoopParams& p,
+                            cudaStream_t st) {
+  constexpr size_t smem = AttnLoopSmem<HDP>::BYTES;
   static bool configured = false;
   if (!configured) {
     FVIT_CUDA(cudaFuncSetAttribute(attn_loop_kernel<HDP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -286,7 +279,7 @@ static int launch_attn_loop(const CUtensorMap& tq, const CUtensorMap& tb, const 
   }
   const long long items = (long long)p.groups * p.heads * p.nqt;
   const int slots = num_sms();
-  attn_loop_kernel<HDP><<<(unsigned)(items < slots ? items : slots), AL_THREADS, smem, st>>>(tq, tb, p);
+  attn_loop_kernel<HDP><<<(unsigned)(items < slots ? items : slots), AL_THREADS, smem, st>>>(tq, tqb, tb, p);
   return post_launch("attn_loop_kernel");
 }
 
@@ -300,7 +293,8 @@ extern "C" int fvit_attn_loop_fwd(const void* qkv, int64_t ldq, int32_t groups, 
   // (any S: one tile is the case nqt = nkt = 1. Inference plans give windows of up to 128 tokens to fvit_attn_tc_fwd / the fused
   // kernel, which pack several windows into a tile; training plans come here from 65 tokens on for the log-sum-exp rows)
   FVIT_CHECK(S > 0, "fvit_attn_loop_fwd: S=%d", S);
-  FVIT_CHECK(hdp == 32 || hdp == 64, "fvit_attn_loop_fwd: padded head dim %d unsupported (32 or 64)", hdp);
+  FVIT_CHECK(hdp == 32 || hdp == 64 || hdp == 80, "fvit_attn_loop_fwd: padded head dim %d unsupported (32, 64 or 80)",
+             hdp);
   FVIT_CHECK(ldq % 8 == 0 && ldo % 8 == 0 && ldq >= 3 * heads * hdp && ldo >= heads * hdp,
              "fvit_attn_loop_fwd: bad leading dimensions");
   FVIT_CHECK(!bias || S % 4 == 0, "fvit_attn_loop_fwd: the bias rows of S=%d tokens are not 16-byte aligned (TMA)", S);
@@ -311,13 +305,9 @@ extern "C" int fvit_attn_loop_fwd(const void* qkv, int64_t ldq, int32_t groups, 
   p.scale_log2e = scale * 1.4426950408889634f;
   p.has_bias = bias ? 1 : 0;
   p.out = (__half*)out, p.ldo = ldo, p.lse = lse;
-  CUtensorMap tq, tb;
+  CUtensorMap tq, tqb, tb;
   {
-    uint64_t dims[2] = {(uint64_t)(3 * heads * hdp), (uint64_t)groups * S};
-    uint64_t strides[1] = {(uint64_t)ldq * 2};
-    uint32_t box[2] = {(uint32_t)hdp, (uint32_t)AL_ROWS};
-    int rc = cached_tmap_16bit(&tq, qkv, 2, dims, strides, box,
-                               hdp == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
+    int rc = head_tile_tmaps(&tq, &tqb, qkv, 3 * heads * hdp, (uint64_t)groups * S, ldq, hdp, AL_ROWS);
     if (rc) return rc;
   }
   if (bias) {
@@ -329,8 +319,9 @@ extern "C" int fvit_attn_loop_fwd(const void* qkv, int64_t ldq, int32_t groups, 
   } else {
     tb = tq;
   }
-  if (hdp == 64) return launch_attn_loop<64>(tq, tb, p, (cudaStream_t)stream);
-  return launch_attn_loop<32>(tq, tb, p, (cudaStream_t)stream);
+  if (hdp == 80) return launch_attn_loop<80>(tq, tqb, tb, p, (cudaStream_t)stream);
+  if (hdp == 64) return launch_attn_loop<64>(tq, tqb, tb, p, (cudaStream_t)stream);
+  return launch_attn_loop<32>(tq, tqb, tb, p, (cudaStream_t)stream);
 }
 
 // =====================================================================================================
@@ -386,18 +377,18 @@ struct AttnBwdLongSmem {
   static constexpr int WORK_BYTES = 2 * AL_ROWS * ALL_HALF_LD * 4;
   static constexpr int CTRL_OFF = WORK_OFF + WORK_BYTES;
   static constexpr int ROWV_OFF = CTRL_OFF + 256;           // delta[nt * 128], lse[nt * 128]
-  static_assert(2 * AL_ROWS * (HDP + 4) * 4 <= WORK_BYTES, "dK / dV staging fits the work area");
+  static_assert(AL_ROWS * (HDP + 4) * 4 <= WORK_BYTES, "dQ / dK / dV staging fits the work area");
 };
 
 template <int HDP>
 __global__ void __launch_bounds__(ALL_THREADS, 1)
     attn_loop_bwd_long_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
+                              const __grid_constant__ CUtensorMap tmap_qkv_b, const __grid_constant__ CUtensorMap tmap_do_b,
                               const __grid_constant__ AttnLoopBwdLongParams pl) {
   using SM = AttnBwdLongSmem<HDP>;
+  using HT = HeadTile<HDP>;
+  constexpr int HA = HT::HA, HB = HT::HB;
   const AttnLoopBwdParams& p = pl.b;
-  constexpr uint32_t SWZ = HDP == 64 ? SWZ_128B : SWZ_64B;
-  constexpr uint32_t ROW_BYTES = HDP * 2;
-  constexpr uint32_t SBO_QKV = 8 * ROW_BYTES;
   constexpr int TILE_BYTES = SM::TILE_BYTES;
   constexpr int NQ = SM::NQ;
   constexpr int G_LD = HDP + 4;  // row stride of the dQ / dK / dV fp32 tiles
@@ -418,6 +409,7 @@ __global__ void __launch_bounds__(ALL_THREADS, 1)
   if (warp == AL_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmap_qkv);
     tma_prefetch_desc(&tmap_do);
+    if (HB > 0) tma_prefetch_desc(&tmap_qkv_b), tma_prefetch_desc(&tmap_do_b);
     for (int i = 0; i < 2; ++i) mbar_init(&qdo_full[i], 1), mbar_init(&qdo_empty[i], 1);
     mbar_init(kv_full, 1), mbar_init(kv_empty, 1);
     fence_mbar_init();
@@ -435,14 +427,17 @@ __global__ void __launch_bounds__(ALL_THREADS, 1)
         for (int j = 0; j < nt; ++j, ++kv_cnt) {
           mbar_wait(kv_empty, (kv_cnt & 1) ^ 1);
           mbar_expect_tx(kv_full, 2 * TILE_BYTES);
-          tma_load_2d(smem + SM::KV_OFF, &tmap_qkv, kv_full, (p.heads + head) * HDP, row0 + j * 128);
-          tma_load_2d(smem + SM::KV_OFF + TILE_BYTES, &tmap_qkv, kv_full, (2 * p.heads + head) * HDP, row0 + j * 128);
+          HT::load(smem + SM::KV_OFF, AL_ROWS, 0, &tmap_qkv, &tmap_qkv_b, kv_full, (p.heads + head) * HDP, row0 + j * 128);
+          HT::load(smem + SM::KV_OFF + TILE_BYTES, AL_ROWS, 0, &tmap_qkv, &tmap_qkv_b, kv_full, (2 * p.heads + head) * HDP,
+                   row0 + j * 128);
           for (int i = 0; i < nt; ++i, ++pair) {
             const int qs = pair % NQ;
             mbar_wait(&qdo_empty[qs], ((pair / NQ) & 1) ^ 1);
             mbar_expect_tx(&qdo_full[qs], 2 * TILE_BYTES);
-            tma_load_2d(smem + SM::QDO_OFF + (2 * qs) * TILE_BYTES, &tmap_qkv, &qdo_full[qs], head * HDP, row0 + i * 128);
-            tma_load_2d(smem + SM::QDO_OFF + (2 * qs + 1) * TILE_BYTES, &tmap_do, &qdo_full[qs], head * HDP, row0 + i * 128);
+            HT::load(smem + SM::QDO_OFF + (2 * qs) * TILE_BYTES, AL_ROWS, 0, &tmap_qkv, &tmap_qkv_b, &qdo_full[qs],
+                     head * HDP, row0 + i * 128);
+            HT::load(smem + SM::QDO_OFF + (2 * qs + 1) * TILE_BYTES, AL_ROWS, 0, &tmap_do, &tmap_do_b, &qdo_full[qs],
+                     head * HDP, row0 + i * 128);
           }
         }
       }
@@ -486,12 +481,16 @@ __global__ void __launch_bounds__(ALL_THREADS, 1)
       for (int j = 0; j < nt; ++j, ++kv_cnt) {
         const int ncols = min(128, S - j * 128);
         mbar_wait(kv_full, kv_cnt & 1);
-        // dV_j / dK_j accumulators (rows 64h .. 64h + 63 = keys of this tile), summed over the query tiles
-        float dv[2][HDP / 2], dk[2][HDP / 2];
+        // dV_j / dK_j accumulators (rows 64h .. 64h + 63 = keys of this tile), summed over the query tiles: head
+        // columns [0, HA) in dv / dk, [HA, HDP) in dvb / dkb
+        float dv[2][HA / 2], dk[2][HA / 2], dvb[2][HB > 0 ? HB / 2 : 1], dkb[2][HB > 0 ? HB / 2 : 1];
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-          for (int u = 0; u < HDP / 2; ++u) dv[h][u] = 0.f, dk[h][u] = 0.f;
+          for (int u = 0; u < HA / 2; ++u) dv[h][u] = 0.f, dk[h][u] = 0.f;
+#pragma unroll
+          for (int u = 0; u < (HB > 0 ? HB / 2 : 1); ++u) dvb[h][u] = 0.f, dkb[h][u] = 0.f;
+        }
         for (int i = 0; i < nt; ++i, ++pair) {
           const int qs = pair % NQ;
           mbar_wait(&qdo_full[qs], (pair / NQ) & 1);
@@ -504,14 +503,12 @@ __global__ void __launch_bounds__(ALL_THREADS, 1)
 #pragma unroll 1
           for (int ch = 0; ch < 2; ++ch) {  // key columns [64ch, 64ch + 64) of the pair
             named_bar_sync(1, 128);         // the work area is free
-            wg_mma_128<64, 0, 0, HDP / 16>(
-          s_half, ALL_HALF_LD,
-                [&](int h, int k) { return make_smem_desc(sQ + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
-                [&](int k) { return make_smem_desc(sK + ch * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); }, false);
-            wg_mma_128<64, 0, 0, HDP / 16>(
-          dp_half, ALL_HALF_LD,
-                [&](int h, int k) { return make_smem_desc(sDO + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
-                [&](int k) { return make_smem_desc(sV + ch * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); }, false);
+            wg_mma_128<64, 0, 0, HT::KSTEPS>(
+                s_half, ALL_HALF_LD, [&](int h, int k) { return HT::kdesc(sQ, AL_ROWS, h * 64, k); },
+                [&](int k) { return HT::kdesc(sK, AL_ROWS, ch * 64, k); }, false);
+            wg_mma_128<64, 0, 0, HT::KSTEPS>(
+                dp_half, ALL_HALF_LD, [&](int h, int k) { return HT::kdesc(sDO, AL_ROWS, h * 64, k); },
+                [&](int k) { return HT::kdesc(sV, AL_ROWS, ch * 64, k); }, false);
             named_bar_sync(1, 128);
 #pragma unroll 1
             for (int cc = 0; cc < 64; cc += 16) {
@@ -565,21 +562,25 @@ __global__ void __launch_bounds__(ALL_THREADS, 1)
           for (int h = 0; h < 2; ++h) {
 #pragma unroll
             for (int ks = 0; ks < 8; ++ks) {
-              Wgmma<HDP, 1, 1, 0>::mma(dv[h], make_smem_desc(sPu + h * (AL_ROWS * 128) + ks * 2048, AL_ROWS * 128, 1024, SWZ_128B),
-                                       make_smem_desc(sDO + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ), 1u);
-              Wgmma<HDP, 1, 1, 0>::mma(dk[h], make_smem_desc(sDSu + h * (AL_ROWS * 128) + ks * 2048, AL_ROWS * 128, 1024, SWZ_128B),
-                                       make_smem_desc(sQ + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ), 1u);
+              const uint64_t ap = make_smem_desc(sPu + h * (AL_ROWS * 128) + ks * 2048, AL_ROWS * 128, 1024, SWZ_128B);
+              const uint64_t ads = make_smem_desc(sDSu + h * (AL_ROWS * 128) + ks * 2048, AL_ROWS * 128, 1024, SWZ_128B);
+              Wgmma<HA, 1, 1, 0>::mma(dv[h], ap, HT::ndesc_a(sDO, ks), 1u);
+              Wgmma<HA, 1, 1, 0>::mma(dk[h], ads, HT::ndesc_a(sQ, ks), 1u);
+              if constexpr (HB > 0) {
+                Wgmma<HB, 1, 1, 0>::mma(dvb[h], ap, HT::ndesc_b(sDO, AL_ROWS, ks), 1u);
+                Wgmma<HB, 1, 1, 0>::mma(dkb[h], ads, HT::ndesc_b(sQ, AL_ROWS, ks), 1u);
+              }
             }
           }
           wgmma_commit();
           wgmma_wait0();
           // partial dQ_i = dS K_j into the work area, then this thread's row into the fp32 scratch
-          wg_mma_128<HDP, 0, 1, 8>(
-          work, G_LD,
+          wg_mma_128_head<HDP, 0, 8>(
+              work, G_LD,
               [&](int h, int ks) {
                 return make_smem_desc(sDSu + (ks >> 2) * (AL_ROWS * 128) + h * 64 * 128 + (ks & 3) * 32, 16, 1024, SWZ_128B);
               },
-              [&](int ks) { return make_smem_desc(sK + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, false);
+              sK, AL_ROWS, false);
           named_bar_sync(1, 128);
           if (tid == 0) mbar_arrive(&qdo_empty[qs]);  // Q_i / dO_i consumed
           if (row_ok) {
@@ -598,43 +599,23 @@ __global__ void __launch_bounds__(ALL_THREADS, 1)
             }
           }
         }
-        // every MMA of this key tile is complete: K_j / V_j are free; dK_j / dV_j (row r = key j*128 + r) through the
+        // every MMA of this key tile is complete: K_j / V_j are free; dK_j, then dV_j (row r = key j*128 + r) through the
         // work area
         named_bar_sync(1, 128);
         if (tid == 0) mbar_arrive(kv_empty);
-        float* gk = work;
-        float* gv = work + AL_ROWS * G_LD;
-        acc_store<HDP>(gk, G_LD, dk[0]);
-        acc_store<HDP>(gk + 64 * G_LD, G_LD, dk[1]);
-        acc_store<HDP>(gv, G_LD, dv[0]);
-        acc_store<HDP>(gv + 64 * G_LD, G_LD, dv[1]);
-        named_bar_sync(1, 128);
         {
           const int key = j * 128 + r;
-          const bool ok = key < S;
           __half* orow = p.dqkv + (row0 + key) * p.lddq + head * HDP;
 #pragma unroll
           for (int which = 1; which < 3; ++which) {
-            const float* src = (which == 1 ? gk : gv) + r * G_LD;
-            const float mul = which == 1 ? p.scale : 1.f;
+            if (which == 2) named_bar_sync(1, 128);  // every dK row is read: dV overwrites the work area
 #pragma unroll
-            for (int c0 = 0; c0 < HDP; c0 += 32) {
-              uint32_t raw[32];
-              ld_row32(src + c0, raw);
-              if (ok) {
-#pragma unroll
-                for (int qq = 0; qq < 4; ++qq) {
-                  uint32_t o4[4];
-#pragma unroll
-                  for (int u = 0; u < 4; ++u) {
-                    const __half2 hh = __floats2half2_rn(__uint_as_float(raw[qq * 8 + 2 * u]) * mul,
-                                                         __uint_as_float(raw[qq * 8 + 2 * u + 1]) * mul);
-                    o4[u] = *reinterpret_cast<const uint32_t*>(&hh);
-                  }
-                  *reinterpret_cast<uint4*>(orow + which * Cp + c0 + qq * 8) = make_uint4(o4[0], o4[1], o4[2], o4[3]);
-                }
-              }
+            for (int h = 0; h < 2; ++h) {
+              acc_store<HA>(work + h * 64 * G_LD, G_LD, which == 1 ? dk[h] : dv[h]);
+              if constexpr (HB > 0) acc_store<HB>(work + h * 64 * G_LD + HA, G_LD, which == 1 ? dkb[h] : dvb[h]);
             }
+            named_bar_sync(1, 128);
+            if (key < S) store_row_f16<HDP>(work + r * G_LD, which == 1 ? p.scale : 1.f, orow + which * Cp);
           }
         }
       }
@@ -662,8 +643,8 @@ __global__ void __launch_bounds__(ALL_THREADS, 1)
 }
 
 template <int HDP>
-static int launch_attn_loop_bwd_long(const CUtensorMap& tq, const CUtensorMap& td, const AttnLoopBwdLongParams& p,
-                                     cudaStream_t st) {
+static int launch_attn_loop_bwd_long(const CUtensorMap& tq, const CUtensorMap& td, const CUtensorMap& tqb,
+                                     const CUtensorMap& tdb, const AttnLoopBwdLongParams& p, cudaStream_t st) {
   const size_t smem = 1024 + (size_t)AttnBwdLongSmem<HDP>::ROWV_OFF + (size_t)p.b.nt * 128 * 8;
   FVIT_CHECK(smem <= 227 * 1024, "fvit_attn_loop_bwd_long: S=%d needs %zu bytes of shared memory", p.b.S, smem);
   static size_t configured = 0;
@@ -673,7 +654,7 @@ static int launch_attn_loop_bwd_long(const CUtensorMap& tq, const CUtensorMap& t
   }
   const int items = p.b.groups * p.b.heads;
   const int sms = num_sms();
-  attn_loop_bwd_long_kernel<HDP><<<items < sms ? items : sms, ALL_THREADS, smem, st>>>(tq, td, p);
+  attn_loop_bwd_long_kernel<HDP><<<items < sms ? items : sms, ALL_THREADS, smem, st>>>(tq, td, tqb, tdb, p);
   return post_launch("attn_loop_bwd_long_kernel");
 }
 
@@ -687,7 +668,7 @@ extern "C" int fvit_attn_loop_bwd_long(const void* qkv, int64_t ldq, const void*
   FVIT_CHECK(qkv && dout && out && lse && dqkv && dq_scratch && groups > 0 && heads > 0, "fvit_attn_loop_bwd_long: bad arguments");
   FVIT_CHECK(S > 0, "fvit_attn_loop_bwd_long: S=%d", S);
   FVIT_CHECK(S % 4 == 0, "fvit_attn_loop_bwd_long: S=%d must be a multiple of 4 (16-byte bias / dbias accesses)", S);
-  FVIT_CHECK(hdp == 32 || hdp == 64, "fvit_attn_loop_bwd_long: padded head dim %d unsupported", hdp);
+  FVIT_CHECK(hdp == 32 || hdp == 64 || hdp == 80, "fvit_attn_loop_bwd_long: padded head dim %d unsupported", hdp);
   FVIT_CHECK(ldq % 8 == 0 && lddo % 8 == 0 && ldo % 8 == 0 && lddq % 8 == 0 && ld_scratch % 4 == 0 &&
                  ld_scratch >= (int64_t)heads * hdp && (reinterpret_cast<uintptr_t>(dq_scratch) & 15) == 0,
              "fvit_attn_loop_bwd_long: bad leading dimensions");
@@ -699,19 +680,12 @@ extern "C" int fvit_attn_loop_bwd_long(const void* qkv, int64_t ldq, const void*
   p.dout = (const __half*)dout, p.lddo = lddo, p.out = (const __half*)out, p.ldo = ldo;
   p.dqkv = (__half*)dqkv, p.lddq = lddq;
   pl.dq32 = dq_scratch, pl.lddq32 = ld_scratch;
-  CUtensorMap tq, td;
-  const CUtensorMapSwizzle swz = hdp == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  uint32_t box[2] = {(uint32_t)hdp, (uint32_t)AL_ROWS};
-  {
-    uint64_t dims[2] = {(uint64_t)(3 * heads * hdp), (uint64_t)groups * S};
-    uint64_t strides[1] = {(uint64_t)ldq * 2};
-    int rc = cached_tmap_16bit(&tq, qkv, 2, dims, strides, box, swz);
-    if (rc) return rc;
-    uint64_t dims2[2] = {(uint64_t)(heads * hdp), (uint64_t)groups * S};
-    uint64_t strides2[1] = {(uint64_t)lddo * 2};
-    rc = cached_tmap_16bit(&td, dout, 2, dims2, strides2, box, swz);
-    if (rc) return rc;
-  }
-  if (hdp == 64) return launch_attn_loop_bwd_long<64>(tq, td, pl, (cudaStream_t)stream);
-  return launch_attn_loop_bwd_long<32>(tq, td, pl, (cudaStream_t)stream);
+  CUtensorMap tq, td, tqb, tdb;
+  int rc = head_tile_tmaps(&tq, &tqb, qkv, 3 * heads * hdp, (uint64_t)groups * S, ldq, hdp, AL_ROWS);
+  if (rc) return rc;
+  rc = head_tile_tmaps(&td, &tdb, dout, heads * hdp, (uint64_t)groups * S, lddo, hdp, AL_ROWS);
+  if (rc) return rc;
+  if (hdp == 80) return launch_attn_loop_bwd_long<80>(tq, td, tqb, tdb, pl, (cudaStream_t)stream);
+  if (hdp == 64) return launch_attn_loop_bwd_long<64>(tq, td, tqb, tdb, pl, (cudaStream_t)stream);
+  return launch_attn_loop_bwd_long<32>(tq, td, tqb, tdb, pl, (cudaStream_t)stream);
 }

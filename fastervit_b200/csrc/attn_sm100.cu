@@ -5,7 +5,7 @@
 // one image); rows of the box beyond gpt*S belong to the next tile and are masked.
 //
 //   warp 4     : TMA producer — Q, K, V head slices (128 x hdp, 16-bit) of the packed qkv matrix into
-//                a ring of swizzled shared-memory tiles
+//                a ring of swizzled shared-memory head tiles (attn_head.cuh: hdp 32, 64 or 80)
 //   warps 0..3 : one warpgroup — S = Q K^T (wgmma, M=128 as two m64 halves, N=128, K=hdp) into an fp32
 //                score tile in shared memory; softmax with one thread per query row: block-diagonal
 //                window mask, relative-position bias from shared memory, fp32 max / exp2 / sum, P written
@@ -18,6 +18,7 @@
 #include <unordered_map>
 
 #include "../../include/fvit.h"
+#include "attn_head.cuh"
 #include "common.h"
 #include "ptx.cuh"
 
@@ -56,12 +57,11 @@ struct AttnSmem {
 // masked as keys, not written as queries).
 template <int HDP>
 __global__ void __launch_bounds__(AT_THREADS, 1)
-    attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ AttnParams p) {
+    attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_qkv_b,
+                   const __grid_constant__ AttnParams p) {
   using SM = AttnSmem<HDP>;
+  using HT = HeadTile<HDP>;
   constexpr int NST = SM::NST;
-  constexpr uint32_t SWZ = HDP == 64 ? SWZ_128B : SWZ_64B;
-  constexpr uint32_t ROW_BYTES = HDP * 2;            // bytes per smem row of Q / K / V
-  constexpr uint32_t SBO_QKV = 8 * ROW_BYTES;        // 8-row group stride
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -74,6 +74,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
 
   if (warp == AT_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmap_qkv);
+    if (HT::HB > 0) tma_prefetch_desc(&tmap_qkv_b);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&qkv_full[i], 1);
       mbar_init(&qkv_empty[i], 1);
@@ -99,10 +100,9 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
           // window (tile*gpt + sl) -> rows [sl*slot, (sl+1)*slot) of the three operand tiles; windows
           // past the end give out-of-range rows, which TMA zero-fills
           const int row0 = (tile * p.gpt + sl) * S;
-          uint8_t* dst = base + sl * p.slot * ROW_BYTES;
-          tma_load_2d(dst, &tmap_qkv, &qkv_full[st], head * HDP, row0);
-          tma_load_2d(dst + SM::TILE_BYTES, &tmap_qkv, &qkv_full[st], (p.heads + head) * HDP, row0);
-          tma_load_2d(dst + 2 * SM::TILE_BYTES, &tmap_qkv, &qkv_full[st], (2 * p.heads + head) * HDP, row0);
+          for (int op = 0; op < 3; ++op)
+            HT::load(base + op * SM::TILE_BYTES, AT_ROWS, sl * p.slot, &tmap_qkv, &tmap_qkv_b, &qkv_full[st],
+                     (op * p.heads + head) * HDP, row0);
         }
       }
     }
@@ -164,10 +164,9 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
       const uint32_t sK = sQ + SM::TILE_BYTES;
       const uint32_t sV = sQ + 2 * SM::TILE_BYTES;
       named_bar_sync(1, 128);  // the previous item's O reads of the accumulator tile are done
-      wg_mma_128<128, 0, 0, HDP / 16>(
-          acc, AT_ACC_LD,
-          [&](int h, int k) { return make_smem_desc(sQ + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
-          [&](int k) { return make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ); }, false);
+      wg_mma_128<128, 0, 0, HT::KSTEPS>(
+          acc, AT_ACC_LD, [&](int h, int k) { return HT::kdesc(sQ, AT_ROWS, h * 64, k); },
+          [&](int k) { return HT::kdesc(sK, AT_ROWS, 0, k); }, false);
       named_bar_sync(1, 128);
       // brow[c - lo] = bias of (this row, key c); rows that are not real queries read row 0 (unused)
       const float* brow = bias_s + (row_ok ? j : 0) * S;
@@ -223,41 +222,25 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
       // P is complete: publish it to the async proxy; every score read is done before O overwrites the tile
       fence_proxy_async_smem();
       named_bar_sync(1, 128);
-      wg_mma_128<HDP, 0, 1, 8>(
+      wg_mma_128_head<HDP, 0, 8>(
           acc, AT_ACC_LD,  // 128 keys in steps of 16
           [&](int h, int ks) {
             return make_smem_desc(sP_u + (ks >> 2) * (AT_ROWS * 128) + h * 64 * 128 + (ks & 3) * 32, 16, 1024, SWZ_128B);
           },
-          [&](int ks) { return make_smem_desc(sV + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, false);
+          sV, AT_ROWS, false);
       named_bar_sync(1, 128);
       if (tid == 0) mbar_arrive(&qkv_empty[st]);  // Q / K / V of this stage are consumed
       const float inv = row_ok ? 1.f / sum : 0.f;
       const long long grow = (long long)grp * S + j;
-      __half* orow = p.out + grow * p.ldo + head * HDP;
-#pragma unroll
-      for (int c0 = 0; c0 < HDP; c0 += 32) {
-        uint32_t raw[32];
-        ld_row32(arow + c0, raw);
-        if (row_ok) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint32_t o4[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const __half2 h = __floats2half2_rn(__uint_as_float(raw[q * 8 + 2 * u]) * inv,
-                                                  __uint_as_float(raw[q * 8 + 2 * u + 1]) * inv);
-              o4[u] = *reinterpret_cast<const uint32_t*>(&h);
-            }
-            *reinterpret_cast<uint4*>(orow + c0 + q * 8) = make_uint4(o4[0], o4[1], o4[2], o4[3]);
-          }
-        }
-      }
+      if (row_ok) store_row_f16<HDP>(arow, inv, p.out + grow * p.ldo + head * HDP);
     }
   }
 }
 
 template <int HDP>
-static int launch_attn(const CUtensorMap& tm, const AttnParams& p, size_t smem, cudaStream_t st) {
+static int launch_attn(const CUtensorMap& tm, const CUtensorMap& tmb, const AttnParams& p, cudaStream_t st) {
+  const size_t smem = 1024 + AttnSmem<HDP>::BIAS_OFF + ((size_t)p.S * p.S * 4 + 15) / 16 * 16 + 128;
+  FVIT_CHECK(smem <= 227 * 1024, "fvit_attn_tc_fwd: needs %zu B of shared memory", smem);
   static bool configured = false;
   if (!configured) {
     FVIT_CUDA(cudaFuncSetAttribute(attn_tc_kernel<HDP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
@@ -265,7 +248,7 @@ static int launch_attn(const CUtensorMap& tm, const AttnParams& p, size_t smem, 
   }
   const int items = p.tiles * p.heads;
   const int slots = num_sms();
-  attn_tc_kernel<HDP><<<items < slots ? items : slots, AT_THREADS, smem, st>>>(tm, p);
+  attn_tc_kernel<HDP><<<items < slots ? items : slots, AT_THREADS, smem, st>>>(tm, tmb, p);
   return post_launch("attn_tc_kernel");
 }
 
@@ -278,7 +261,8 @@ extern "C" int fvit_attn_tc_fwd(const void* qkv, int64_t ldq, int32_t groups, in
                                 void* stream) {
   FVIT_CHECK(qkv && out && groups > 0 && heads > 0, "fvit_attn_tc_fwd: bad arguments");
   FVIT_CHECK(S >= 1 && S <= 128, "fvit_attn_tc_fwd: S=%d unsupported (1..128)", S);
-  FVIT_CHECK(hdp == 32 || hdp == 64, "fvit_attn_tc_fwd: padded head dim %d unsupported (32 or 64)", hdp);
+  FVIT_CHECK(hdp == 32 || hdp == 64 || hdp == 80, "fvit_attn_tc_fwd: padded head dim %d unsupported (32, 64 or 80)",
+             hdp);
   FVIT_CHECK(ldq % 8 == 0 && ldo % 8 == 0 && ldq >= 3 * heads * hdp && ldo >= heads * hdp,
              "fvit_attn_tc_fwd: bad leading dimensions");
   FVIT_CHECK((reinterpret_cast<uintptr_t>(out) & 15) == 0, "fvit_attn_tc_fwd: out must be 16-byte aligned");
@@ -294,20 +278,12 @@ extern "C" int fvit_attn_tc_fwd(const void* qkv, int64_t ldq, int32_t groups, in
   p.bias = bias;
   p.out = (__half*)out;
   p.ldo = ldo;
-  CUtensorMap tm;
-  {
-    uint64_t dims[2] = {(uint64_t)(3 * heads * hdp), (uint64_t)p.rows_total};
-    uint64_t strides[1] = {(uint64_t)ldq * 2};
-    uint32_t box[2] = {(uint32_t)hdp, (uint32_t)p.slot};
-    int rc = cached_tmap_16bit(&tm, qkv, 2, dims, strides, box,
-                               hdp == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
-    if (rc) return rc;
-  }
-  const size_t smem = 1024 + (hdp == 64 ? AttnSmem<64>::BIAS_OFF : AttnSmem<32>::BIAS_OFF) +
-                      ((size_t)S * S * 4 + 15) / 16 * 16 + 128;
-  FVIT_CHECK(smem <= 227 * 1024, "fvit_attn_tc_fwd: needs %zu B of shared memory", smem);
-  if (hdp == 64) return launch_attn<64>(tm, p, smem, (cudaStream_t)stream);
-  return launch_attn<32>(tm, p, smem, (cudaStream_t)stream);
+  CUtensorMap tm, tmb;
+  int rc = head_tile_tmaps(&tm, &tmb, qkv, 3 * heads * hdp, p.rows_total, ldq, hdp, p.slot);
+  if (rc) return rc;
+  if (hdp == 80) return launch_attn<80>(tm, tmb, p, (cudaStream_t)stream);
+  if (hdp == 64) return launch_attn<64>(tm, tmb, p, (cudaStream_t)stream);
+  return launch_attn<32>(tm, tmb, p, (cudaStream_t)stream);
 }
 
 // =====================================================================================================
@@ -332,10 +308,9 @@ struct AttnBwdParams {
 template <int HDP>
 __global__ void __launch_bounds__(AT_THREADS, 1)
     attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const __grid_constant__ CUtensorMap tmap_do,
+                       const __grid_constant__ CUtensorMap tmap_qkv_b, const __grid_constant__ CUtensorMap tmap_do_b,
                        const __grid_constant__ AttnBwdParams p) {
-  constexpr uint32_t SWZ = HDP == 64 ? SWZ_128B : SWZ_64B;
-  constexpr uint32_t ROW_BYTES = HDP * 2;
-  constexpr uint32_t SBO_QKV = 8 * ROW_BYTES;
+  using HT = HeadTile<HDP>;
   constexpr int TILE_BYTES = AT_ROWS * HDP * 2;
   constexpr int STAGE_BYTES = 4 * TILE_BYTES;  // Q, K, V, dO
   constexpr int NST = HDP == 32 ? 2 : 1;
@@ -357,6 +332,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
   if (warp == AT_PRODUCER && lane == 0) {
     tma_prefetch_desc(&tmap_qkv);
     tma_prefetch_desc(&tmap_do);
+    if (HT::HB > 0) tma_prefetch_desc(&tmap_qkv_b), tma_prefetch_desc(&tmap_do_b);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&ld_full[i], 1);
       mbar_init(&ld_empty[i], 1);
@@ -396,11 +372,10 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
         mbar_expect_tx(&ld_full[st], STAGE_BYTES);
         for (int sl = 0; sl < nslots; ++sl) {
           const int row0 = (tile * p.gpt + sl) * S;
-          uint8_t* dst = base + sl * p.slot * ROW_BYTES;
-          tma_load_2d(dst, &tmap_qkv, &ld_full[st], head * HDP, row0);
-          tma_load_2d(dst + TILE_BYTES, &tmap_qkv, &ld_full[st], (p.heads + head) * HDP, row0);
-          tma_load_2d(dst + 2 * TILE_BYTES, &tmap_qkv, &ld_full[st], (2 * p.heads + head) * HDP, row0);
-          tma_load_2d(dst + 3 * TILE_BYTES, &tmap_do, &ld_full[st], head * HDP, row0);
+          for (int op = 0; op < 3; ++op)
+            HT::load(base + op * TILE_BYTES, AT_ROWS, sl * p.slot, &tmap_qkv, &tmap_qkv_b, &ld_full[st],
+                     (op * p.heads + head) * HDP, row0);
+          HT::load(base + 3 * TILE_BYTES, AT_ROWS, sl * p.slot, &tmap_do, &tmap_do_b, &ld_full[st], head * HDP, row0);
         }
       }
     }
@@ -476,10 +451,9 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
       const uint32_t sK = sQ + TILE_BYTES, sV = sQ + 2 * TILE_BYTES, sDO = sQ + 3 * TILE_BYTES;
       const uint32_t sPu = smem_u32(sP), sDSu = smem_u32(sDS);
       named_bar_sync(1, 128);  // the previous item's gradient reads of the accumulator tile are done
-      wg_mma_128<128, 0, 0, HDP / 16>(
-          acc, AT_ACC_LD,
-          [&](int h, int k) { return make_smem_desc(sQ + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
-          [&](int k) { return make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ); }, false);
+      wg_mma_128<128, 0, 0, HT::KSTEPS>(
+          acc, AT_ACC_LD, [&](int h, int k) { return HT::kdesc(sQ, AT_ROWS, h * 64, k); },
+          [&](int k) { return HT::kdesc(sK, AT_ROWS, 0, k); }, false);
       named_bar_sync(1, 128);
       const float* brow = bias_s + (row_ok ? j : 0) * S;
       const bool use_bias = p.bias != nullptr;
@@ -515,10 +489,9 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
       }
       const float inv = row_ok ? 1.f / sum : 0.f;
       named_bar_sync(1, 128);  // every score read is done: dP = dO V^T overwrites the tile
-      wg_mma_128<128, 0, 0, HDP / 16>(
-          acc, AT_ACC_LD,
-          [&](int h, int k) { return make_smem_desc(sDO + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
-          [&](int k) { return make_smem_desc(sV + k * 32, 16, SBO_QKV, SWZ); }, false);
+      wg_mma_128<128, 0, 0, HT::KSTEPS>(
+          acc, AT_ACC_LD, [&](int h, int k) { return HT::kdesc(sDO, AT_ROWS, h * 64, k); },
+          [&](int k) { return HT::kdesc(sV, AT_ROWS, 0, k); }, false);
       named_bar_sync(1, 128);
       float delta = 0.f;
 #pragma unroll
@@ -575,41 +548,24 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
       for (int which = 0; which < 3; ++which) {
         named_bar_sync(1, 128);  // P / dS are complete, the previous tile reads are done
         if (which == 0) {        // dQ = dS K
-          wg_mma_128<HDP, 0, 1, 8>(
-          acc, AT_ACC_LD,
+          wg_mma_128_head<HDP, 0, 8>(
+              acc, AT_ACC_LD,
               [&](int h, int ks) {
                 return make_smem_desc(sDSu + (ks >> 2) * (AT_ROWS * 128) + h * 64 * 128 + (ks & 3) * 32, 16, 1024, SWZ_128B);
               },
-              [&](int ks) { return make_smem_desc(sK + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, false);
+              sK, AT_ROWS, false);
         } else {                 // dK = dS^T Q, dV = P^T dO: A read MN-major (M = keys), K = 128 query rows
           const uint32_t sA = which == 1 ? sDSu : sPu;
           const uint32_t sB = which == 1 ? sQ : sDO;
-          wg_mma_128<HDP, 1, 1, 8>(
-          acc, AT_ACC_LD,
+          wg_mma_128_head<HDP, 1, 8>(
+              acc, AT_ACC_LD,
               [&](int h, int ks) { return make_smem_desc(sA + h * (AT_ROWS * 128) + ks * 2048, AT_ROWS * 128, 1024, SWZ_128B); },
-              [&](int ks) { return make_smem_desc(sB + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, false);
+              sB, AT_ROWS, false);
         }
         named_bar_sync(1, 128);
         if (which == 2 && tid == 0) mbar_arrive(&ld_empty[st]);  // Q / K / V / dO of this stage are consumed
         const float mul = which == 2 ? 1.f : p.scale;
-#pragma unroll
-        for (int c0 = 0; c0 < HDP; c0 += 32) {
-          uint32_t raw[32];
-          ld_row32(arow + c0, raw);
-          if (row_ok) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              uint32_t o4[4];
-#pragma unroll
-              for (int u = 0; u < 4; ++u) {
-                const __half2 h = __floats2half2_rn(__uint_as_float(raw[q * 8 + 2 * u]) * mul,
-                                                    __uint_as_float(raw[q * 8 + 2 * u + 1]) * mul);
-                o4[u] = *reinterpret_cast<const uint32_t*>(&h);
-              }
-              *reinterpret_cast<uint4*>(orow + which * Cp + c0 + q * 8) = make_uint4(o4[0], o4[1], o4[2], o4[3]);
-            }
-          }
-        }
+        if (row_ok) store_row_f16<HDP>(arow, mul, orow + which * Cp);
       }
     }
     flush_dbias(staged_head);
@@ -617,8 +573,8 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
 }
 
 template <int HDP>
-static int launch_attn_bwd(const CUtensorMap& tq, const CUtensorMap& td, const AttnBwdParams& p, size_t smem,
-                           cudaStream_t st) {
+static int launch_attn_bwd(const CUtensorMap& tq, const CUtensorMap& td, const CUtensorMap& tqb, const CUtensorMap& tdb,
+                           const AttnBwdParams& p, size_t smem, cudaStream_t st) {
   static bool configured = false;
   if (!configured) {
     FVIT_CUDA(cudaFuncSetAttribute(attn_bwd_tc_kernel<HDP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
@@ -626,7 +582,7 @@ static int launch_attn_bwd(const CUtensorMap& tq, const CUtensorMap& td, const A
   }
   const int items = p.tiles * p.heads;
   const int sms = num_sms();
-  attn_bwd_tc_kernel<HDP><<<items < sms ? items : sms, AT_THREADS, smem, st>>>(tq, td, p);
+  attn_bwd_tc_kernel<HDP><<<items < sms ? items : sms, AT_THREADS, smem, st>>>(tq, td, tqb, tdb, p);
   return post_launch("attn_bwd_tc_kernel");
 }
 
@@ -638,7 +594,7 @@ extern "C" int fvit_attn_tc_bwd(const void* qkv, int64_t ldq, const void* dout, 
   using namespace fvit;
   FVIT_CHECK(qkv && dout && dqkv && groups > 0 && heads > 0, "fvit_attn_tc_bwd: bad arguments");
   FVIT_CHECK(S >= 1 && S <= 64, "fvit_attn_tc_bwd: S=%d unsupported (1..64)", S);
-  FVIT_CHECK(hdp == 32 || hdp == 64, "fvit_attn_tc_bwd: padded head dim %d unsupported", hdp);
+  FVIT_CHECK(hdp == 32 || hdp == 64 || hdp == 80, "fvit_attn_tc_bwd: padded head dim %d unsupported", hdp);
   FVIT_CHECK(ldq % 8 == 0 && lddo % 8 == 0 && lddq % 8 == 0, "fvit_attn_tc_bwd: bad leading dimensions");
   AttnBwdParams p;
   p.groups = groups, p.S = S, p.heads = heads, p.hd = head_dim;
@@ -650,23 +606,15 @@ extern "C" int fvit_attn_tc_bwd(const void* qkv, int64_t ldq, const void* dout, 
   p.bias = bias, p.dbias = dbias;
   p.dqkv = (__half*)dqkv, p.lddq = lddq;
   const int rows_total = groups * S;
-  CUtensorMap tq, td;
-  {
-    uint64_t dims[2] = {(uint64_t)(3 * heads * hdp), (uint64_t)rows_total};
-    uint64_t strides[1] = {(uint64_t)ldq * 2};
-    uint32_t box[2] = {(uint32_t)hdp, (uint32_t)p.slot};
-    int rc = cached_tmap_16bit(&tq, qkv, 2, dims, strides, box,
-                               hdp == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
-    if (rc) return rc;
-    uint64_t dims2[2] = {(uint64_t)(heads * hdp), (uint64_t)rows_total};
-    uint64_t strides2[1] = {(uint64_t)lddo * 2};
-    rc = cached_tmap_16bit(&td, dout, 2, dims2, strides2, box,
-                           hdp == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
-    if (rc) return rc;
-  }
+  CUtensorMap tq, td, tqb, tdb;
+  int rc = head_tile_tmaps(&tq, &tqb, qkv, 3 * heads * hdp, rows_total, ldq, hdp, p.slot);
+  if (rc) return rc;
+  rc = head_tile_tmaps(&td, &tdb, dout, heads * hdp, rows_total, lddo, hdp, p.slot);
+  if (rc) return rc;
   const size_t ss = ((size_t)S * S * 4 + 15) / 16 * 16;
   const size_t smem = 1024 + (size_t)(hdp == 32 ? 2 : 1) * 4 * AT_ROWS * hdp * 2 + 2 * AT_ROWS * 128 * 2 + AT_ACC_BYTES + ss + 128;
   FVIT_CHECK(smem <= 227 * 1024, "fvit_attn_tc_bwd: needs %zu B of shared memory", smem);
-  if (hdp == 64) return launch_attn_bwd<64>(tq, td, p, smem, (cudaStream_t)stream);
-  return launch_attn_bwd<32>(tq, td, p, smem, (cudaStream_t)stream);
+  if (hdp == 80) return launch_attn_bwd<80>(tq, td, tqb, tdb, p, smem, (cudaStream_t)stream);
+  if (hdp == 64) return launch_attn_bwd<64>(tq, td, tqb, tdb, p, smem, (cudaStream_t)stream);
+  return launch_attn_bwd<32>(tq, td, tqb, tdb, p, smem, (cudaStream_t)stream);
 }

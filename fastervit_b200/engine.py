@@ -629,7 +629,7 @@ class Plan:
         """Which attention core serves a window sequence of S tokens with padded head dim hdp: "tile" (one 128-row
         wgmma tile, fvit_attn_tc_fwd), "loop" (key-loop wgmma kernel for longer windows: its TMA-staged bias rows
         need S % 4 == 0) or "simt" (generic fallback for geometries neither covers)."""
-        if hdp > 64:
+        if hdp > 80:
             return "simt"
         if S <= 128:
             return "tile"
@@ -637,9 +637,9 @@ class Plan:
 
     @staticmethod
     def _head_pad(hd: int) -> int:
-        """Padded head dim of the tensor-core attention kernel (TMA boxes need 16-byte rows; the
-        kernel is instantiated for 32 and 64). Larger heads use the generic SIMT core unpadded."""
-        return 32 if hd <= 32 else (64 if hd <= 64 else hd)
+        """Padded head dim of the tensor-core attention kernels (TMA boxes need 16-byte rows; the
+        kernels are instantiated for 32, 64 and 80). Larger heads use the generic SIMT core unpadded."""
+        return 32 if hd <= 32 else (64 if hd <= 64 else (80 if hd <= 80 else hd))
 
     def _emit_attention(self, nm: str, attn, gamma, rows: int, groups: int, S: int, xin, ld_in, qkv, ao,
                         bias_buf, stream_buf) -> None:
@@ -653,7 +653,7 @@ class Plan:
         Cp = h * hdp
         wq, ldq, qb_ptr, wp, ldp = self._pack_attention(nm, attn, hdp)
         scale = float(getattr(attn, "scale", hd ** -0.5))   # qk_scale or head_dim ** -0.5 (fv.py:544)
-        fused = (self._attn_kind(S, hdp) == "tile" and self.fused_hat != "0"
+        fused = (self._attn_kind(S, hdp) == "tile" and self.fused_hat != "0" and hdp <= 64   # (fused kernel: 32 / 64)
                  and (self.fused_hat == "1" or hdp == 64))
         if fused:
             # ONE kernel: qkv projection + softmax(q k^T * scale + bias) + P v; the qkv matrix never reaches HBM

@@ -244,10 +244,11 @@ def _attn_fwd_train(self, nm: str, attn, gamma, rows: int, groups: int, S: int, 
     Cc, h, hd = attn.qkv.in_features, attn.num_heads, attn.head_dim
     hdp = self._head_pad(hd)
     kind = self._attn_kind(S, hdp)
-    if kind == "tile" and S > 64 and S % 4 == 0:
+    if kind == "tile" and S % 4 == 0 and _attn_bwd_entry(S, hdp, True) != "fvit_attn_tc_bwd":
         # one window per 128-row tile either way; the key-loop forward also writes the log-sum-exp rows its tensor-core
-        # backward needs (fvit_attn_tc_bwd stops at 64-row window slots: without this, 65..128-token windows -- any-res
-        # models with 8 x 8 ... 11 x 11 windows -- would train through the SIMT backward)
+        # backward needs (fvit_attn_tc_bwd stops at 64-row window slots, and at 63 tokens for 80-wide heads: without
+        # this, 65..128-token windows -- any-res models with 8 x 8 ... 11 x 11 windows -- would train through the SIMT
+        # backward)
         kind = "loop"
     use_tc = kind != "simt"
     if not use_tc:
@@ -605,8 +606,9 @@ def _emit_attn_core_bwd(self, at: dict, dao, dqkv, groups: int, S: int, want_dbi
 
 
 def _attn_bwd_entry(S: int, hdp: int, use_tc: bool) -> str:
-    """tensor-core attention backward when the tile fits (S <= 64, head slices of 32/64, shared memory budget)"""
-    if use_tc and S <= 64 and hdp in (32, 64):
+    """tensor-core attention backward when the tile fits (S <= 64, head slices of 32/64/80, shared memory budget:
+    S <= 63 at 80)"""
+    if use_tc and S <= 64 and hdp in (32, 64, 80):
         ss = (S * S * 4 + 15) // 16 * 16
         if 1024 + (2 if hdp == 32 else 1) * 4 * 128 * hdp * 2 + 2 * 128 * 128 * 2 + 128 * 132 * 4 + ss + 128 <= 227 * 1024:
             return "fvit_attn_tc_bwd"

@@ -231,7 +231,8 @@ int fvit_attn_core_fwd(const void* qkv, int64_t ldq, int32_t groups, int32_t S, 
 /* Tensor-core version of the same attention core (wgmma: S = QK^T and O = PV with fp32 accumulators
  * staged in shared memory, TMA-staged head slices, per-row softmax; scores and probabilities never
  * leave the SM). qkv fp16 [groups*S, 3*heads*hdp] with head_dim zero-padded to
- * hdp in {32, 64}; out fp16 [groups*S, heads*hdp]; S <= 128. bias fp32 [heads, S, S] or NULL. */
+ * hdp in {32, 64, 80}; out fp16 [groups*S, heads*hdp]; S <= 128. bias fp32 [heads, S, S] or NULL. At hdp 80 a head
+ * slice is staged as a 64-column 128B-swizzled box plus a 16-column 32B-swizzled box. */
 int fvit_attn_tc_fwd(const void* qkv, int64_t ldq, int32_t groups, int32_t S, int32_t heads, int32_t hdp,
                      const float* bias, float scale, void* out, int64_t ldo, void* stream);
 
@@ -249,7 +250,8 @@ int fvit_hat_attn_fwd(const void* xn16, int64_t ldx, int32_t C, const void* wqkv
 /* Key-loop tensor-core attention core for window sequences longer than one 128-row tile (any-res level 2:
  * S = 12*12 + 4 = 148, faster_vit_any_res.py:805-817; 21k windows S = 196 .. 2304, faster_vit.py:1253-1418):
  * work item = (window, head, 128 query rows); key tiles of 128 are visited twice (row maxima, then probabilities and
- * O += P V in an fp32 shared-memory accumulator). Same qkv / out layout as fvit_attn_tc_fwd; bias [heads, S, S] fp32 is staged by TMA, so
+ * O += P V in an fp32 shared-memory accumulator). Same qkv / out layout (hdp in {32, 64, 80}) as fvit_attn_tc_fwd;
+ * bias [heads, S, S] fp32 is staged by TMA, so
  * S % 4 == 0 is required when a bias is given. lse (optional, [groups*S, heads] fp32) receives the log2-domain
  * log-sum-exp of the scaled, biased scores (saved for the backward pass). */
 int fvit_attn_loop_fwd(const void* qkv, int64_t ldq, int32_t groups, int32_t S, int32_t heads, int32_t hdp,
@@ -433,13 +435,16 @@ int fvit_ln_bwd(const void* dy16, int64_t lddy, const int32_t* dy_map, const voi
 int fvit_attn_core_bwd(const void* qkv, int64_t ldq, const void* dout, int64_t lddo, int32_t groups, int32_t S,
                        int32_t heads, int32_t head_dim, int32_t hdp, const float* bias, float scale, void* dqkv,
                        int64_t lddq, float* dbias, void* stream);
-/* Tensor-core version for S <= 64 and hdp in {32, 64} (wgmma: S = QK^T, dP = dO V^T, then dV = P^T dO,
- * dK = dS^T Q, dQ = dS K with the P / dS tiles read as MN-major / K-major operands); same contract. */
+/* Tensor-core version for S <= 64 and hdp in {32, 64, 80} (wgmma: S = QK^T, dP = dO V^T, then dV = P^T dO,
+ * dK = dS^T Q, dQ = dS K with the P / dS tiles read as MN-major / K-major operands); same contract. At hdp 80 the
+ * shared-memory layout leaves room for S <= 63 (S = 64 returns an error: the training plans send it to
+ * fvit_attn_loop_fwd / fvit_attn_loop_bwd_long). */
 int fvit_attn_tc_bwd(const void* qkv, int64_t ldq, const void* dout, int64_t lddo, int32_t groups, int32_t S,
                      int32_t heads, int32_t head_dim, int32_t hdp, const float* bias, float scale, void* dqkv,
                      int64_t lddq, float* dbias, void* stream);
-/* Tensor-core backward for windows longer than the tile kernel takes, the mirror of fvit_attn_loop_fwd (any S with
- * S % 4 == 0; the training plans use it from 65 tokens on): any-res S = 148, the 24 x 24 / 32 x 32 / 48 x 48 windows of
+/* Tensor-core backward for windows longer than the tile kernel takes, the mirror of fvit_attn_loop_fwd (hdp in
+ * {32, 64, 80}; any S with S % 4 == 0 whose two 128-entry row vectors per query tile fit in shared memory: S <= 1664 at
+ * hdp 80; the training plans use it from 65 tokens on, from 64 at hdp 80): any-res S = 148, the 24 x 24 / 32 x 32 / 48 x 48 windows of
  * the 21k models (fv.py:1253-1418, WindowAttention.forward fv.py:557-568 differentiated). Needs the forward's output
  * `out` (for delta = rowsum(dO * O)) and its log-sum-exp vector `lse`. Key tiles outside, query tiles inside; dV_j /
  * dK_j accumulate in registers over the query loop, the per-pair partial dQ_i = dS K_j is added to the row of the fp32
