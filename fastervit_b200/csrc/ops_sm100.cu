@@ -998,7 +998,9 @@ int fvit_ln_fwd(const float* x, int64_t ldx, const int32_t* in_map, int32_t rows
                 void* stream) {
   FVIT_CHECK(x && gamma && beta && out && rows > 0, "fvit_ln_fwd: bad arguments");
   FVIT_CHECK(!xhat_out || ldxh % 4 == 0, "fvit_ln_fwd: xhat stride must be a multiple of 4");
-  FVIT_CHECK(C % 4 == 0 && C <= 32 * 4 * 16, "fvit_ln_fwd: C=%d unsupported", C);
+  static_assert(FVIT_LN_MAX_C == 32 * 4 * 20, "the widest ln_fwd_kernel instantiation holds FVIT_LN_MAX_C channels");
+  FVIT_CHECK(C % 4 == 0 && C <= FVIT_LN_MAX_C, "fvit_ln_fwd: C=%d unsupported (C %% 4 == 0, C <= %d)", C,
+             FVIT_LN_MAX_C);
   FVIT_CHECK(ldx % 4 == 0 && ldo % 4 == 0 && (!wb || ldwb % 4 == 0), "fvit_ln_fwd: unaligned strides");
   FVIT_CHECK(!add || group > 0, "fvit_ln_fwd: add needs group > 0");
   const int nvec = C / 4;
@@ -1017,7 +1019,8 @@ int fvit_ln_fwd(const float* x, int64_t ldx, const int32_t* in_map, int32_t rows
   else if (nvec <= 64) FVIT_LN_LAUNCH(16, 4);
   else if (nvec <= 128) FVIT_LN_LAUNCH(32, 4);
   else if (nvec <= 256) FVIT_LN_LAUNCH(32, 8);
-  else FVIT_LN_LAUNCH(32, 16);
+  else if (nvec <= 512) FVIT_LN_LAUNCH(32, 16);
+  else FVIT_LN_LAUNCH(32, 20);  // FasterViT-5 / -6 level 3 (2560 channels)
 #undef FVIT_LN_LAUNCH
   return post_launch("ln_fwd_kernel");
 }

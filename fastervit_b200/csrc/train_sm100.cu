@@ -498,7 +498,9 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-constexpr int LNB_MAXV = 7;  // 8-half vectors per lane: C <= 32 * 8 * 7 = 1792
+constexpr int LNB_MAXV = 7;       // 8-half vectors per lane: C <= 32 * 8 * 7 = 1792
+constexpr int LNB_MAXV_WIDE = 10;  // FasterViT-5 / -6 level 3: C <= 32 * 8 * 10 = 2560
+static_assert(32 * 8 * LNB_MAXV_WIDE == FVIT_LN_MAX_C, "the vectorised LayerNorm backward takes every fvit_ln_fwd width");
 // Vectorised dx part (C % 8 == 0): one warp per row, the row's dy / xhat live in registers between the two
 // passes. MAXV (vectors per lane) is a template parameter so narrow rows do not pay for wide rows' registers.
 template <int MAXV, bool PREFETCH_G>
@@ -1696,19 +1698,20 @@ static void ln_dx_launch(const __half* dyh, int64_t lddy, const int32_t* dy_map,
     const char* e = getenv("FVIT_LN_PREFETCH");
     prefetch_g = e ? atoi(e) : 1;
   }
-#define FVIT_LN_DX(MV)                                                                                              \
-  do {                                                                                                              \
-    if (prefetch_g)                                                                                                 \
-      ln_bwd_dx_kernel<MV, true><<<(unsigned)grid, block, 0, st>>>(dyh, lddy, dy_map, xhh, ldxh, rstd, gamma, rows, C, g, \
-                                                                   ldg, in_map, use_g, clear_moved);                \
-    else                                                                                                            \
-      ln_bwd_dx_kernel<MV, false><<<(unsigned)grid, block, 0, st>>>(dyh, lddy, dy_map, xhh, ldxh, rstd, gamma, rows, C, g, \
-                                                                    ldg, in_map, use_g, clear_moved);               \
+#define FVIT_LN_DX(MV, PF)                                                                                          \
+  ln_bwd_dx_kernel<MV, PF><<<(unsigned)grid, block, 0, st>>>(dyh, lddy, dy_map, xhh, ldxh, rstd, gamma, rows, C, g, ldg, \
+                                                             in_map, use_g, clear_moved)
+#define FVIT_LN_DX_AB(MV)                  \
+  do {                                     \
+    if (prefetch_g) FVIT_LN_DX(MV, true);  \
+    else FVIT_LN_DX(MV, false);            \
   } while (0)
-  if (nvl <= 1) FVIT_LN_DX(1);
-  else if (nvl <= 2) FVIT_LN_DX(2);
-  else if (nvl <= 4) FVIT_LN_DX(4);
-  else FVIT_LN_DX(LNB_MAXV);
+  if (nvl <= 1) FVIT_LN_DX_AB(1);
+  else if (nvl <= 2) FVIT_LN_DX_AB(2);
+  else if (nvl <= 4) FVIT_LN_DX_AB(4);
+  else if (nvl <= LNB_MAXV) FVIT_LN_DX_AB(LNB_MAXV);
+  else FVIT_LN_DX(LNB_MAXV_WIDE, false);  // prefetching g at ten vectors per lane spills past 255 registers
+#undef FVIT_LN_DX_AB
 #undef FVIT_LN_DX
 }
 
@@ -1718,7 +1721,7 @@ int fvit_ln_bwd(const void* dy16, int64_t lddy, const int32_t* dy_map, const voi
                 float* dbeta, void* stream) {
   FVIT_CHECK(dy16 && xhat16 && rstd && gamma && g && dgamma && dbeta && rows > 0 && C > 0,
              "fvit_ln_bwd: bad arguments");
-  const bool vec = C % 8 == 0 && C <= 32 * 8 * LNB_MAXV && lddy % 8 == 0 && ldxh % 8 == 0 && ldg % 4 == 0;
+  const bool vec = C % 8 == 0 && C <= 32 * 8 * LNB_MAXV_WIDE && lddy % 8 == 0 && ldxh % 8 == 0 && ldg % 4 == 0;
   const int block = 256, wpb = 8;
   long long grid = ((long long)rows + wpb - 1) / wpb;
   const cudaStream_t st = (cudaStream_t)stream;
@@ -1757,7 +1760,7 @@ int fvit_ln_dgrad(const void* dy16, int64_t lddy, const int32_t* dy_map, const v
                   const int32_t* in_map, int32_t use_g, int32_t clear_moved, void* stream) {
   FVIT_CHECK(dy16 && xhat16 && rstd && gamma && g && rows > 0 && C > 0, "fvit_ln_dgrad: bad arguments");
   const cudaStream_t st = (cudaStream_t)stream;
-  if (C % 8 == 0 && C <= 32 * 8 * LNB_MAXV && lddy % 8 == 0 && ldxh % 8 == 0 && ldg % 4 == 0) {
+  if (C % 8 == 0 && C <= 32 * 8 * LNB_MAXV_WIDE && lddy % 8 == 0 && ldxh % 8 == 0 && ldg % 4 == 0) {
     ln_dx_launch((const __half*)dy16, lddy, dy_map, (const __half*)xhat16, ldxh, rstd, gamma, rows, C, g, ldg, in_map,
                  use_g, clear_moved, st);
     return post_launch("ln_bwd_dx_kernel");

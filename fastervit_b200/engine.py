@@ -26,6 +26,7 @@ import torch.nn as nn
 from . import lib as L
 
 STEM_MAX_CIN = 64   # in_chans limit of the stem kernels (FVIT_STEM_MAX_CIN, include/fvit.h)
+LN_MAX_C = 2560     # widest LayerNorm row of fvit_ln_fwd / fvit_ln_bwd / fvit_ln_dgrad (FVIT_LN_MAX_C, include/fvit.h)
 
 
 def _ru(x: int, m: int) -> int:
@@ -228,6 +229,7 @@ class Plan:
         self._x_static = None
         self._deploy_mods: list = []
         self.marks: list[tuple[int, str, dict]] = []   # (ops issued so far, reference module name, where its output lives)
+        self.check_ln_widths()
         self._build()
 
     # ---- per-module activation taps (parity tests against the reference's forward hooks) ---------
@@ -445,6 +447,15 @@ class Plan:
         if not 1 <= cin <= STEM_MAX_CIN:
             raise L.FvitError(f"in_chans={cin}: the stem kernels support 1 <= in_chans <= {STEM_MAX_CIN}")
         return 9 * cin, (self.STEM_LD if cin == 3 else _ru(9 * cin, 32))
+
+    def check_ln_widths(self) -> None:
+        """Raise FvitError for a model whose LayerNorm rows (a Downsample's channel norm, the norms of the transformer
+        blocks) are wider than the LayerNorm kernels take, before any buffer is allocated or kernel launched."""
+        for i, level in enumerate(self.model.levels):
+            normed = level.downsample is not None or (not level.conv and len(level.blocks) > 0)
+            if normed and level.dim > LN_MAX_C:
+                raise L.FvitError(f"level {i}: {level.dim}-channel LayerNorm rows, but the LayerNorm kernels take at "
+                                  f"most {LN_MAX_C} channels")
 
     def _s2_taps(self, Wo: int) -> list[tuple[int, int]]:
         """9 taps of a 3x3 stride-2 pad-1 convolution over the parity-plane layout: input row 2*oh+r-1

@@ -213,7 +213,11 @@ int fvit_stem_im2col(const float* x, int64_t sb, int64_t sc, int64_t sh, int64_t
  *   wb[r] = v (optional fp32 write-back of the updated residual stream)
  *   out[out_map ? out_map[r] : r] = (half)((v - mean) * rstd * gamma + beta)
  * mean_out / rstd_out (optional) receive the row statistics and xhat_out (optional, fp16 [rows, ldxh])
- * the normalised pre-affine rows for the backward pass. */
+ * the normalised pre-affine rows for the backward pass.
+ * C % 4 == 0 and C <= FVIT_LN_MAX_C. One warp per row with the row in registers: ln_fwd_kernel<LPR, MAXV> with LPR
+ * lanes per row and MAXV float4 per lane, chosen by C / 4: <= 16 <8, 2>, <= 32 <8, 4>, <= 64 <16, 4>, <= 128 <32, 4>,
+ * <= 256 <32, 8>, <= 512 <32, 16>, <= 640 <32, 20> (FasterViT-5 / -6 level 3, C = 2560). */
+#define FVIT_LN_MAX_C 2560
 int fvit_ln_fwd(const float* x, int64_t ldx, const int32_t* in_map, int32_t rows, int32_t C,
                 const float* add, int32_t group, int32_t skip, float* wb, int64_t ldwb,
                 const float* gamma, const float* beta, float eps, void* out, int64_t ldo,
@@ -425,7 +429,12 @@ int fvit_group_sum(const float* a, int64_t lda, int32_t ngroups, int32_t group, 
 /* LayerNorm backward for the forward of fvit_ln_fwd (same row maps): with gv = (use_g ? g[r] : 0) +
  * rstd[r]*(gamma*dy - mean(gamma*dy) - xhat*mean(gamma*dy*xhat)):  g[in_map ? in_map[r] : r] = gv (with
  * clear_moved, g[r] is zeroed when the source is another row — r must then index rows of g); dgamma[c] += *scalar*sum dy*xhat; dbeta[c] += *scalar*sum dy.
- * dy16 rows through dy_map (rows with dy_map < 0 are skipped). */
+ * dy16 rows through dy_map (rows with dy_map < 0 are skipped).
+ * Any C > 0. With C % 8 == 0, C <= FVIT_LN_MAX_C, lddy and ldxh multiples of 8 and ldg a multiple of 4, g is updated
+ * by the vectorised ln_bwd_dx_kernel<MAXV, PREFETCH_G> (one warp per row, the row's dy and xhat in registers, MAXV
+ * 8-half vectors per lane: 1, 2, 4, 7 up to C = 1792, 10 up to C = 2560 without prefetching g, which would spill) and
+ * dgamma / dbeta by ln_bwd_param_kernel; any other row goes to ln_bwd_generic_kernel (scalar loads, per-CTA partial
+ * sums in 64 * C bytes of shared memory). */
 int fvit_ln_bwd(const void* dy16, int64_t lddy, const int32_t* dy_map, const void* xhat16, int64_t ldxh,
                 const float* rstd, const float* gamma, int32_t rows, int32_t C, float* g, int64_t ldg,
                 const int32_t* in_map, int32_t use_g, int32_t clear_moved, const float* scalar, float* dgamma,
@@ -549,7 +558,9 @@ int fvit_bn_eval_dgrad(const void* gin, int32_t g_is_f16, int64_t ldg, const int
                        int64_t ldr, const int32_t* r_rows, int32_t nrows, int32_t C, const float* scale,
                        const float* shift, int32_t act, const float* colmul, const float* scalar, void* out16,
                        int64_t ldo, const int32_t* o_rows, void* stream);
-/* The g update of fvit_ln_bwd without dgamma / dbeta (same dy_map / in_map / use_g / clear_moved conventions). */
+/* The g update of fvit_ln_bwd without dgamma / dbeta (same dy_map / in_map / use_g / clear_moved conventions). The same
+ * ln_bwd_dx_kernel serves the same widths, so its g equals fvit_ln_bwd's bit for bit there; other rows go to
+ * ln_dgrad_generic_kernel. */
 int fvit_ln_dgrad(const void* dy16, int64_t lddy, const int32_t* dy_map, const void* xhat16, int64_t ldxh,
                   const float* rstd, const float* gamma, int32_t rows, int32_t C, float* g, int64_t ldg,
                   const int32_t* in_map, int32_t use_g, int32_t clear_moved, void* stream);
