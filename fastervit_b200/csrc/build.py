@@ -7,7 +7,6 @@ objects go to fastervit_b200/csrc/build/.
 from __future__ import annotations
 
 import hashlib
-import os
 import shutil
 import subprocess
 import sys
@@ -17,12 +16,8 @@ from pathlib import Path
 CSRC = Path(__file__).resolve().parent
 PKG = CSRC.parent
 ROOT = PKG.parent
-# A/B builds: FVIT_BUILD_DEFINES="-D..." FVIT_BUILD_OUT=libfvit_sm100_ab.so python -m fastervit_b200.csrc.build
-# (select at run time with FVIT_LIB=<path>); the default build takes neither.
-_EXTRA = os.environ.get("FVIT_BUILD_DEFINES", "").split()
-_OUT = os.environ.get("FVIT_BUILD_OUT", "libfvit_sm100.so")
-LIB_PATH = PKG / _OUT
-OBJ_DIR = CSRC / ("build" if _OUT == "libfvit_sm100.so" else "build_" + Path(_OUT).stem)
+LIB_PATH = PKG / "libfvit_sm100.so"
+OBJ_DIR = CSRC / "build"
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -30,7 +25,6 @@ NVCC_FLAGS = [
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
     "-I", str(ROOT / "include"),
-    *_EXTRA,
 ]
 
 

@@ -1042,14 +1042,9 @@ static int select_variant(const fvit_gemm_args* a, uint32_t* variant) {
   if (a->bf16) return 0;  // bf16 operands: only the generic kernel instantiates their MMAs
   {
     // row-per-thread epilogue (EF_DIRECT): 16-bit outputs only, everything a lane touches in 32-byte pieces
-    static int direct = -1;  // FVIT_GEMM_DIRECT=0: staging-tile epilogue everywhere (A/B)
-    if (direct < 0) {
-      const char* e = getenv("FVIT_GEMM_DIRECT");
-      direct = e ? atoi(e) : 1;
-    }
     auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
     const uint32_t allowed = EF_O16 | EF_PRE | EF_PREGRAD | EF_ALPHAPTR | EF_OSUM | (7u << EF_ACT_SHIFT);
-    const bool ok = direct && (feat & ~allowed) == 0 && (feat & EF_O16) && b_ntaps == 1 && a->n % 16 == 0 &&
+    const bool ok = (feat & ~allowed) == 0 && (feat & EF_O16) && b_ntaps == 1 && a->n % 16 == 0 &&
                     a->ld_out_f16 % 16 == 0 && al32(a->out_f16) &&
                     (!a->out_pre16 || (a->ld_out_pre16 % 16 == 0 && al32(a->out_pre16))) &&
                     (!a->aux || (a->ld_aux % 16 == 0 && al32(a->aux))) &&
@@ -1132,13 +1127,8 @@ extern "C" int fvit_gemm(const fvit_gemm_args* a, void* stream) {
   p.kb_per_tap = ceil_div(a->kc, BK);
   p.num_kb = num_kb;
   {
-    static int kskip = -1;  // FVIT_GEMM_KSKIP=0: issue the zero-filled K steps too (A/B)
-    if (kskip < 0) {
-      const char* e = getenv("FVIT_GEMM_KSKIP");
-      kskip = e ? atoi(e) : 1;
-    }
     const int tail = a->kc - (p.kb_per_tap - 1) * BK;  // 1..64 real columns in the last block
-    p.k_tail16 = kskip ? ceil_div(tail, MMA_K) : BK / MMA_K;
+    p.k_tail16 = ceil_div(tail, MMA_K);
   }
   p.a_mn = a->a_mn_major ? 1 : 0;
   p.b_mn = a->b_mn_major ? 1 : 0;

@@ -52,11 +52,11 @@ template <int HDP>
 __global__ void __launch_bounds__(HT_THREADS, 1)
     hat_attn_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                     const __grid_constant__ HatParams p) {
-  constexpr uint32_t SWZ = HDP == 64 ? SWZ_128B : SWZ_64B;
+  static_assert(HDP == 64, "the Q / K / V operand tiles are 128-byte rows in the 128B swizzle");
   constexpr uint32_t ROW_BYTES = HDP * 2;
   constexpr uint32_t SBO_QKV = 8 * ROW_BYTES;
   constexpr int A_BYTES = HT_ROWS * HT_BK * 2;        // 16 KB
-  constexpr int B_BYTES = 3 * HDP * HT_BK * 2;        // 24 KB / 12 KB
+  constexpr int B_BYTES = 3 * HDP * HT_BK * 2;        // 24 KB
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   constexpr int OPER_BYTES = HT_ROWS * HDP * 2;       // one of Q / K / V as fp16 operand tile
   extern __shared__ uint8_t smem_raw[];
@@ -126,10 +126,9 @@ __global__ void __launch_bounds__(HT_THREADS, 1)
         *reinterpret_cast<uint4*>(s_p + (c >> 6) * (HT_ROWS * 128) + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4)) =
             make_uint4(0, 0, 0, 0);
     }
-    // byte offset of element (row, col) inside a Q / K / V operand tile (128B / 64B swizzle)
+    // byte offset of element (row, col) inside a Q / K / V operand tile (128B swizzle)
     auto oper_off = [&](int row, int col) -> uint32_t {
-      if (HDP == 64) return (uint32_t)(row * 128 + ((((col >> 3) ^ (row & 7))) << 4) + (col & 7) * 2);
-      return (uint32_t)(row * 64 + ((((col >> 3) ^ ((row >> 1) & 3))) << 4) + (col & 7) * 2);
+      return (uint32_t)(row * 128 + ((((col >> 3) ^ (row & 7))) << 4) + (col & 7) * 2);
     };
     int stage = 0;
     uint32_t phase = 0, it = 0;
@@ -223,8 +222,8 @@ __global__ void __launch_bounds__(HT_THREADS, 1)
       // ---- (2) scores and softmax over the window's keys
       wg_mma_128<128, 0, 0, HDP / 16>(
           sacc, HT_ACC_LD,
-          [&](int h, int k) { return make_smem_desc(sQ + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ); },
-          [&](int k) { return make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ); }, false);
+          [&](int h, int k) { return make_smem_desc(sQ + h * 64 * ROW_BYTES + k * 32, 16, SBO_QKV, SWZ_128B); },
+          [&](int k) { return make_smem_desc(sK + k * 32, 16, SBO_QKV, SWZ_128B); }, false);
       named_bar_sync(1, 128);
       const float* brow = bias_s + (row_ok ? j : 0) * S;
       const bool use_bias = p.bias != nullptr;
@@ -280,7 +279,7 @@ __global__ void __launch_bounds__(HT_THREADS, 1)
           [&](int h, int ks) {
             return make_smem_desc(sPu + (ks >> 2) * (HT_ROWS * 128) + h * 64 * 128 + (ks & 3) * 32, 16, 1024, SWZ_128B);
           },
-          [&](int ks) { return make_smem_desc(sV + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ); }, false);
+          [&](int ks) { return make_smem_desc(sV + ks * 16 * ROW_BYTES, 0, SBO_QKV, SWZ_128B); }, false);
       named_bar_sync(1, 128);
       const float inv = row_ok ? 1.f / sum : 0.f;
       __half* orow = p.out + grow * p.ldo + head * HDP;
@@ -340,7 +339,7 @@ extern "C" int fvit_hat_attn_fwd(const void* xn16, int64_t ldx, int32_t C, const
                                  void* stream) {
   FVIT_CHECK(xn16 && wqkv16 && out && groups > 0 && heads > 0 && C > 0, "fvit_hat_attn_fwd: bad arguments");
   FVIT_CHECK(S >= 1 && S <= 128, "fvit_hat_attn_fwd: S=%d unsupported (1..128)", S);
-  FVIT_CHECK(hdp == 32 || hdp == 64, "fvit_hat_attn_fwd: padded head dim %d unsupported (32 or 64)", hdp);
+  FVIT_CHECK(hdp == 64, "fvit_hat_attn_fwd: padded head dim %d unsupported (64 only)", hdp);
   FVIT_CHECK(ldx % 8 == 0 && ldw % 8 == 0 && ldo % 8 == 0 && ldo >= heads * hdp, "fvit_hat_attn_fwd: bad leading dimensions");
   FVIT_CHECK(!qkv_out || (ldq % 8 == 0 && ldq >= 3 * heads * hdp), "fvit_hat_attn_fwd: bad qkv_out leading dimension");
   FVIT_CHECK((reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(qkv_out) & 15) == 0,
@@ -371,6 +370,5 @@ extern "C" int fvit_hat_attn_fwd(const void* xn16, int64_t ldx, int32_t C, const
     rc = cached_tmap_16bit(&tw, wqkv16, 2, dimsw, stridesw, boxw, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  if (hdp == 64) return launch_hat<64>(tx, tw, p, (cudaStream_t)stream);
-  return launch_hat<32>(tx, tw, p, (cudaStream_t)stream);
+  return launch_hat<64>(tx, tw, p, (cudaStream_t)stream);
 }

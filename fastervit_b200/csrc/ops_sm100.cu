@@ -1032,15 +1032,7 @@ int fvit_attn_core_fwd(const void* qkv, int64_t ldq, int32_t groups, int32_t S, 
              "fvit_attn_core_fwd: bad arguments");
   const int C = heads * head_dim;
   const size_t smem = ((size_t)3 * S * (head_dim + 1) + (size_t)S * (S + 1)) * sizeof(float);
-  // FVIT_ATTN_STREAM_MIN_S=<S>: experiment switch — also route windows with S >= <S> that would fit the one-shot kernel
-  // through the streaming kernel (3 CTAs per SM instead of 1 at S = 148); unset = shared-memory limit only
-  static int stream_min_s = -1;
-  if (stream_min_s < 0) {
-    const char* e = getenv("FVIT_ATTN_STREAM_MIN_S");
-    stream_min_s = e ? atoi(e) : 0;
-  }
-  const bool force_stream = stream_min_s > 0 && S >= stream_min_s && probs_out == nullptr;
-  if (smem > 227 * 1024 || force_stream) {  // large windows (21k models): stream the keys, 64 x 64 score tiles
+  if (smem > 227 * 1024) {  // large windows (21k models): stream the keys, 64 x 64 score tiles
     FVIT_CHECK(probs_out == nullptr, "fvit_attn_core_fwd: probs_out is not available for S=%d (streaming kernel)", S);
     const size_t sm2 = ((size_t)(2 * ATT_QT + 2 * ATT_KT) * (head_dim + 1) + (size_t)ATT_QT * (ATT_KT + 1) +
                         3 * ATT_QT) * sizeof(float);

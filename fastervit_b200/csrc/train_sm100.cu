@@ -1693,25 +1693,15 @@ static void ln_dx_launch(const __half* dyh, int64_t lddy, const int32_t* dy_map,
   const long long cap = (long long)num_sms() * 16;
   if (grid > cap) grid = cap;
   const int nvl = (C / 8 + 31) / 32;
-  static int prefetch_g = -1;  // fetch g with the operands instead of after the warp reductions ; FVIT_LN_PREFETCH=0 = A/B
-  if (prefetch_g < 0) {
-    const char* e = getenv("FVIT_LN_PREFETCH");
-    prefetch_g = e ? atoi(e) : 1;
-  }
+  // up to LNB_MAXV vectors per lane, g is fetched with the operands instead of after the warp reductions
 #define FVIT_LN_DX(MV, PF)                                                                                          \
   ln_bwd_dx_kernel<MV, PF><<<(unsigned)grid, block, 0, st>>>(dyh, lddy, dy_map, xhh, ldxh, rstd, gamma, rows, C, g, ldg, \
                                                              in_map, use_g, clear_moved)
-#define FVIT_LN_DX_AB(MV)                  \
-  do {                                     \
-    if (prefetch_g) FVIT_LN_DX(MV, true);  \
-    else FVIT_LN_DX(MV, false);            \
-  } while (0)
-  if (nvl <= 1) FVIT_LN_DX_AB(1);
-  else if (nvl <= 2) FVIT_LN_DX_AB(2);
-  else if (nvl <= 4) FVIT_LN_DX_AB(4);
-  else if (nvl <= LNB_MAXV) FVIT_LN_DX_AB(LNB_MAXV);
+  if (nvl <= 1) FVIT_LN_DX(1, true);
+  else if (nvl <= 2) FVIT_LN_DX(2, true);
+  else if (nvl <= 4) FVIT_LN_DX(4, true);
+  else if (nvl <= LNB_MAXV) FVIT_LN_DX(LNB_MAXV, true);
   else FVIT_LN_DX(LNB_MAXV_WIDE, false);  // prefetching g at ten vectors per lane spills past 255 registers
-#undef FVIT_LN_DX_AB
 #undef FVIT_LN_DX
 }
 
@@ -1865,12 +1855,7 @@ int fvit_bn_bwd(const void* gin, int32_t g_is_f16, int64_t ldg, const int32_t* g
   const bool vec = C % 4 == 0 && ldg % 4 == 0 && ldr % 4 == 0 && ldo % 4 == 0 &&
                    (reinterpret_cast<uintptr_t>(gin) % 16 == 0) && (reinterpret_cast<uintptr_t>(raw16) % 8 == 0) &&
                    (reinterpret_cast<uintptr_t>(out16) % 8 == 0);
-  static int bn_v8 = -1;  // FVIT_BN_V8=0 selects the 4-channel kernels (A/B)
-  if (bn_v8 < 0) {
-    const char* e = getenv("FVIT_BN_V8");
-    bn_v8 = e ? atoi(e) : 1;
-  }
-  const bool vec8 = bn_v8 && vec && ldr % 8 == 0 && ldo % 8 == 0 && (g_is_f16 ? ldg % 8 == 0 : true) &&
+  const bool vec8 = vec && ldr % 8 == 0 && ldo % 8 == 0 && (g_is_f16 ? ldg % 8 == 0 : true) &&
                     (reinterpret_cast<uintptr_t>(raw16) % 16 == 0) && (reinterpret_cast<uintptr_t>(out16) % 16 == 0) &&
                     (reinterpret_cast<uintptr_t>(gin) % 16 == 0);
   if (vec8) {

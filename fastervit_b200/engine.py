@@ -210,21 +210,10 @@ class Plan:
         self._gemm_keep: list = []        # keeps ctypes structs alive
         self._x_args: list = []           # stem-conv calls that take the input pointer at run time
         self.op_flops: dict[int, float] = {}  # op index -> algorithmic FLOPs (GEMM launches)
-        # FVIT_FUSED_HAT=0 falls back to the three-launch attention (qkv GEMM, attention core, proj GEMM) for A/B runs
-        # FVIT_FUSED_HAT: "0" = always the three-launch attention (qkv GEMM, attention core, proj GEMM), "1" = the fused
-        # kernel wherever it applies; default = fused for 64-wide (padded) heads, where the projection is long enough to
-        # amortise the kernel's serial projection / softmax phases; 32-wide heads take the three-launch attention
         import os
-        self.fused_hat = os.environ.get("FVIT_FUSED_HAT", "auto")
+        # with graphs on, a training plan's independent launches (weight re-packing, leaf gradient chains) run as
+        # parallel branches of the graph (engine_train.py)
         self.use_graphs = os.environ.get("FVIT_CUDA_GRAPH", "1") != "0" and device.type == "cuda"
-        # independent launches (weight re-packing, leaf gradient chains) as parallel branches of the launch graph
-        # (FVIT_SIDE_BRANCHES=0 off, 2 = re-packing only, 3 = backward leaf chains only: A/B switches)
-        sb = os.environ.get("FVIT_SIDE_BRANCHES", "1") if self.use_graphs else "0"
-        self.side_branches = sb in ("1", "3")
-        self.prep_branches = sb in ("1", "2")
-        # weight-gradient GEMMs as side-branch launches too (engine_train.py: _side_from / _before_write): their CTAs fill
-        # the tails of the data-gradient chain's persistent grids. FVIT_WGRAD_SIDE=0 = A/B switch. Decided at plan build: the markers are inert when side branches are off.
-        self.wgrad_side = os.environ.get("FVIT_WGRAD_SIDE", "1") == "1"
         self._graphs: dict = {}
         self._x_static = None
         self._deploy_mods: list = []
@@ -664,8 +653,9 @@ class Plan:
         Cp = h * hdp
         wq, ldq, qb_ptr, wp, ldp = self._pack_attention(nm, attn, hdp)
         scale = float(getattr(attn, "scale", hd ** -0.5))   # qk_scale or head_dim ** -0.5 (fv.py:544)
-        fused = (self._attn_kind(S, hdp) == "tile" and self.fused_hat != "0" and hdp <= 64   # (fused kernel: 32 / 64)
-                 and (self.fused_hat == "1" or hdp == 64))
+        # the fused kernel takes 64-wide (padded) heads, where the projection is long enough to amortise its serial
+        # projection / softmax phases
+        fused = self._attn_kind(S, hdp) == "tile" and hdp == 64
         if fused:
             # ONE kernel: qkv projection + softmax(q k^T * scale + bias) + P v; the qkv matrix never reaches HBM
             self._op(self.ops, "fvit_hat_attn_fwd", xin.data_ptr(), ld_in, Cc, wq.data_ptr(), ldq, qb_ptr, groups, S, h,

@@ -14,8 +14,6 @@ so no fp16 product underflows. Parameter gradients are fp32 and exact in scale.
 """
 from __future__ import annotations
 
-import os
-
 import torch
 
 from . import lib as L
@@ -252,26 +250,20 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
     # overwrites such a buffer first waits for the event behind its last side-branch reader (`wait_side`).
     def _side_from(self, first: int, *reads: int) -> None:
         """make backward launches [first, now) side-branch launches that read the reusable buffers `reads`"""
-        if not self.wgrad_side:
-            return
         for i in range(first, len(self.bwd_ops)):
             self._bwd_side_wgrad.add(i)
             self._side_reads[i] = tuple(reads)
 
-    def _side_set(self, data_parallel: bool):
-        """Launches that go to the side branch. Under a gradient all-reduce the weight-gradient GEMMs stay there too: a
-        second persistent grid does compete with NCCL's CTAs for the SMs the capped launches leave free.
-        FVIT_WGRAD_SIDE_DDP=0 keeps them on the main branch (A/B switch)."""
-        if not self.side_branches:
+    def _side_set(self):
+        """Launches that go to the side branch (graphs only). Under a gradient all-reduce the weight-gradient GEMMs stay
+        there too: a second persistent grid does compete with NCCL's CTAs for the SMs the capped launches leave free."""
+        if not self.use_graphs:
             return None
-        if data_parallel and os.environ.get("FVIT_WGRAD_SIDE_DDP", "1") != "1":
-            return self._bwd_side
         return self._bwd_side | self._bwd_side_wgrad
 
     def _before_write(self, *ptrs: int) -> None:
         """the next backward launch overwrites `ptrs`: order it behind their side-branch readers"""
-        if self.wgrad_side:
-            self.bwd_ops.append(("wait_side", tuple(ptrs), "wait_side"))
+        self.bwd_ops.append(("wait_side", tuple(ptrs), "wait_side"))
 
     def _split_k(self, m: int, n: int, k_rows: int, ntaps: int = 1) -> int:
         tiles = ((m + 127) // 128) * ((n + 127) // 128) * ntaps
@@ -348,7 +340,7 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
                 t.zero_()
             if self.drop_specs:
                 self._gen_drop_masks()   # stochastic-depth masks of this step (torch RNG, like timm's DropPath)
-            if self.prep_branches:
+            if self.use_graphs:
                 self.run_ops_branches(self.prep_ops)
             else:
                 self.run_ops(self.prep_ops, None)
@@ -385,7 +377,7 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
 
             def body():
                 self._bwd_start(None)
-                self.run_ops(self.bwd_ops, None, side=self._side_set(False))
+                self.run_ops(self.bwd_ops, None, side=self._side_set())
             self.run_captured("backward", body)
             return
         # data parallel: each bucket's all-reduce is issued the moment the launches that finish its gradients are
@@ -413,7 +405,7 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
                         self._bwd_start(None)
                     self._op_base = lo
                     try:
-                        self.run_ops(self.bwd_ops[lo:hi], None, side=self._side_set(True))
+                        self.run_ops(self.bwd_ops[lo:hi], None, side=self._side_set())
                     finally:
                         self._op_base = 0
                 if hi > lo or n == 0:   # (the list ends with a bucket point: nothing to capture after it)

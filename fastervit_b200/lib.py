@@ -10,10 +10,7 @@ from pathlib import Path
 
 import torch
 
-_PKG = Path(__file__).resolve().parent
-import os as _os
-
-LIB_PATH = Path(_os.environ["FVIT_LIB"]) if _os.environ.get("FVIT_LIB") else _PKG / "libfvit_sm100.so"   # (A/B builds)
+LIB_PATH = Path(__file__).resolve().parent / "libfvit_sm100.so"
 
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_GELU_BWD, ACT_RELU_BWD, ACT_MUL_AUX = 0, 1, 2, 3, 4, 5
 # fvit_gemm kernel-variant bits (include/fvit.h FVIT_GEMM_F_*); the activation code sits in bits 1..3

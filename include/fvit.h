@@ -149,7 +149,7 @@ enum {
   FVIT_GEMM_F_PREGRAD = 1 << 14,  /* pre_is_grad in effect (act == FVIT_ACT_GELU with out_pre16) */
   FVIT_GEMM_F_DIRECT = 1 << 15    /* row-per-thread epilogue: 16-bit outputs only, n and every leading dimension a
                                      multiple of 16 elements, outputs and aux 32-byte aligned, per-column vectors
-                                     16-byte aligned, b_ntaps <= 1 (FVIT_GEMM_DIRECT=0 turns it off) */
+                                     16-byte aligned, b_ntaps <= 1 */
 };
 #define FVIT_GEMM_F_ACT(x) ((uint32_t)(x) << FVIT_GEMM_F_ACT_SHIFT)
 /* The kernel variant fvit_gemm would launch for *args (same validation, no launch, no device access):
@@ -244,8 +244,8 @@ int fvit_attn_tc_fwd(const void* qkv, int64_t ldq, int32_t groups, int32_t S, in
  * of faster_vit.py:546): out = softmax((x Wq^T + bq)(x Wk^T + bk)^T * scale + bias)(x Wv^T + bv) per window and head
  * in ONE wgmma kernel. xn16 [groups*S, C] is the LayerNorm-ed fp16 activation (norm1 / hat_norm1 output, row stride
  * ldx), wqkv16 the head-padded packed qkv weight [3*heads*hdp, C] (fvit_cast_headpad_f16; row stride ldw), qkv_bias
- * its padded bias [3*heads*hdp] or NULL, bias the relative-position bias [heads, S, S] or NULL. S <= 128, hdp in
- * {32, 64}. out [groups*S, heads*hdp] as fvit_attn_tc_fwd. qkv_out (optional, [groups*S, 3*heads*hdp] fp16) receives
+ * its padded bias [3*heads*hdp] or NULL, bias the relative-position bias [heads, S, S] or NULL. S <= 128, hdp 64.
+ * out [groups*S, heads*hdp] as fvit_attn_tc_fwd. qkv_out (optional, [groups*S, 3*heads*hdp] fp16) receives
  * the projected q | k | v for the backward pass; when NULL the qkv matrix never exists in HBM. */
 int fvit_hat_attn_fwd(const void* xn16, int64_t ldx, int32_t C, const void* wqkv16, int64_t ldw, const float* qkv_bias,
                       int32_t groups, int32_t S, int32_t heads, int32_t hdp, const float* bias, float scale, void* out,

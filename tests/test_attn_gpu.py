@@ -203,10 +203,11 @@ def test_attn_loop_long_backward_matches_autograd(S, heads, hd, groups):
 @pytest.mark.parametrize("save_qkv", [False, True])
 def test_fused_hat_attention_matches_unfused_math(S, heads, hd, groups, C, save_qkv):
     """fvit_hat_attn_fwd (QKV projection + softmax(QK^T + bias) + PV in one wgmma kernel) against fp32 torch on
-    the same fp16 activations / head-padded weights, with q, k, v rounded to fp16 as the kernel's operand tiles are."""
+    the same fp16 activations / head-padded weights, with q, k, v rounded to fp16 as the kernel's operand tiles are.
+    Every head is zero-padded to the kernel's 64 columns, as fv's 49-wide heads are; other padded widths raise."""
     from fastervit_b200 import lib
     lib.load()
-    hdp = 32 if hd <= 32 else 64
+    hdp = 64
     g = torch.Generator(device="cuda").manual_seed(S * 131 + heads + C)
     rows = groups * S
     x = torch.randn(rows, C, device="cuda", generator=g).half()
@@ -231,3 +232,6 @@ def test_fused_hat_attention_matches_unfused_math(S, heads, hd, groups, C, save_
     assert err < 2e-3, err
     if save_qkv:
         assert ((qkv_out.float() - qkv.float()).abs().max() / qkv.float().abs().max()).item() < 1e-3
+    with pytest.raises(lib.FvitError, match="padded head dim 32"):
+        lib.call("fvit_hat_attn_fwd", x.data_ptr(), x.stride(0), C, w16.data_ptr(), w16.stride(0), qb.data_ptr(), groups,
+                 S, heads, 32, bias.data_ptr(), scale, out.data_ptr(), out.stride(0), None, 0)

@@ -68,14 +68,13 @@ def test_train_plans_keep_their_launch_lists():
 
 
 @pytest.mark.parametrize("name", ["faster_vit_0_224", "faster_vit_0_any_res"])
-def test_eval_grad_side_branch_weight_gradients_never_race_a_buffer_rewrite(name, monkeypatch):
+def test_eval_grad_side_branch_weight_gradients_never_race_a_buffer_rewrite(name):
     """the hazard walk of the train plan's side-branch weight gradients (test_product_cpu.py), on the eval-grad
     backward, whose conv-bias column sums join the side branch"""
-    monkeypatch.setenv("FVIT_WGRAD_SIDE", "1")
     _, plan = _plan(name)
-    assert plan.wgrad_side and any(o[0] == "wait_side" for o in plan.bwd_ops)
+    assert any(o[0] == "wait_side" for o in plan.bwd_ops)
     side_all = plan._bwd_side | plan._bwd_side_wgrad
-    assert plan._side_set(True) is None     # (no launch graphs on the host: every marker is inert)
+    assert plan._side_set() is None         # (no launch graphs on the host: every marker is inert)
     pure_readers = {"fvit_colsum"}          # main-branch launches that only read the activation gradient they are handed
     outstanding: dict[int, int] = {}        # buffer -> index of the side launch still reading it
     n_side_gemm = n_wgrad = 0

@@ -60,7 +60,7 @@ def test_every_attention_of_the_hd80_models_runs_on_tensor_cores(hd80):
         assert launches, desc
         names = {n for n, _, _ in launches}
         assert not names & {"fvit_attn_core_fwd", "fvit_attn_core_bwd"}, (desc, launches)
-        assert "fvit_hat_attn_fwd" not in names, desc       # the fused kernel is 32 / 64 only
+        assert "fvit_hat_attn_fwd" not in names, desc       # the fused kernel is 64 only
         assert all(d == 80 for _, _, d in launches), (desc, launches)
         if "train" in desc or "gradient" in desc:
             assert any(n.endswith("_bwd") or n.endswith("_bwd_long") for n in names), desc
