@@ -170,7 +170,12 @@ _OP_SIGS: dict[str, list] = {
     "fvit_optim_lamb_stage1": [_P, _I, _P, _P, _P, _P, _P, _P, _P, _F, _F, _F, _P, _P, _P],
     "fvit_optim_lamb_stage2": [_P, _I, _P, _P, _P, _P, _P, _I, _I, _P, _P, _F, _P],
     "fvit_optim_ema": [_P, _I, _P, _P, _F, _P],
+    # multi-scale deformable attention core (include/fvit.h "Multi-scale deformable attention"; deform.py)
+    "fvit_msda_fwd": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P],
+    "fvit_msda_bwd": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P],
 }
+# FVIT_MSDA_MAX_LEVELS of include/fvit.h
+MSDA_MAX_LEVELS = 16
 
 
 _weights_epoch = 0

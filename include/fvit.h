@@ -622,6 +622,29 @@ int fvit_optim_lamb_stage2(const int32_t* chunks, int32_t nchunks, const int64_t
 int fvit_optim_ema(const int32_t* chunks, int32_t nchunks, const int64_t* seg_ema, const int64_t* seg_src, float decay,
                    void* stream);
 
+/* ---- Multi-scale deformable attention (MSDeformAttn of the DINO and MOTRv2 transformers) ----------------
+ * Replaces the MultiScaleDeformableAttention extension's ms_deform_attn_forward / _backward (and its
+ * ms_deform_attn_core_pytorch restatement). All float tensors are fp32 and contiguous:
+ *   value [N, S, M, D], spatial_shapes [L, 2] int64 (H_l, W_l), level_start_index [L] int64,
+ *   sampling_locations [N, Lq, M, L, P, 2] (x, y in [0, 1] of the level, any value allowed),
+ *   attention_weights [N, Lq, M, L, P], out / grad_out [N, Lq, M*D].
+ * out[n, q, m*D + c] = sum_{l, p} attention_weights[n, q, m, l, p] * bilinear sample of channel c of head m of level l
+ * at h = y*H_l - 0.5, w = x*W_l - 0.5 (grid_sample bilinear, zero padding, align_corners=False): a sample contributes
+ * only if -1 < h < H_l and -1 < w < W_l, and corners outside the map read zero. Any D >= 1 and 1 <= L <=
+ * FVIT_MSDA_MAX_LEVELS. spatial_shapes and level_start_index stay on the device (nothing synchronises); a level
+ * whose rows fall outside [0, S) reads as zero rather than out of bounds. */
+#define FVIT_MSDA_MAX_LEVELS 16
+int fvit_msda_fwd(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
+                  const float* sampling_locations, const float* attention_weights, int32_t N, int32_t S, int32_t M,
+                  int32_t D, int32_t Lq, int32_t L, int32_t P, float* out, void* stream);
+/* grad_value += d out / d value (the caller zeroes it on the stream; float atomics, so the order of additions is not
+ * deterministic); grad_sampling_locations [N, Lq, M, L, P, 2] and grad_attention_weights [N, Lq, M, L, P] are written
+ * whole, deterministically. The location gradient carries the factors W_l (x) and H_l (y). */
+int fvit_msda_bwd(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
+                  const float* sampling_locations, const float* attention_weights, const float* grad_out, int32_t N,
+                  int32_t S, int32_t M, int32_t D, int32_t Lq, int32_t L, int32_t P, float* grad_value,
+                  float* grad_sampling_locations, float* grad_attention_weights, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
