@@ -155,17 +155,37 @@ __global__ void __launch_bounds__(kMsdaThreads)
   }
 }
 
-// Backward: grad_value (zeroed by the caller) gets every sample's corner weight * attn * grad_out by vector atomics;
-// grad_attn and grad_loc of each sample are reduced over the group's channels by shuffles and written by lane 0 of the
-// group, so they need no atomics and are deterministic. Every element of grad_loc and grad_attn is written.
-template <int VEC>
-__global__ void __launch_bounds__(kMsdaThreads)
-    msda_bwd_kernel(const float* __restrict__ value, const int64_t* __restrict__ shapes,
-                    const int64_t* __restrict__ starts, const float* __restrict__ loc, const float* __restrict__ attn,
-                    const float* __restrict__ grad_out, float* __restrict__ grad_value, float* __restrict__ grad_loc,
-                    float* __restrict__ grad_attn, MsdaGeom q) {
-  __shared__ int s_h[FVIT_MSDA_MAX_LEVELS], s_w[FVIT_MSDA_MAX_LEVELS], s_start[FVIT_MSDA_MAX_LEVELS];
-  load_levels(shapes, starts, q.L, q.S, s_h, s_w, s_start);
+// Where the backward puts a corner's s * grad_out * attn into grad_value. FloatSink: fp32 vector atomics, whose order
+// of additions is not deterministic. FixedSink: int64 fixed point in units of 2^-k, one round-to-nearest per
+// contribution (the fp32 product of the float path, scaled by 2^k exactly); integer addition is associative, so the
+// sums do not depend on the order of the samples.
+struct FloatSink {
+  float* base;
+  template <int VEC>
+  __device__ __forceinline__ void add(float* p, float s, const Chunk<VEC>& c) const {
+    red_add<VEC>(p, s, c);
+  }
+};
+
+struct FixedSink {
+  unsigned long long* base;
+  double scale;  // 2^k
+  template <int VEC>
+  __device__ __forceinline__ void add(unsigned long long* p, float s, const Chunk<VEC>& c) const {
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) atomicAdd(p + i, (unsigned long long)__double2ll_rn((double)(s * c.v[i]) * scale));
+  }
+};
+
+// Backward: grad_value gets every sample's corner weight * attn * grad_out through the sink; grad_attn and grad_loc of
+// each sample are reduced over the group's channels by shuffles and written by lane 0 of the group, so they need no
+// atomics and are deterministic. Every element of grad_loc and grad_attn is written.
+template <int VEC, class Sink>
+__device__ __forceinline__ void msda_bwd_body(const float* __restrict__ value, const int* s_h, const int* s_w,
+                                              const int* s_start, const float* __restrict__ loc,
+                                              const float* __restrict__ attn, const float* __restrict__ grad_out,
+                                              const Sink& sink, float* __restrict__ grad_loc,
+                                              float* __restrict__ grad_attn, const MsdaGeom& q) {
   const int G = q.G, gl = threadIdx.x & (G - 1);
   const long long grp = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / G;
   const bool live = grp < q.groups;
@@ -204,7 +224,7 @@ __global__ void __launch_bounds__(kMsdaThreads)
           const long long c = (long long)cv * VEC;
           const Chunk<VEC> go = c0 == 0 ? go0 : load_chunk<VEC>(gobase + c);
           const float* __restrict__ vc = value + vofs + c;
-          float* gv = grad_value + vofs + c;
+          auto* gv = sink.base + vofs + c;
           const Chunk<VEC> v1 = b.c1 ? load_chunk<VEC>(vc + b.row * vstride) : zero_chunk<VEC>();
           const Chunk<VEC> v2 = b.c2 ? load_chunk<VEC>(vc + (b.row + 1) * vstride) : zero_chunk<VEC>();
           const Chunk<VEC> v3 = b.c3 ? load_chunk<VEC>(vc + (b.row + W) * vstride) : zero_chunk<VEC>();
@@ -220,10 +240,10 @@ __global__ void __launch_bounds__(kMsdaThreads)
             gh = fmaf(tg.v[i], dh, gh);
             gw = fmaf(tg.v[i], dw, gw);
           }
-          if (b.c1) red_add<VEC>(gv + b.row * vstride, w1, tg);
-          if (b.c2) red_add<VEC>(gv + (b.row + 1) * vstride, w2, tg);
-          if (b.c3) red_add<VEC>(gv + (b.row + W) * vstride, w3, tg);
-          if (b.c4) red_add<VEC>(gv + (b.row + W + 1) * vstride, w4, tg);
+          if (b.c1) sink.template add<VEC>(gv + b.row * vstride, w1, tg);
+          if (b.c2) sink.template add<VEC>(gv + (b.row + 1) * vstride, w2, tg);
+          if (b.c3) sink.template add<VEC>(gv + (b.row + W) * vstride, w3, tg);
+          if (b.c4) sink.template add<VEC>(gv + (b.row + W + 1) * vstride, w4, tg);
         }
       }
       for (int o = G >> 1; o > 0; o >>= 1) {
@@ -241,6 +261,96 @@ __global__ void __launch_bounds__(kMsdaThreads)
   }
 }
 
+template <int VEC>
+__global__ void __launch_bounds__(kMsdaThreads)
+    msda_bwd_kernel(const float* __restrict__ value, const int64_t* __restrict__ shapes,
+                    const int64_t* __restrict__ starts, const float* __restrict__ loc, const float* __restrict__ attn,
+                    const float* __restrict__ grad_out, float* __restrict__ grad_value, float* __restrict__ grad_loc,
+                    float* __restrict__ grad_attn, MsdaGeom q) {
+  __shared__ int s_h[FVIT_MSDA_MAX_LEVELS], s_w[FVIT_MSDA_MAX_LEVELS], s_start[FVIT_MSDA_MAX_LEVELS];
+  load_levels(shapes, starts, q.L, q.S, s_h, s_w, s_start);
+  msda_bwd_body<VEC>(value, s_h, s_w, s_start, loc, attn, grad_out, FloatSink{grad_value}, grad_loc, grad_attn, q);
+}
+
+// ---- deterministic backward: bound pass, fixed-point accumulation, conversion ----
+
+// bound[0] |= max |attn|, bound[1] |= max |grad_out|, as the bit patterns of non-negative floats, which order like
+// their values; a NaN (sign cleared) sorts above inf, so a non-finite input leaves a pattern >= 0x7f800000. Maxima do
+// not depend on the order. bound is zeroed before the launch.
+__global__ void __launch_bounds__(kMsdaThreads)
+    msda_bound_kernel(const float* __restrict__ attn, long long na, const float* __restrict__ grad_out, long long ng,
+                      unsigned* __restrict__ bound) {
+  const long long stride = (long long)gridDim.x * blockDim.x, i0 = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  unsigned ma = 0, mg = 0;
+#pragma unroll 4
+  for (long long i = i0; i < ng; i += stride) mg = max(mg, __float_as_uint(fabsf(__ldg(grad_out + i))));
+  for (long long i = i0; i < na; i += stride) ma = max(ma, __float_as_uint(fabsf(__ldg(attn + i))));
+  ma = __reduce_max_sync(kFull, ma);
+  mg = __reduce_max_sync(kFull, mg);
+  if ((threadIdx.x & 31) == 0) {
+    atomicMax(bound, ma);
+    atomicMax(bound + 1, mg);
+  }
+}
+
+// Fixed-point exponent k of grad_value's sums (they count units of 2^-k); false if A = max |attn| or
+// G = max |grad_out| is not finite.
+//
+// Bound: an element (n, pixel, m, c) of grad_value receives at most one contribution per sample of its (n, m), since
+// a sample's four corners are distinct pixels; rows of different levels may coincide (level_start_index is not
+// checked), so that is up to ns = Lq * L * P contributions. Each is w * (a * g) in fp32 with a corner weight w <= 1,
+// |a| <= A, |g| <= G, so every partial or whole sum is at most B = ns * A * G (times (1 + 2^-24)^2 for the two fp32
+// roundings). With B < 2^e <= 2B, k = 62 - e puts B * 2^k below 2^62; rounding adds at most ns / 2 < 2^62 units
+// (ns < 2^35 for any attention_weights that fits in memory), so the sums stay below 2^63 in magnitude.
+// Error: one contribution rounds by at most 2^-(k+1) <= B * 2^-62, so an element with ne contributions is within
+// ne * B * 2^-62 <= ns^2 * A * G * 2^-62 of the exact sum of the fp32 contributions, before its conversion to fp32.
+// At DINO's 5-scale encoder (ns = 1.8 M) that is 7e-7 * A * G.
+__device__ __forceinline__ bool fixed_exponent(const unsigned* __restrict__ bound, long long ns, int* k) {
+  const unsigned ab = bound[0], gb = bound[1];
+  *k = 0;
+  if (ab >= 0x7f800000u || gb >= 0x7f800000u) return false;
+  const double B = (double)ns * (double)__uint_as_float(ab) * (double)__uint_as_float(gb);
+  if (B > 0.0) {
+    int e;
+    frexp(B, &e);  // B = f * 2^e, f in [0.5, 1)
+    *k = 62 - e;
+  }
+  return true;
+}
+
+// msda_bwd_kernel<1> with grad_value summed in int64 fixed point (acc, zeroed before the launch). One channel per
+// lane, so each 64-bit atomic instruction of a group covers consecutive addresses; with msda_bwd_kernel<4>'s float4
+// layout (four channels per lane) an instruction's addresses lie 32 bytes apart, and that variant took 2.2 to 2.4
+// times as long at the README's four workloads on an H100.
+__global__ void __launch_bounds__(kMsdaThreads)
+    msda_bwd_fixed_kernel(const float* __restrict__ value, const int64_t* __restrict__ shapes,
+                          const int64_t* __restrict__ starts, const float* __restrict__ loc,
+                          const float* __restrict__ attn, const float* __restrict__ grad_out,
+                          unsigned long long* __restrict__ acc, const unsigned* __restrict__ bound,
+                          float* __restrict__ grad_loc, float* __restrict__ grad_attn, MsdaGeom q) {
+  __shared__ int s_h[FVIT_MSDA_MAX_LEVELS], s_w[FVIT_MSDA_MAX_LEVELS], s_start[FVIT_MSDA_MAX_LEVELS];
+  load_levels(shapes, starts, q.L, q.S, s_h, s_w, s_start);
+  int k;
+  // with a non-finite bound the sums are meaningless (and harmless: unsigned adds wrap); msda_fixed_to_float_kernel
+  // writes NaN instead
+  fixed_exponent(bound, (long long)q.Lq * q.L * q.P, &k);
+  msda_bwd_body<1>(value, s_h, s_w, s_start, loc, attn, grad_out, FixedSink{acc, ldexp(1.0, k)}, grad_loc, grad_attn,
+                   q);
+}
+
+// grad_value = acc * 2^-k (one rounding to double when |acc| > 2^53, exact scaling, one rounding to fp32), or NaN
+// everywhere when the bound is not finite
+__global__ void __launch_bounds__(kMsdaThreads)
+    msda_fixed_to_float_kernel(const unsigned long long* __restrict__ acc, long long count,
+                               const unsigned* __restrict__ bound, long long ns, float* __restrict__ grad_value) {
+  int k;
+  const bool finite = fixed_exponent(bound, ns, &k);
+  const double unit = ldexp(1.0, -k);
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < count; i += stride)
+    grad_value[i] = finite ? (float)((double)(long long)acc[i] * unit) : __int_as_float(0x7fc00000);
+}
+
 // lanes per group: the channel vectors of one head rounded up to a power of two, at most a warp
 int group_lanes(int nvec) {
   int g = 1;
@@ -249,6 +359,12 @@ int group_lanes(int nvec) {
 }
 
 bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
+
+// blocks of a grid-stride pass over count elements: enough to fill an H100 (132 SMs x 8 blocks), at least one
+unsigned stream_blocks(long long count) {
+  const long long b = ceil_div64(count, kMsdaThreads);
+  return b < 1 ? 1u : b > 1056 ? 1056u : (unsigned)b;
+}
 
 int check_geom(const char* fn, int32_t N, int32_t S, int32_t M, int32_t D, int32_t Lq, int32_t L, int32_t P,
                MsdaGeom* q) {
@@ -312,4 +428,40 @@ int fvit_msda_bwd(const float* value, const int64_t* spatial_shapes, const int64
       value, spatial_shapes, level_start_index, sampling_locations, attention_weights, grad_out, grad_value,
       grad_sampling_locations, grad_attention_weights, q);
   return post_launch("msda_bwd_kernel<1>");
+}
+
+int fvit_msda_bwd_deterministic(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
+                                const float* sampling_locations, const float* attention_weights, const float* grad_out,
+                                int32_t N, int32_t S, int32_t M, int32_t D, int32_t Lq, int32_t L, int32_t P,
+                                float* grad_value, float* grad_sampling_locations, float* grad_attention_weights,
+                                int64_t* scratch, float* workspace, void* stream) {
+  MsdaGeom q;
+  if (int rc = check_geom("fvit_msda_bwd_deterministic", N, S, M, D, Lq, L, P, &q)) return rc;
+  const long long nvalue = (long long)N * S * M * D, ns = (long long)Lq * L * P;
+  if (q.groups == 0 && nvalue == 0) return 0;
+  FVIT_CHECK(value && spatial_shapes && level_start_index && sampling_locations && attention_weights && grad_out &&
+                 grad_value && grad_sampling_locations && grad_attention_weights && scratch && workspace,
+             "fvit_msda_bwd_deterministic: null pointer");
+  q.G = group_lanes(D);  // one channel per lane for any D and alignment (msda_bwd_fixed_kernel)
+  const long long blocks = ceil_div64(q.groups * q.G, kMsdaThreads);
+  FVIT_CHECK(blocks <= 0x7fffffffLL, "fvit_msda_bwd_deterministic: %lld query-heads is too many for one launch",
+             q.groups);
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned* bound = reinterpret_cast<unsigned*>(workspace);
+  unsigned long long* acc = reinterpret_cast<unsigned long long*>(scratch);
+  FVIT_CUDA(cudaMemsetAsync(bound, 0, FVIT_MSDA_DET_WORKSPACE * sizeof(float), st));
+  FVIT_CUDA(cudaMemsetAsync(acc, 0, (size_t)nvalue * sizeof(int64_t), st));
+  const long long na = q.groups * L * P, ng = q.groups * D;
+  msda_bound_kernel<<<stream_blocks(std::max(na, ng)), kMsdaThreads, 0, st>>>(attention_weights, na, grad_out, ng,
+                                                                               bound);
+  if (int rc = post_launch("msda_bound_kernel")) return rc;
+  if (q.groups > 0) {
+    msda_bwd_fixed_kernel<<<(unsigned)blocks, kMsdaThreads, 0, st>>>(
+        value, spatial_shapes, level_start_index, sampling_locations, attention_weights, grad_out, acc, bound,
+        grad_sampling_locations, grad_attention_weights, q);
+    if (int rc = post_launch("msda_bwd_fixed_kernel")) return rc;
+  }
+  if (nvalue == 0) return 0;
+  msda_fixed_to_float_kernel<<<stream_blocks(nvalue), kMsdaThreads, 0, st>>>(acc, nvalue, bound, ns, grad_value);
+  return post_launch("msda_fixed_to_float_kernel");
 }

@@ -76,6 +76,12 @@ def _empty_work(value, sampling_locations) -> bool:
     return sampling_locations.numel() == 0 or value.numel() == 0
 
 
+def deterministic_scratch_sizes(N: int, S: int, M: int, D: int) -> tuple[int, int]:
+    """(int64 elements of the fixed-point grad_value scratch, fp32 elements of the bound workspace) that the
+    deterministic backward (fvit_msda_bwd_deterministic) of a value [N, S, M, D] takes."""
+    return N * S * M * D, lib.MSDA_DET_WORKSPACE
+
+
 class MSDeformAttnFunction(Function):
     """apply(value, spatial_shapes, level_start_index, sampling_locations, attention_weights, im2col_step) -> out.
 
@@ -83,6 +89,11 @@ class MSDeformAttnFunction(Function):
     sampling_locations [N, Lq, M, L, P, 2] (x, y), attention_weights [N, Lq, M, L, P]; out [N, Lq, M*D]. float32,
     contiguous, CUDA. im2col_step is accepted and ignored: the kernel needs no column buffer, so any batch size works.
     The level geometry is read on the device; levels whose rows do not fit in S read as zero.
+
+    The backward is deterministic under torch.use_deterministic_algorithms(True): grad_value is then summed in int64
+    fixed point (fvit_msda_bwd_deterministic, a scratch of twice grad_value's size) instead of by float atomics, and is
+    NaN throughout if attention_weights or grad_output holds an inf or NaN. The other two gradients are deterministic
+    either way.
     """
 
     @staticmethod
@@ -111,15 +122,26 @@ class MSDeformAttnFunction(Function):
         grad_output = grad_output.contiguous()
         if grad_output.dtype != torch.float32:
             grad_output = grad_output.float()
-        grad_value = torch.zeros_like(value)
-        if _empty_work(value, locs):
+        empty = _empty_work(value, locs)
+        # under torch.use_deterministic_algorithms (warn_only too) grad_value is summed in fixed point, which writes
+        # all of it; the default backward adds into zeros with float atomics
+        deterministic = torch.are_deterministic_algorithms_enabled() and not empty
+        grad_value = torch.empty_like(value) if deterministic else torch.zeros_like(value)
+        if empty:
             return grad_value, None, None, torch.zeros_like(locs), torch.zeros_like(weights), None
         grad_locs = torch.empty_like(locs)
         grad_weights = torch.empty_like(weights)
+        args = (value.data_ptr(), shapes.data_ptr(), starts.data_ptr(), locs.data_ptr(), weights.data_ptr(),
+                grad_output.data_ptr(), N, S, M, D, Lq, L, P, grad_value.data_ptr(), grad_locs.data_ptr(),
+                grad_weights.data_ptr())
         with torch.cuda.device(value.device):
-            lib.call("fvit_msda_bwd", value.data_ptr(), shapes.data_ptr(), starts.data_ptr(), locs.data_ptr(),
-                     weights.data_ptr(), grad_output.data_ptr(), N, S, M, D, Lq, L, P, grad_value.data_ptr(),
-                     grad_locs.data_ptr(), grad_weights.data_ptr())
+            if deterministic:
+                n_scratch, n_workspace = deterministic_scratch_sizes(N, S, M, D)
+                scratch = torch.empty(n_scratch, dtype=torch.int64, device=value.device)
+                workspace = torch.empty(n_workspace, dtype=torch.float32, device=value.device)
+                lib.call("fvit_msda_bwd_deterministic", *args, scratch.data_ptr(), workspace.data_ptr())
+            else:
+                lib.call("fvit_msda_bwd", *args)
         return grad_value, None, None, grad_locs, grad_weights, None
 
 

@@ -173,9 +173,11 @@ _OP_SIGS: dict[str, list] = {
     # multi-scale deformable attention core (include/fvit.h "Multi-scale deformable attention"; deform.py)
     "fvit_msda_fwd": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P],
     "fvit_msda_bwd": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P],
+    "fvit_msda_bwd_deterministic": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P],
 }
-# FVIT_MSDA_MAX_LEVELS of include/fvit.h
+# FVIT_MSDA_MAX_LEVELS and FVIT_MSDA_DET_WORKSPACE (fp32 elements) of include/fvit.h
 MSDA_MAX_LEVELS = 16
+MSDA_DET_WORKSPACE = 2
 
 
 _weights_epoch = 0

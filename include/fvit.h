@@ -644,6 +644,25 @@ int fvit_msda_bwd(const float* value, const int64_t* spatial_shapes, const int64
                   const float* sampling_locations, const float* attention_weights, const float* grad_out, int32_t N,
                   int32_t S, int32_t M, int32_t D, int32_t Lq, int32_t L, int32_t P, float* grad_value,
                   float* grad_sampling_locations, float* grad_attention_weights, void* stream);
+/* fvit_msda_bwd with a grad_value that is bitwise independent of the order in which samples are processed (for
+ * torch.use_deterministic_algorithms). grad_value is written whole (the caller does not zero it); the location and
+ * weight gradients come from fvit_msda_bwd's code with one channel per lane (its layout for D % 4 != 0), equal to its
+ * up to fp32 rounding and deterministic. Two memsets and three kernels on the stream, no host synchronisation:
+ *   - A = max |attention_weights| and G = max |grad_out| are reduced on the device into workspace
+ *     (FVIT_MSDA_DET_WORKSPACE floats);
+ *   - every contribution w * (a * g) (corner weight w <= 1, the fp32 product of fvit_msda_bwd) is scaled by 2^k and
+ *     rounded once to an integer, and summed with 64-bit integer atomics into scratch (N*S*M*D int64, value's layout),
+ *     where 2^k is the largest power of two with Lq*L*P * A * G * 2^k < 2^62: no sum can overflow, and an element
+ *     summing ne contributions is within ne * Lq*L*P * A * G * 2^-62 of the exact sum of those fp32 contributions;
+ *   - grad_value = scratch * 2^-k, rounded to fp32.
+ * If A or G is not finite (inf or NaN in attention_weights or grad_out), every element of grad_value is NaN.
+ * The library zeroes scratch and workspace itself; their contents on entry are ignored and undefined on return. */
+#define FVIT_MSDA_DET_WORKSPACE 2
+int fvit_msda_bwd_deterministic(const float* value, const int64_t* spatial_shapes, const int64_t* level_start_index,
+                                const float* sampling_locations, const float* attention_weights, const float* grad_out,
+                                int32_t N, int32_t S, int32_t M, int32_t D, int32_t Lq, int32_t L, int32_t P,
+                                float* grad_value, float* grad_sampling_locations, float* grad_attention_weights,
+                                int64_t* scratch, float* workspace, void* stream);
 
 #ifdef __cplusplus
 }
