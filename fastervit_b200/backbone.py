@@ -59,6 +59,11 @@ class FasterViTBackbone(nn.Module):
         self.body.enable_input_grad(enabled)
         return self
 
+    def set_train_forwards_in_flight(self, n: int = 1):
+        """train-mode forwards that may await their backward at once (FasterViT.set_train_forwards_in_flight)"""
+        self.body.set_train_forwards_in_flight(n)
+        return self
+
     def forward_raw(self, x: torch.Tensor) -> tuple:
         """fastervit.py:816-827: tuple of the normalised level outputs, NCHW. Under .train() (detector fine-tuning,
         dino/backbone.py:158-160) the body runs its training launch list up to the highest requested level, every

@@ -1029,24 +1029,56 @@ class Plan:
                      **self._op_desc(op)) for i, op in enumerate(self.ops)]
 
 
+def forwards_in_flight(model) -> int:
+    """how many train-mode forwards of one input key may await their backward at once (set_train_forwards_in_flight)"""
+    return getattr(model, "_train_forwards_in_flight", 1)
+
+
 class Engine:
     """Per-model cache of plans keyed by input signature; owns packed weights and workspaces."""
 
     def __init__(self, model):
         self.model = model
-        self.plans: dict = {}     # in least-recently-used-first order
+        self.plans: dict = {}     # in least-recently-used-first order; a train key maps to the first of its instances
+        self.pools: dict = {}     # train key -> its TrainPlan instances, each holding the activations of one forward
         self._prepped: dict = {}
         self._ptr_sig: tuple | None = None
+        self._fwd_seq = 0         # train forwards handed an instance so far (the age of an instance's last forward)
 
     def trim_plans(self) -> None:
-        """Keep at most model.plan_cache_size plans (None or absent: no bound), dropping the least recently used. A
-        dropped plan's device memory goes once nothing holds it: an autograd node of a forward that has not run its
+        """Keep at most model.plan_cache_size plans (None or absent: no bound), dropping the least recently used; a
+        train key's instances go together. Pools above the model's forwards-in-flight bound lose their last instances.
+        A dropped plan's device memory goes once nothing holds it: an autograd node of a forward that has not run its
         backward yet keeps its plan until then. Its `_prepped` entry goes with it (keyed by id(), which a new plan may
         reuse: a stale entry would skip that plan's weight packing)."""
         cap = getattr(self.model, "plan_cache_size", None)
         while cap is not None and len(self.plans) > cap:
-            plan = self.plans.pop(next(iter(self.plans)))
+            key = next(iter(self.plans))
+            plan = self.plans.pop(key)
             self._prepped.pop(id(plan), None)
+            self.pools.pop(key, None)
+        n = forwards_in_flight(self.model)
+        for pool in self.pools.values():
+            del pool[n:]
+
+    def _train_instance(self, key, x: torch.Tensor, spec: dict | None) -> Plan:
+        """The instance of a train key's pool the next forward runs on: one that no autograd node holds (TrainPlan.
+        in_flight), else a new one while the pool is smaller than the model's forwards-in-flight bound, else the one
+        with the oldest forward, whose node's backward then raises the stale-forward error."""
+        pool = self.pools[key]
+        plan = next((p for p in pool if not p.in_flight()), None)
+        if plan is None and len(pool) < forwards_in_flight(self.model):
+            from .engine_train import TrainPlan
+            with torch.cuda.device(x.device):
+                plan = TrainPlan(self.model, x.shape[0], x.shape[2], x.shape[3], x.device, spec=spec)
+            plan._norm_sig = pool[0]._norm_sig
+            plan.adopt_pivots(pool[0])
+            pool.append(plan)
+        if plan is None:
+            plan = min(pool, key=lambda p: p.fwd_seq)
+        self._fwd_seq += 1
+        plan.fwd_seq = self._fwd_seq
+        return plan
 
     def _check_weights(self) -> tuple:
         """The kernels read parameters / buffers through raw pointers as dense row-major fp32 (int64 for the
@@ -1084,6 +1116,7 @@ class Engine:
             # parameters were re-allocated (.to(), .data = ..., load_state_dict(assign=True)): every cached plan
             # holds dangling pointers
             self.plans.clear()
+            self.pools.clear()
             self._prepped.clear()
             self._ptr_sig = sig
         key = (tuple(x.shape), training, x.device.index)
@@ -1098,10 +1131,11 @@ class Engine:
         plan = self.plans.pop(key, None)
         if plan is not None and getattr(plan, "_norm_sig", ()) != norm_sig:
             self._prepped.pop(id(plan), None)
+            self.pools.pop(key, None)
             plan = None
         if plan is not None:
             self.plans[key] = plan     # most recently used last
-            return plan
+            return self._train_instance(key, x, spec) if key in self.pools else plan
         if getattr(self.model, "carriers_from_input", False) and spec is not None and spec.get("eval"):
             raise L.FvitError("the detection backbone has no eval-mode gradients: train it under .train(), or run eval "
                               "under torch.no_grad()")
@@ -1113,6 +1147,11 @@ class Engine:
                 plan = Plan(self.model, x.shape[0], x.shape[2], x.shape[3], training, x.device)
         plan._norm_sig = norm_sig
         self.plans[key] = plan
+        if training and not (spec is not None and spec.get("eval")):
+            # train plans: a pool of instances (the eval-grad plans recompute in their backward and stay one per key)
+            self.pools[key] = [plan]
+            self._fwd_seq += 1
+            plan.fwd_seq = self._fwd_seq
         self.trim_plans()
         return plan
 

@@ -14,6 +14,8 @@ so no fp16 product underflows. Parameter gradients are fp32 and exact in scale.
 """
 from __future__ import annotations
 
+import weakref
+
 import torch
 
 from . import lib as L
@@ -329,6 +331,30 @@ class TrainPlan(Plan, ConvPartEmitters, TokenLevelEmitters):
     # forward / backward emitters: the ConvPartEmitters / TokenLevelEmitters mixins (engine_train_conv.py, engine_train_levels.py)
 
     # ------------------------------------------------------------------------------ execution
+    def claim(self) -> "_Claim":
+        """Mark this instance in flight (engine.Engine._train_instance then hands the next forward another one): its
+        saved activations belong to the autograd node that keeps the returned token, until release(token) after that
+        node's backward, or until the node, and the token with it, is freed without one."""
+        token = _Claim()
+        self._claim = weakref.ref(token)
+        return token
+
+    def release(self, token: "_Claim") -> None:
+        if self.in_flight() and self._claim() is token:
+            self._claim = None
+
+    def in_flight(self) -> bool:
+        ref = getattr(self, "_claim", None)
+        return ref is not None and ref() is not None
+
+    def adopt_pivots(self, first: "TrainPlan") -> None:
+        """Centre this instance's BatchNorm sums on the pivots of its pool's first instance (engine_train_conv.
+        _bn_col_shift: the running means when that one was built), so that a forward of one input key rounds the same
+        way whichever instance it runs on."""
+        for name, t in first.bufs.named.items():
+            if name.endswith(".pivot"):
+                self.bufs.named[name].copy_(t)
+
     def run_forward(self, x: torch.Tensor) -> torch.Tensor:
         # saved activations / batch statistics / drop masks live in this plan's persistent buffers: a new forward
         # invalidates the state an earlier, not yet differentiated forward left behind (checked in backward)
@@ -554,28 +580,42 @@ def allreduce_mean_(flat: torch.Tensor, group=None) -> torch.Tensor:
     return flat
 
 
+class _Claim:
+    """the token by which an autograd node holds its train plan instance (TrainPlan.claim)"""
+    __slots__ = ("__weakref__",)
+
+
+def _check_fresh(ctx, plan: TrainPlan, what: str) -> None:
+    if ctx.generation != plan.fwd_generation:
+        raise L.FvitError(
+            f"backward of a stale forward: another train-mode forward of the same {what} ran in between and overwrote "
+            "the saved activations of this one. Call backward before the next forward, or let several forwards await "
+            "their backward with model.set_train_forwards_in_flight(n) (multi-view losses, clips of frames; each "
+            "costs one more set of activations on the device)")
+
+
 class _FasterViTFunction(torch.autograd.Function):
     """One autograd node for the whole network: forward runs the train plan, backward runs the backward
-    plan and hands out views of the flat gradient buffer (one per nn.Parameter, in .parameters() order)."""
+    plan and hands out views of the flat gradient buffer (one per nn.Parameter, in .parameters() order).
+    The node holds its plan instance (TrainPlan.claim) until its backward has run."""
 
     @staticmethod
     def forward(ctx, plan: TrainPlan, x: torch.Tensor, *params):
         ctx.plan = plan
         logits = plan.run_forward(x)
         ctx.generation = plan.fwd_generation
+        ctx.claim = plan.claim()
         return logits.clone()
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, dlogits):
         plan: TrainPlan = ctx.plan
-        if ctx.generation != plan.fwd_generation:
-            raise L.FvitError(
-                "backward of a stale forward: another train-mode forward of the same input shape ran in between and "
-                "overwrote the saved activations of this one (one autograd node per step: call backward before the "
-                "next forward, or use different plans / model copies for multi-view losses)")
+        _check_fresh(ctx, plan, "input shape")
         plan.run_backward(dlogits.contiguous().float())
-        return (None, _train_dx(ctx, plan), *plan.grad_views())
+        res = (None, _train_dx(ctx, plan), *plan.grad_views())
+        plan.release(ctx.claim)
+        return res
 
 
 class _DenseFunction(torch.autograd.Function):
@@ -588,18 +628,18 @@ class _DenseFunction(torch.autograd.Function):
         ctx.plan = plan
         plan.run_forward(x)
         ctx.generation = plan.fwd_generation
+        ctx.claim = plan.claim()
         return tuple(o.clone() for o in plan.outputs)
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, *grads):
         plan: TrainPlan = ctx.plan
-        if ctx.generation != plan.fwd_generation:
-            raise L.FvitError(
-                "backward of a stale forward: another train-mode forward of the same input shape and outputs ran in "
-                "between and overwrote the saved activations of this one (call backward before the next forward)")
+        _check_fresh(ctx, plan, "input shape and outputs")
         plan.run_backward([None if g is None else g.contiguous().float() for g in grads])
-        return (None, _train_dx(ctx, plan), *plan.grad_views_on_path())
+        res = (None, _train_dx(ctx, plan), *plan.grad_views_on_path())
+        plan.release(ctx.claim)
+        return res
 
 
 def _train_dx(ctx, plan: TrainPlan):

@@ -10,6 +10,7 @@ hot path as hand-written CUDA kernels. There is no PyTorch/CPU fallback — CPU 
 from __future__ import annotations
 
 import math
+import numbers
 from typing import Sequence
 
 import torch
@@ -253,6 +254,7 @@ class FasterViT(nn.Module):
         self._engine = None
         self._grad_allreduce = None
         self._train_input_grad = False
+        self._train_forwards_in_flight = 1
 
     # fv.py:930-943: Linear trunc_normal(.02)/zero bias, norms to identity, convs keep torch default
     def _init_weights(self, m):
@@ -299,6 +301,25 @@ class FasterViT(nn.Module):
         input raises, as it always did: the plan for it is a second one per input shape, and a caller that merely forgot
         to detach should hear about it. Eval mode needs no switch."""
         self._train_input_grad = bool(enabled)
+        return self
+
+    def set_train_forwards_in_flight(self, n: int = 1):
+        """Let up to n train-mode forwards of the same input shape (and outputs) await their backward at once: losses
+        over several views or crops through one model, the frames of a clip summed into one backward. Each such forward
+        keeps its own set of saved activations, one train plan's device memory, until its backward has run or its
+        outputs are freed; the sets are built as they are first needed and reused from step to step. A forward beyond n
+        overwrites the oldest one, whose backward then raises. Forwards under torch.no_grad() (checkpointed segments)
+        hold no set. Default 1: a second forward before the first one's backward raises there, so a forgotten
+        backward() is reported rather than paid for in memory. Under enable_grad_allreduce() each forward's backward
+        all-reduces its own gradients (the mean of a sum is the sum of the means): one all-reduce per forward, and the
+        first backward of every new set times the all-reduce once, a collective that all ranks reach in the same
+        order."""
+        from .lib import FvitError
+        if isinstance(n, bool) or not isinstance(n, numbers.Integral) or n < 1:
+            raise FvitError(f"set_train_forwards_in_flight takes an integer n >= 1, got {n!r}")
+        self._train_forwards_in_flight = int(n)
+        if self._engine is not None:
+            self._engine.trim_plans()
         return self
 
     def switch_to_deploy(self):
