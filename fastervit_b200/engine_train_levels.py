@@ -278,7 +278,7 @@ def _attn_fwd_train(self, nm: str, attn, gamma, rows: int, groups: int, S: int, 
                col_shift=P(attn.proj.bias), col_scale2=P(ls), row_scale=rs, out_pre16=P(u16),
                ld_pre16=n if ls is not None else 0, resid=stream_buf, ld_resid=n, out_f32=stream_buf, ld_o32=n,
                flops=2.0 * rows * n * Cc)
-    return dict(rs=rs, attn=attn, wq=wq, ldq=ldq, wp=wp, ldp=ldp, hd=hd, hdp=hdp, Cp=Cp, use_tc=use_tc, kind=kind, lse=lse,
+    return dict(nm=nm, rs=rs, attn=attn, wq=wq, ldq=ldq, wp=wp, ldp=ldp, hd=hd, hdp=hdp, Cp=Cp, use_tc=use_tc, kind=kind, lse=lse,
                 scale=scale, S=S, groups=groups, rows=rows, qkv=qkv, ao=ao, y16=y16, bias=bias, u16=u16)
 
 
@@ -600,7 +600,15 @@ def _emit_attn_core_bwd(self, at: dict, dao, dqkv, groups: int, S: int, want_dbi
                  at["lse"].data_ptr(), groups, S, h, hdp, at["bias"]["out"].data_ptr(), at["scale"], dqkv.data_ptr(), 3 * Cp,
                  dbias, scr.data_ptr(), Cp)
     else:
-        self._op(ops, _attn_bwd_entry(S, hdp, at["use_tc"]), at["qkv"].data_ptr(), 3 * Cp, dao.data_ptr(), Cp, groups, S, h, hd,
+        entry = _attn_bwd_entry(S, hdp, at["use_tc"])
+        if entry == "fvit_attn_core_bwd" and _simt_bwd_smem(S, hd) > 227 * 1024:
+            # refused here, while the plan is built, rather than by the kernel in the middle of the first backward
+            level = at["nm"].split(".")[0][1:]
+            raise L.FvitError(f"level {level} ({at['nm']}): the attention backward of {S}-token windows with {hd}-wide "
+                              f"heads runs on fvit_attn_core_bwd, which holds a whole window in shared memory and needs "
+                              f"{_simt_bwd_smem(S, hd) / 1024:.0f} KiB of the 227 KiB an SM has; this model trains only "
+                              f"with smaller windows (or head widths the tensor-core kernels take)")
+        self._op(ops, entry, at["qkv"].data_ptr(), 3 * Cp, dao.data_ptr(), Cp, groups, S, h, hd,
                  hdp, at["bias"]["out"].data_ptr(), at["scale"], dqkv.data_ptr(), 3 * Cp, dbias)
     self.bwd_flops[len(ops) - 1] = 10.0 * groups * h * S * S * hd
 
@@ -613,6 +621,12 @@ def _attn_bwd_entry(S: int, hdp: int, use_tc: bool) -> str:
         if 1024 + (2 if hdp == 32 else 1) * 4 * 128 * hdp * 2 + 2 * 128 * 128 * 2 + 128 * 132 * 4 + ss + 128 <= 227 * 1024:
             return "fvit_attn_tc_bwd"
     return "fvit_attn_core_bwd"
+
+
+def _simt_bwd_smem(S: int, hd: int) -> int:
+    """shared memory of fvit_attn_core_bwd (train_sm100.cu): q, k, v, dO rows of hd + 1 floats, the [S, S + 1] P / dS
+    matrix and one row vector, all for one whole window"""
+    return (4 * S * (hd + 1) + S * (S + 1) + S) * 4
 
 
 def _posemb_bwd(self, pe: dict) -> None:

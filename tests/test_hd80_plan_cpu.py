@@ -8,6 +8,7 @@ import torch
 import fastervit_b200 as F
 from fastervit_b200 import lib as L
 
+import _attn_geometry
 import _gemm_variants as V
 from test_gemm_variants_cpu import plan_gemms, plans as existing_plans, signature
 
@@ -15,21 +16,12 @@ from test_gemm_variants_cpu import plan_gemms, plans as existing_plans, signatur
 HD80 = dict(dim=80, in_dim=16, num_heads=[1, 2, 4, 8], depths=[1, 1, 2, 2], layer_scale=1e-5)
 AR80 = dict(HD80, resolution=[384, 576], window_size=[7, 7, 12, 6], ct_size=2)
 
-# argument positions of (S, padded head dim) per attention entry point (include/fvit.h)
-_ATTN = {"fvit_attn_tc_fwd": (3, 5), "fvit_attn_loop_fwd": (3, 5), "fvit_hat_attn_fwd": (7, 9),
-         "fvit_attn_tc_bwd": (5, 8), "fvit_attn_loop_bwd_long": (8, 10),
-         "fvit_attn_core_fwd": (3, 5), "fvit_attn_core_bwd": (5, 8)}
-
 
 def attention_launches(plan):
     """(entry point, S, padded head dim) of every attention-core launch in the plan's launch lists (for the SIMT
     forward the last field is the unpadded head dim, its only head-width argument)"""
-    for lst in (v for v in vars(plan).values() if isinstance(v, list)):
-        for op in lst:
-            if isinstance(op, tuple) and len(op) == 3 and isinstance(op[2], str) and op[2] in _ATTN:
-                args = op[1][2] if op[0] == "unless_deploy" else op[1]
-                s, d = _ATTN[op[2]]
-                yield op[2], args[s], args[d]
+    for a in _attn_geometry.attention_launches(plan):
+        yield a.entry, a.S, a.hdp
 
 
 def _plans(name, kw, res, drop_path_rate=0.1):
